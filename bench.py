@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Flagship benchmark: MoE-layer training step (fwd + bwd + SGD) throughput, whole job, device-timed.
 
-Config (BASELINE.json #2, weak scaling): helloworld model, top-2, 8 global experts (8/N per GPU), bf16,
+Config (weak scaling): helloworld model, top-2, 8 global experts (8/N per GPU), bf16,
 model_dim 4096, hidden 14336, 16 x 512 = 8192 tokens per GPU, capacity_factor 1.0, synthetic data, random init.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
@@ -40,7 +40,29 @@ def parse():
     ap.add_argument('--fp8', action='store_true')                  # ours only: e4m3 forward + data-gradient GEMMs
     ap.add_argument('--graph', default='auto', choices=['auto', 'off'])     # ours, 1 GPU: replay the whole step as one CUDA graph
     ap.add_argument('--fp8_mode', default='row', choices=['row', 'mx'])   # row scales (fused engine) or MX 32-element block scales
+    # write what the last timed step returned to its caller (loss, input and parameter gradients) as DIR/<name>.npy
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR')
     return ap.parse_args()
+
+
+DUMP_MAX_ELEMS = 2 * 1024 * 1024      # per array: 8 MB of float32; larger tensors are sampled at fixed, seeded positions
+
+
+def dump_outputs(path, loss, x, model):
+    """What the step handed to its caller: the loss, the gradient of the input and the gradients of the parameters."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    arrays = {'loss': loss.detach().reshape(1), 'input_grad': x.grad}
+    for name, p in model.named_parameters():
+        if p.grad is not None:
+            arrays['param_grad.' + name] = p.grad
+    for i, (name, t) in enumerate(arrays.items()):
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(1234 + i).choice(flat.numel(), DUMP_MAX_ELEMS, replace=False))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        np.save(os.path.join(path, name + '.npy'), flat.float().cpu().numpy())
 
 
 def main():
@@ -48,7 +70,7 @@ def main():
     if args.impl == 'reference':
         ref = os.path.join(ROOT, 'baseline', '_ref')
         if not os.path.isdir(os.path.join(ref, 'tutel')):
-            print(json.dumps({'impl': 'reference', 'unavailable': 'baseline/_ref is not installed (pip install --target baseline/_ref /root/reference)'}))
+            print(json.dumps({'impl': 'reference', 'unavailable': 'baseline/_ref is not installed (pip install --target baseline/_ref <reference checkout>)'}))
             return
         sys.path.insert(0, ref)
         try:
@@ -94,6 +116,10 @@ def main():
 
     model = Model().to(device)
     optimizer = torch.optim.SGD(model.parameters(), lr=1e-5)
+    # --dump-outputs: the number of warm-up steps depends on how fast the step time settles, so the parameters are put
+    # back to their initial values right before the timed steps - what the last timed step computes then depends on the
+    # arguments alone
+    initial_params = [p.detach().clone() for p in model.parameters()] if args.dump_outputs else None
     shared = [p for p in model.parameters() if not hasattr(p, 'skip_allreduce') and p.requires_grad]
 
     torch.manual_seed(rank)
@@ -192,6 +218,14 @@ def main():
         launches0 = backend.launch_count()
     # (both arms) no cyclic-garbage collection inside a timed region: with tightly coupled ranks one collector pause on any
     # rank stalls every rank
+    if initial_params is not None:
+        with torch.no_grad():
+            for p, p0 in zip(model.parameters(), initial_params):
+                p.copy_(p0)
+        if args.impl == 'ours':
+            from tutel_b200.ops import gemm as gemm_ops
+            gemm_ops.invalidate_fp8_cache()
+        sync()
     gc.collect()
     gc.disable()
     t_wall0 = time.time()
@@ -204,6 +238,8 @@ def main():
     t_wall1 = time.time()
     gc.enable()
     ms = maxreduce(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, x_dev, model)
     launches = (backend.launch_count() - launches0) if args.impl == 'ours' else None
     clocks = None
     if sampler is not None:
@@ -289,8 +325,9 @@ def main():
                    'global_batch': world * BATCH, 'seq_len': TOKENS, 'tokens_per_gpu': BATCH * TOKENS,
                    'parallelism': 'ep%d (%d local experts/GPU)' % (world, local_experts), 'capacity_factor': 1.0,
                    'step': 'zero_grad + fwd + nll_loss + bwd (incl. input gradient) + gate-grad all-reduce + SGD',
-                   'l2': 'working set (weights %.1f GB + activations) exceeds the 126 MB L2; no explicit flush' % (
-                       local_experts * 2 * args.model_dim * args.hidden * 2 / 1e9),
+                   'l2': 'working set (weights %.1f GB + activations) exceeds the %.0f MB L2; no explicit flush' % (
+                       local_experts * 2 * args.model_dim * args.hidden * 2 / 1e9,
+                       torch.cuda.get_device_properties(device).L2_cache_size / 1e6),
                    'a2a_ffn_overlap_degree': args.overlap, **graph_info},
         'tflops_per_gpu': flops / (ms / args.steps * 1e-3) * 1e-12,
         'clocks': clocks, 'e2e': e2e, 'gpu_launches': launches, 'loss': float(loss.item()), 'first_step_loss': first_loss,

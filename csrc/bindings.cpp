@@ -8,7 +8,7 @@
 
 #include "cpu_kernels.h"
 #include "gemm_mx.h"
-#include "gemm_sm100.h"
+#include "gemm_sm90.h"
 #include "jit_nvrtc.h"
 #include "moe_kernels.h"
 #include "p2p_kernels.h"
@@ -131,7 +131,7 @@ void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn,
   }
   if (act != 0) p.act = static_cast<int>(act);
   const char* why = nullptr;
-  cudaError_t e = tb::gemm_sm100_launch(p, cur_stream(), &why);
+  cudaError_t e = tb::gemm_sm90_launch(p, cur_stream(), &why);
   TORCH_CHECK(e == cudaSuccess, "tutel_b200.gemm launch failed: ", why ? why : cudaGetErrorString(e));
 }
 
@@ -542,7 +542,7 @@ void gemm_glu(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::
     p.row_counts = row_counts->data_ptr<int>();
   }
   const char* why = nullptr;
-  cudaError_t e = tb::gemm_sm100_launch(p, cur_stream(), &why);
+  cudaError_t e = tb::gemm_sm90_launch(p, cur_stream(), &why);
   TORCH_CHECK(e == cudaSuccess, "tutel_b200.gemm_glu launch failed: ", why ? why : cudaGetErrorString(e));
 }
 
@@ -603,7 +603,7 @@ void register_cpu_bindings(pybind11::module& m);   // cpu_kernels.cpp
 void register_jit_bindings(pybind11::module& m);   // jit_nvrtc.cpp
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "tutel_b200 native runtime: sm_100a tcgen05 grouped GEMM, routing/dispatch kernels, symmetric heap, "
+  m.doc() = "tutel_b200 native runtime: sm_90a wgmma grouped GEMM, routing/dispatch kernels, symmetric heap, "
             "P2P collectives, NVRTC JIT";
   m.def("gemm", &gemm);
   m.def("gemm_ex", &gemm_ex);

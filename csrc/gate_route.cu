@@ -1,4 +1,4 @@
-// Fused gating + routing for sm_100a: TWO launches take the gate logits to everything the dispatch needs.
+// Fused gating + routing for sm_90a: TWO launches take the gate logits to everything the dispatch needs.
 //
 // The reference spends ~15 PyTorch kernels on softmax / top-k / one-hot masks / GShard loss / gate normalisation
 // (tutel/impls/moe_layer.py:283-305, tutel/impls/losses.py:12-19) and k cumsum passes + k compares on the locations

@@ -1,26 +1,20 @@
-// MX block-scaled fp8 GEMM for sm_100a:  D[g] = A[g] * B[g]^T  with e4m3 operands that carry one UE8M0 scale per
-// 32 consecutive K elements (OCP MX), multiplied INSIDE the tensor core:
-//     tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale  [d_tmem], a_desc, b_desc, idesc, [sfa_tmem], [sfb_tmem], p
+// MX block-scaled fp8 GEMM for sm_90a:  D[g] = A[g] * B[g]^T  with e4m3 operands that carry one UE8M0 scale per
+// 32 consecutive K elements (OCP MX).  Hopper's tensor cores know no block scales, so every 32-element K block is one
+//     wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3
+// into a scratch fragment that the issuing threads then fold into the fp32 accumulator with the block's two scales:
+//     acc[m, n] += scratch[m, n] * 2^(sfa[m, kb] - 127) * 2^(sfb[n, kb] - 127).
 // The reference has no reduced-precision expert path at all (tutel/experts/ffn.py runs torch.matmul in the model
-// dtype); the row-scaled e4m3 path of gemm_sm100.cu is what the fused engine uses, this kernel is the finer-grained
+// dtype); the row-scaled e4m3 path of gemm_sm90.cu is what the fused engine uses, this kernel is the finer-grained
 // alternative (outliers only cost the 32 elements next to them their precision, not the whole row).
 //
-// Layout of one CTA (192 threads; K walked in 128-element = 128-byte steps):
-//   warp 0      TMA producer: A tile [128 x 128 B] and B tile (SWIZZLE_128B) plus the scale atoms (512 B per 128 rows)
-//               per stage, all completing on the stage's "full" mbarrier
-//   warp 1      one elected lane: tcgen05.cp (scales smem -> TMEM; 32 lanes x 4 columns per 128 rows, replicated over
-//               the four lane quarters) followed by four K=32 MMAs whose descriptors select byte 0..3 of those columns;
-//               tcgen05.commit releases the stage.  tcgen05.cp and tcgen05.mma of one thread execute in issue order,
-//               so the scale columns are single-buffered.
-//   warps 2-5   epilogue: tcgen05.ld (thread = accumulator row) -> bias / ReLU in fp32 -> packed bf16 in registers ->
-//               accumulator released -> (ReLU-backward mask) -> 16-byte global stores, overlapping the next tile
-// Persistent.  Tensor memory holds ONE accumulator (BN columns) plus 4 + BN / 32 scale columns: a second 256-column
-// accumulator would not leave room for the scales, hence the register hand-off instead of double buffering.
-// Variants:  CG = 2 (default for M > 128, N % 256 == 0): a CTA pair owns a 256 x 256 tile, cta_group::2 MMAs; each CTA
-//            stages its 128 A rows, half of the B tile, its A scales and ALL B scales (6 stages, 207 KB);
-//            CG = 1, BN = 256: 4 stages (198 KB), one CTA per SM;  CG = 1, BN = 128: 3 stages (100 KB), two CTAs per SM.
-// Measured on a B200 (bench/mx_check.py, profiles/r2/mx): 2.77-3.10 PFLOP/s (CG = 2) on 8192 x {4096, 14336} x {4096,
-// 14336}, row-scaled fp8 kernel of gemm_sm100.cu 2.58-3.00, bf16 1.60-1.70.
+// Layout of one CTA (384 threads, 128 x 128 tiles; K walked in 128-element = 128-byte steps, 6 stages):
+//   warp 0        TMA producer: A and B tiles [128 x 128 B] (SWIZZLE_128B) plus the two scale atoms (512 B per 128 rows)
+//                 per stage, all completing on the stage's "full" mbarrier
+//   warps 4..11   two consumer warpgroups, 64 rows of the tile each: per stage the scale words of the thread's 2 rows
+//                 and 32 columns are read once, then four times {wgmma k32 -> scratch, scale-and-add}; while one
+//                 warpgroup scales, the other one's wgmma keeps the tensor cores busy.  Epilogue straight from the
+//                 accumulator fragment: bias / ReLU / ReLU-backward mask in fp32, packed bf16 pairs to global memory.
+// Persistent: CTA b works on tiles b, b + grid, ...; the producer runs ahead into the next tile during the epilogue.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -31,6 +25,7 @@
 #include <mutex>
 
 #include "gemm_mx.h"
+#include "gemm_sm90.h"
 #include "moe_kernels.h"
 #include "ptx.cuh"
 
@@ -38,25 +33,20 @@ namespace tb {
 namespace {
 
 constexpr int kBM = 128;
+constexpr int kBN = 128;
 constexpr int kBK = 128;                 // e4m3 elements = bytes per K step (one 128-byte swizzle row)
 constexpr int kSfAtomBytes = 512;        // scales of 128 rows x 128 K elements
-constexpr int kMxThreads = 192;
+constexpr int kMxThreads = 384;          // producer warpgroup + two consumer warpgroups
 
-template <int CG, int BN>
 struct MxCfg {
-  static constexpr int BN_CTA = BN / CG;                        // B rows this CTA stages (a pair splits the B tile)
-  static constexpr int STAGES = (CG == 2) ? 6 : ((BN == 256) ? 4 : 3);
+  static constexpr int STAGES = 6;
   static constexpr uint32_t A_BYTES = kBM * kBK;
-  static constexpr uint32_t B_BYTES = BN_CTA * kBK;
+  static constexpr uint32_t B_BYTES = kBN * kBK;
   static constexpr uint32_t OP_BYTES = A_BYTES + B_BYTES;
-  static constexpr uint32_t SFB_BYTES = kSfAtomBytes * (BN / 128);   // scales of ALL BN columns, in every CTA
-  static constexpr uint32_t SF_BYTES = kSfAtomBytes + SFB_BYTES;
-  static constexpr uint32_t BAR_BYTES = 192;
+  static constexpr uint32_t SF_BYTES = 2 * kSfAtomBytes;            // A rows' and B columns' scales of one K step
+  static constexpr uint32_t BAR_BYTES = 128;
   static constexpr uint32_t SMEM_BYTES = 1024 + STAGES * (OP_BYTES + SF_BYTES) + BAR_BYTES;
-  static constexpr uint32_t SFA_COL = BN;            // TMEM columns: [0, BN) accumulator, then 4 of A scales, then B's
-  static constexpr uint32_t SFB_COL = BN + 4;
-  static constexpr uint32_t TMEM_COLS = (BN == 256) ? 512 : 256;
-  static constexpr int CTAS_PER_SM = (CG == 1 && BN == 128) ? 2 : 1;
+  static_assert(SMEM_BYTES <= 232448, "227 KB of shared memory per block");
 };
 
 struct MxArgs {
@@ -81,35 +71,14 @@ __device__ __forceinline__ void bulk_load(uint32_t smem_dst, const void* gsrc, u
                : "memory");
 }
 
-// 32 rows x 16 bytes of shared memory -> TMEM lanes 0..31 (copied to all four lane quarters), 4 columns.
-// With cta_group::2 the copy runs in both CTAs of the pair, each from its own shared memory into its own TMEM.
-template <int CG>
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t taddr, uint64_t sdesc) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-  else
-    asm volatile("tcgen05.cp.cta_group::2.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
 }
 
-template <int CG>
-__device__ __forceinline__ void umma_mxf8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t sfa,
-                                          uint32_t sfb, uint32_t accumulate) {
-  if constexpr (CG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(sfa), "r"(sfb)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(sfa), "r"(sfb)
-        : "memory");
-  }
-}
+// byte k of a word of four UE8M0 scales -> 2^(byte - 127) as a float (byte 0, which only all-zero blocks get, -> 0)
+__device__ __forceinline__ float ue8m0_to_float(uint32_t w, int k) { return __uint_as_float(((w >> (8 * k)) & 0xFFu) << 23); }
 
 // Output tiles are walked in bands of 8 row tiles so that co-resident CTAs share A and B tiles in L2.
 __device__ __forceinline__ void decode_tile(long long t, int tiles_m, int tiles_n, int& g, int& m_blk, int& n_blk) {
@@ -124,14 +93,9 @@ __device__ __forceinline__ void decode_tile(long long t, int tiles_m, int tiles_
   n_blk = in_band / rows;
 }
 
-template <int CG, int BN>
-__global__ void __launch_bounds__(kMxThreads, MxCfg<CG, BN>::CTAS_PER_SM)
-mx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmSFA, const __grid_constant__ CUtensorMap tmSFB, const MxArgs args) {
-  using C = MxCfg<CG, BN>;
-  static_assert(CG == 1 || BN == 256, "CTA pairs work on 256 x 256 tiles");
-  const uint32_t cta_rank = (CG == 2) ? ptx::cluster_ctarank() : 0u;
-  const bool is_leader = (cta_rank == 0);
+__global__ void __launch_bounds__(kMxThreads, 1)
+mx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const MxArgs args) {
+  using C = MxCfg;
   extern __shared__ uint8_t smem_raw[];
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
@@ -145,199 +109,135 @@ mx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   auto smem_sfb = [&](int s) { return sf_base + s * C::SF_BYTES + kSfAtomBytes; };
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
-  const uint32_t tfull_bar = bar_base + 128u;
-  const uint32_t tempty_bar = bar_base + 136u;
-  const uint32_t tmem_slot = bar_base + 144u;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - ptx::smem_u32(smem_raw)));
 
   if (warp == 0 && ptx::elect_one()) {
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmB);
-    if constexpr (CG == 2) {
-      ptx::prefetch_tensormap(&tmSFA);
-      ptx::prefetch_tensormap(&tmSFB);
-    }
   }
-  if (warp == 2 && lane == 0) {
+  if (warp == 1 && lane == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       ptx::mbar_init(full_bar(s), 1);
-      ptx::mbar_init(empty_bar(s), 1);
+      ptx::mbar_init(empty_bar(s), 8);      // one arrival per consumer warp: each reads the stage's scales itself
     }
-    ptx::mbar_init(tfull_bar, 1);
-    ptx::mbar_init(tempty_bar, 4 * CG);     // one arrival per epilogue warp of every CTA of the group
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc<CG>(tmem_slot, C::TMEM_COLS);
-  ptx::tc_fence_before();
-  if constexpr (CG == 2) ptx::cluster_sync(); else __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_ptr, 0);
+  __syncthreads();
   const int num_kb = args.K / kBK;
+  const long long tile_first = blockIdx.x, tile_step = gridDim.x;
 
-  // Persistent: CTA (pair) b works on tiles b, b + grid, ...; the TMA producer runs ahead into the next tile while the
-  // epilogue warps still hold the previous one in registers.  A pair (CG == 2) shares one 256 x 256 tile: each CTA
-  // stages its 128 rows of A, HALF of the B tile (the tensor core reads the other half from the peer's shared memory)
-  // and the scales of its A rows and of all B columns; the leader issues every tcgen05 instruction for both.
-  const long long tile_first = blockIdx.x / CG, tile_step = gridDim.x / CG;
-  constexpr int kTileM = kBM * CG;
-  if (warp == 0) {
-    // =============================== TMA producer ===============================
-    int s = 0;
-    uint32_t ph = 0;
-    for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
-      int g, m_blk, n_blk;
-      decode_tile(t, args.tiles_m, args.tiles_n, g, m_blk, n_blk);
-      const int m0 = m_blk * kTileM + static_cast<int>(cta_rank) * kBM, n0 = n_blk * BN;
-      const uint8_t* sfa_g = args.sfa + static_cast<long long>(g) * num_kb * args.sfa_row_tiles * kSfAtomBytes;
-      const uint8_t* sfb_g = args.sfb + static_cast<long long>(g) * num_kb * args.sfb_row_tiles * kSfAtomBytes;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        ptx::mbar_wait(empty_bar(s), ph ^ 1u);
-        if (ptx::elect_one()) {
-          const uint32_t fb = full_bar(s);
-          if constexpr (CG == 1) {
+  if (warp < 4) {
+    ptx::setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // =============================== TMA producer ===============================
+      int s = 0;
+      uint32_t ph = 0;
+      for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
+        int g, m_blk, n_blk;
+        decode_tile(t, args.tiles_m, args.tiles_n, g, m_blk, n_blk);
+        const int m0 = m_blk * kBM, n0 = n_blk * kBN;
+        const uint8_t* sfa_g = args.sfa + static_cast<long long>(g) * num_kb * args.sfa_row_tiles * kSfAtomBytes;
+        const uint8_t* sfb_g = args.sfb + static_cast<long long>(g) * num_kb * args.sfb_row_tiles * kSfAtomBytes;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          ptx::mbar_wait_quiet(empty_bar(s), ph ^ 1u);
+          if (ptx::elect_one()) {
+            const uint32_t fb = full_bar(s);
             ptx::mbar_expect_tx(fb, C::OP_BYTES + C::SF_BYTES);
             ptx::tma_load_3d(smem_a(s), &tmA, fb, kb * kBK, m0, g);
             ptx::tma_load_3d(smem_b(s), &tmB, fb, kb * kBK, n0, g);
             bulk_load(smem_sfa(s), sfa_g + (static_cast<long long>(kb) * args.sfa_row_tiles + m_blk) * kSfAtomBytes,
                       kSfAtomBytes, fb);
-            bulk_load(smem_sfb(s),
-                      sfb_g + (static_cast<long long>(kb) * args.sfb_row_tiles + n_blk * (BN / 128)) * kSfAtomBytes,
-                      C::SFB_BYTES, fb);
-          } else {
-            // everything is credited to the LEADER's barrier; the scale atoms travel as [128 x uint32] rows of a tensor
-            // map (a plain bulk copy could only signal a barrier of the destination CTA)
-            if (is_leader) ptx::mbar_expect_tx(fb, 2 * (C::OP_BYTES + C::SF_BYTES));
-            ptx::tma_load_3d_2sm(smem_a(s), &tmA, fb, kb * kBK, m0, g);
-            ptx::tma_load_3d_2sm(smem_b(s), &tmB, fb, kb * kBK, n0 + static_cast<int>(cta_rank) * C::BN_CTA, g);
-            ptx::tma_load_3d_2sm(smem_sfa(s), &tmSFA, fb, 0, m_blk * CG + static_cast<int>(cta_rank), g * num_kb + kb);
-            ptx::tma_load_3d_2sm(smem_sfb(s), &tmSFB, fb, 0, n_blk * (BN / 128), g * num_kb + kb);
+            bulk_load(smem_sfb(s), sfb_g + (static_cast<long long>(kb) * args.sfb_row_tiles + n_blk) * kSfAtomBytes,
+                      kSfAtomBytes, fb);
           }
+          __syncwarp();
+          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
         }
-        __syncwarp();
-        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
       }
     }
-  } else if (warp == 1 && (CG == 1 || is_leader)) {
-    // =============================== MMA issuer ===============================
-    int s = 0;
-    uint32_t ph = 0, tph = 0;
+  } else {
+    ptx::setmaxnreg_inc<232>();
+    // =============================== consumers ===============================
+    const int cw = warp - 4;                       // consumer warp 0..7
+    const int wg = cw >> 2;                        // warpgroup: tile rows [64 wg, 64 wg + 64)
+    const int r0 = cw * 16 + (lane >> 2);          // this thread's accumulator rows in the tile: r0 and r0 + 8
+    const int c0 = (lane & 3) * 2;                 // ... and columns 8 j + c0 + {0, 1}, j = 0..15
+    // position of row / column i's four scale bytes inside a 512-byte atom (gemm_mx.h)
+    auto sf_off = [](int i) { return static_cast<uint32_t>((i % 32) * 16 + (i / 32) * 4); };
+    const uint32_t sa_off0 = sf_off(r0), sa_off1 = sf_off(r0 + 8);
     // Operand descriptors: K-major, SWIZZLE_128B, 8-row groups 1024 B apart; a K=32 step advances the start by 32 B.
-    constexpr uint32_t op_hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-    // Scale descriptors: K-major, no swizzle: 8-row x 16-byte core matrices of 128 contiguous bytes, 128 B apart.
-    constexpr uint32_t sf_hi = (128u >> 4) | (1u << 14);
-    // Instruction descriptor (block-scaled form): A/B format e4m3 (0), both K-major, N >> 3 at [17,23),
-    // scale format UE8M0 at [23], M >> 4 at [24,29); the scale byte of a K=32 step goes to [4,6) (B) and [29,31) (A).
-    // (The same byte index is mirrored into bits [30,32) of the scale addresses, as CUTLASS does; measured: the
-    // hardware takes it from the descriptor, results are identical without the mirror.)
-    constexpr uint32_t idesc0 = (static_cast<uint32_t>(BN >> 3) << 17) | (1u << 23) | (static_cast<uint32_t>((kBM * CG) >> 4) << 24);
-    const uint32_t d_tmem = tmem_base;
-    const uint32_t sfa_tmem = tmem_base + C::SFA_COL;
-    const uint32_t sfb_tmem = tmem_base + C::SFB_COL;
-    for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
-      ptx::mbar_wait(tempty_bar, tph ^ 1u);     // the epilogue warps have read the previous tile out of TMEM
-      ptx::tc_fence_after();
-      for (int kb = 0; kb < num_kb; ++kb) {
-        ptx::mbar_wait(full_bar(s), ph);
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) {
-          const uint32_t a_lo = ((smem_a(s) >> 4) & 0x3FFFu) | (1u << 16);
-          const uint32_t b_lo = ((smem_b(s) >> 4) & 0x3FFFu) | (1u << 16);
-          tmem_cp_32x128b_warpx4<CG>(sfa_tmem, (static_cast<uint64_t>(sf_hi) << 32) | ((smem_sfa(s) >> 4) & 0x3FFFu) | (1u << 16));
-#pragma unroll
-          for (int j = 0; j < BN / 128; ++j)
-            tmem_cp_32x128b_warpx4<CG>(sfb_tmem + 4u * j, (static_cast<uint64_t>(sf_hi) << 32) |
-                                                          (((smem_sfb(s) + j * kSfAtomBytes) >> 4) & 0x3FFFu) | (1u << 16));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t ad = (static_cast<uint64_t>(op_hi) << 32) | (a_lo + 2u * k);
-            const uint64_t bd = (static_cast<uint64_t>(op_hi) << 32) | (b_lo + 2u * k);
-            const uint32_t idesc = idesc0 | (static_cast<uint32_t>(k) << 4) | (static_cast<uint32_t>(k) << 29);
-            const uint32_t sub = static_cast<uint32_t>(k) << 30;
-            umma_mxf8<CG>(d_tmem, ad, bd, idesc, sfa_tmem + sub, sfb_tmem + sub, (kb | k) != 0);
-          }
-          ptx::umma_commit<CG>(empty_bar(s));
-          if (kb == num_kb - 1) ptx::umma_commit<CG>(tfull_bar);
-        }
-        __syncwarp();
-        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
-      }
-      tph ^= 1u;
-    }
-  } else if (warp >= 2) {
-    // =============================== epilogue ===============================
-    // Phase A moves the whole accumulator row of this thread into registers as packed bf16 (bias / ReLU applied in
-    // fp32 on the way) and hands TMEM back to the MMA warp; phase B (ReLU-backward mask, global stores) then overlaps
-    // the next tile's main loop.  There is only ONE accumulator buffer: 2 x 256 columns would leave no room for the
-    // scale columns in the 512-column tensor memory.
-    const int q = warp & 3;                 // TMEM lane quarter this warp may read
-    uint32_t tph = 0;
+    constexpr uint32_t desc_hi = (1024u >> 4) | (1u << 30);
+    int s = 0;
+    uint32_t ph = 0;
     const int epi = args.epi;
     for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
       int g, m_blk, n_blk;
       decode_tile(t, args.tiles_m, args.tiles_n, g, m_blk, n_blk);
-      const int n0 = n_blk * BN;
-      const int row = m_blk * kTileM + static_cast<int>(cta_rank) * kBM + q * 32 + lane;
-      const __nv_bfloat16* bias = args.bias == nullptr ? nullptr : args.bias + static_cast<long long>(g) * args.bias_group_stride + n0;
-      uint32_t pk[BN / 2];
-      ptx::mbar_wait(tfull_bar, tph);
-      ptx::tc_fence_after();
+      float acc[64];
 #pragma unroll
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t r[32];
-        ptx::tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(c * 32), r);
-        uint4 braw[4];                    // 32 bias values (bf16), fetched while the TMEM load is in flight
-        if (bias != nullptr) {
-#pragma unroll
-          for (int v = 0; v < 4; ++v) braw[v] = __ldg(reinterpret_cast<const uint4*>(bias + c * 32 + v * 8));
-        } else {
-#pragma unroll
-          for (int v = 0; v < 4; ++v) braw[v] = make_uint4(0u, 0u, 0u, 0u);
-        }
-        ptx::tmem_ld_wait();
-        const uint32_t* bw = reinterpret_cast<const uint32_t*>(braw);
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        ptx::mbar_wait_quiet(full_bar(s), ph);
+        const uint32_t a_lo = (((smem_a(s) + static_cast<uint32_t>(wg) * 8192u) >> 4) & 0x3FFFu) | (1u << 16);
+        const uint32_t b_lo = ((smem_b(s) >> 4) & 0x3FFFu) | (1u << 16);
+        const uint32_t saw0 = lds_u32(smem_sfa(s) + sa_off0), saw1 = lds_u32(smem_sfa(s) + sa_off1);
+        uint32_t sbw[32];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          // a bf16 is the upper half of the fp32 with the same value
-          float lo = __uint_as_float(r[2 * j]) + __uint_as_float(bw[j] << 16);
-          float hi = __uint_as_float(r[2 * j + 1]) + __uint_as_float(bw[j] & 0xFFFF0000u);
-          if (epi == MX_EPI_RELU) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
-          const __nv_bfloat162 p = __floats2bfloat162_rn(lo, hi);
-          pk[c * 16 + j] = *reinterpret_cast<const uint32_t*>(&p);
+          sbw[2 * j] = lds_u32(smem_sfb(s) + sf_off(8 * j + c0));
+          sbw[2 * j + 1] = lds_u32(smem_sfb(s) + sf_off(8 * j + c0 + 1));
         }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float part[64];
+          ptx::wgmma_fence();
+          ptx::wgmma_m64n128<DT_E4M3, false, false>(part, (static_cast<uint64_t>(desc_hi) << 32) | (a_lo + 2u * k),
+                                                    (static_cast<uint64_t>(desc_hi) << 32) | (b_lo + 2u * k), 0u);
+          ptx::wgmma_commit();
+          const float sa0 = ue8m0_to_float(saw0, k), sa1 = ue8m0_to_float(saw1, k);
+          ptx::wgmma_wait<0>();
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float sb = ue8m0_to_float(sbw[2 * j + e], k);
+              acc[4 * j + e] = fmaf(part[4 * j + e], sa0 * sb, acc[4 * j + e]);
+              acc[4 * j + 2 + e] = fmaf(part[4 * j + 2 + e], sa1 * sb, acc[4 * j + 2 + e]);
+            }
+          }
+        }
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(empty_bar(s));
+        if (++s == C::STAGES) { s = 0; ph ^= 1u; }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CG == 1) ptx::mbar_arrive(tempty_bar);
-        else ptx::mbar_arrive_cluster(tempty_bar, 0);
-      }
-      tph ^= 1u;
-      if (row < args.M) {
+
+      // ------------------------------- epilogue -------------------------------
+      const int n0 = n_blk * kBN + c0;
+      const __nv_bfloat16* bias = args.bias == nullptr ? nullptr : args.bias + static_cast<long long>(g) * args.bias_group_stride + n0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = m_blk * kBM + r0 + 8 * h;
+        if (row >= args.M) continue;
         __nv_bfloat16* drow = args.d + static_cast<long long>(g) * args.d_group_stride + static_cast<long long>(row) * args.ldd + n0;
         const __nv_bfloat16* arow = (epi == MX_EPI_RELU_BWD)
             ? args.aux + static_cast<long long>(g) * args.aux_group_stride + static_cast<long long>(row) * args.ld_aux + n0 : nullptr;
 #pragma unroll
-        for (int v = 0; v < BN / 8; ++v) {
-          uint4 w = make_uint4(pk[v * 4], pk[v * 4 + 1], pk[v * 4 + 2], pk[v * 4 + 3]);
-          if (epi == MX_EPI_RELU_BWD) {
-            // keep the gradient where the forward activation (bf16 pairs in `a`) was positive
-            const uint4 a = ptx::ld_nc_v4(arow + v * 8);
-            auto keep = [](uint32_t x) {
-              uint32_t m = 0u;
-              if ((x & 0x8000u) == 0u && (x & 0x7FFFu) != 0u) m |= 0xFFFFu;
-              if ((x & 0x80000000u) == 0u && (x & 0x7FFF0000u) != 0u) m |= 0xFFFF0000u;
-              return m;
-            };
-            w.x &= keep(a.x); w.y &= keep(a.y); w.z &= keep(a.z); w.w &= keep(a.w);
+        for (int j = 0; j < 16; ++j) {
+          float lo = acc[4 * j + 2 * h], hi = acc[4 * j + 2 * h + 1];
+          if (bias != nullptr) {
+            const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + 8 * j));
+            lo += b.x; hi += b.y;
           }
-          *reinterpret_cast<uint4*>(drow + v * 8) = w;
+          if (epi == MX_EPI_RELU) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
+          if (epi == MX_EPI_RELU_BWD) {
+            // keep the gradient where the forward activation was positive
+            const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(arow + 8 * j));
+            lo = a.x > 0.f ? lo : 0.f; hi = a.y > 0.f ? hi : 0.f;
+          }
+          *reinterpret_cast<__nv_bfloat162*>(drow + 8 * j) = __floats2bfloat162_rn(lo, hi);
         }
       }
     }
   }
-  ptx::tc_fence_before();
-  if constexpr (CG == 2) ptx::cluster_sync(); else __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<CG>(tmem_base, C::TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -478,24 +378,10 @@ bool mx_operand_map(CUtensorMap* map, const void* base, long long rows, long lon
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// scale atoms [groups * num_kb, row_tiles, 128 x uint32]: one box = `atoms` consecutive 512-byte atoms of one K step
-bool mx_scale_map(CUtensorMap* map, const void* base, long long row_tiles, long long kb_total, int atoms) {
-  EncodeTiledFn enc = mx_encode_fn();
-  if (enc == nullptr) return false;
-  cuuint64_t dims[3] = {128, static_cast<cuuint64_t>(row_tiles), static_cast<cuuint64_t>(kb_total)};
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(kSfAtomBytes), static_cast<cuuint64_t>(row_tiles) * kSfAtomBytes};
-  cuuint32_t box[3] = {128, static_cast<cuuint32_t>(atoms), 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, const_cast<void*>(base), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-template <int CG, int BN>
 cudaError_t mx_launch(const MxGemmProblem& p, cudaStream_t stream, const char** why) {
-  using C = MxCfg<CG, BN>;
-  CUtensorMap ta, tb_, tsa, tsb;
-  if (!mx_operand_map(&ta, p.a, p.M, p.K, p.G, kBM) || !mx_operand_map(&tb_, p.b, p.N, p.K, p.G, C::BN_CTA)) {
+  using C = MxCfg;
+  CUtensorMap ta, tb_;
+  if (!mx_operand_map(&ta, p.a, p.M, p.K, p.G, kBM) || !mx_operand_map(&tb_, p.b, p.N, p.K, p.G, kBN)) {
     if (why) *why = "cuTensorMapEncodeTiled failed for an MX operand";
     return cudaErrorInvalidValue;
   }
@@ -506,8 +392,8 @@ cudaError_t mx_launch(const MxGemmProblem& p, cudaStream_t stream, const char** 
   a.ldd = p.ldd;
   a.d_group_stride = p.d_group_stride;
   a.M = p.M; a.N = p.N; a.K = p.K; a.G = p.G;
-  a.tiles_m = (p.M + kBM * CG - 1) / (kBM * CG);
-  a.tiles_n = p.N / BN;
+  a.tiles_m = (p.M + kBM - 1) / kBM;
+  a.tiles_n = p.N / kBN;
   a.sfa_row_tiles = (p.M + 127) / 128;
   a.sfb_row_tiles = (p.N + 127) / 128;
   a.bias = static_cast<const __nv_bfloat16*>(p.bias);
@@ -516,21 +402,10 @@ cudaError_t mx_launch(const MxGemmProblem& p, cudaStream_t stream, const char** 
   a.ld_aux = p.ld_aux;
   a.aux_group_stride = p.aux_group_stride;
   a.epi = p.epilogue;
-  if (CG == 2) {
-    const long long kb_total = static_cast<long long>(p.G) * (p.K / kBK);
-    if (!mx_scale_map(&tsa, p.sfa, a.sfa_row_tiles, kb_total, 1) || !mx_scale_map(&tsb, p.sfb, a.sfb_row_tiles, kb_total, BN / 128)) {
-      if (why) *why = "cuTensorMapEncodeTiled failed for the MX scales";
-      return cudaErrorInvalidValue;
-    }
-  } else {
-    tsa = ta;
-    tsb = ta;
-  }
-  auto* kern = mx_gemm_kernel<CG, BN>;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [kern] {
-    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+  std::call_once(once, [] {
+    attr_err = cudaFuncSetAttribute(mx_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
   });
   if (attr_err != cudaSuccess) return attr_err;
   a.num_tiles = static_cast<long long>(a.tiles_m) * a.tiles_n * p.G;
@@ -538,23 +413,13 @@ cudaError_t mx_launch(const MxGemmProblem& p, cudaStream_t stream, const char** 
   if (sms == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
-  long long groups = static_cast<long long>(sms) * C::CTAS_PER_SM / CG;    // resident CTAs (pairs)
-  if (p.max_ctas > 0) groups = std::max<long long>(1, std::min<long long>(groups, p.max_ctas / CG));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(std::min<long long>(a.num_tiles, groups) * CG));
-  cfg.blockDim = dim3(kMxThreads);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, ta, tb_, tsa, tsb, a);
+  long long ctas = sms;                                                    // one resident CTA per SM
+  if (p.max_ctas > 0) ctas = std::max<long long>(1, std::min<long long>(ctas, p.max_ctas));
+  const unsigned grid = static_cast<unsigned>(std::min<long long>(a.num_tiles, ctas));
+  mx_gemm_kernel<<<grid, kMxThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
+  return cudaGetLastError();
 }
 
 }  // namespace
@@ -568,20 +433,17 @@ cudaError_t mx_gemm_launch(const MxGemmProblem& p, cudaStream_t stream, const ch
        reinterpret_cast<uintptr_t>(p.sfb) | reinterpret_cast<uintptr_t>(p.d)) & 15)
     return fail("MX GEMM: operands must be 16-byte aligned");
   if (p.ldd % 8 != 0 || p.d_group_stride % 8 != 0) return fail("MX GEMM: output strides must be multiples of 8 elements");
-  int bn = p.block_n;
-  if (bn == 0) bn = (p.N % 256 == 0) ? 256 : 128;
-  if (bn == 256 && p.N % 256 != 0) return fail("MX GEMM: block_n 256 needs N % 256 == 0");
   if (p.epilogue == MX_EPI_RELU_BWD && (p.aux == nullptr || (reinterpret_cast<uintptr_t>(p.aux) & 15) || p.ld_aux % 8 || p.aux_group_stride % 8))
     return fail("MX GEMM: the ReLU-backward epilogue needs a 16-byte aligned aux operand");
   if (p.bias != nullptr && ((reinterpret_cast<uintptr_t>(p.bias) & 15) || p.bias_group_stride % 8))
     return fail("MX GEMM: bias must be 16-byte aligned");
-  int cg = p.cta_group;
-  if (cg == 0) cg = (bn == 256 && p.M > 128) ? 2 : 1;     // pairs halve the B traffic per SM: 2.8-3.1 vs 2.4-2.6 PFLOP/s
-  if (cg == 2 && bn != 256) return fail("MX GEMM: CTA pairs need block_n 256");
-  if (cg == 2) return mx_launch<2, 256>(p, stream, why);
-  if (bn == 256) return mx_launch<1, 256>(p, stream, why);
-  if (bn == 128) return mx_launch<1, 128>(p, stream, why);
-  return fail("MX GEMM: block_n must be 128 or 256");
+  // block_n / cta_group are the tile-shape hints of callers written for wider tiles and CTA pairs: validated, but this
+  // kernel has ONE tile shape (128 x 128, one CTA), so they do not change what runs.
+  if (p.block_n != 0 && p.block_n != 128 && p.block_n != 256) return fail("MX GEMM: block_n must be 0, 128 or 256");
+  if (p.block_n == 256 && p.N % 256 != 0) return fail("MX GEMM: block_n 256 needs N % 256 == 0");
+  if (p.cta_group < 0 || p.cta_group > 2) return fail("MX GEMM: cta_group must be 0, 1 or 2");
+  if (p.cta_group == 2 && p.block_n != 0 && p.block_n != 256) return fail("MX GEMM: CTA pairs need block_n 256");
+  return mx_launch(p, stream, why);
 }
 
 cudaError_t mx_quantize(const void* x, void* q, void* sf, int groups, int rows, int k, int elem_type, cudaStream_t stream) {
@@ -589,7 +451,7 @@ cudaError_t mx_quantize(const void* x, void* q, void* sf, int groups, int rows, 
   const long long total = static_cast<long long>(groups) * rows * (k / 8);
   if (total == 0) return cudaSuccess;
   const int row_tiles = (rows + 127) / 128;
-  const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 148LL * 16));
+  const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 132LL * 16));
   if (elem_type == ET_BF16)
     mx_quantize_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), static_cast<uint8_t*>(q),
                                                                   static_cast<uint8_t*>(sf), total, rows, k, row_tiles);

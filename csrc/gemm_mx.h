@@ -1,4 +1,4 @@
-// Host API of the MX block-scaled fp8 GEMM (tcgen05.mma kind::mxf8f6f4.block_scale) and its quantiser; see gemm_mx.cu.
+// Host API of the MX block-scaled fp8 GEMM (one e4m3 wgmma per 32-element K block, scales applied to the fp32 partial sums) and its quantiser; see gemm_mx.cu.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -6,7 +6,7 @@
 namespace tb {
 
 // Scale factors (UE8M0, one per 32 consecutive K elements of a row) are stored in the tile order the tensor core
-// reads them from TMEM:   sf[g][kb][rt][ (r % 32) * 16 + ((r % 128) / 32) * 4 + (k % 128) / 32 ]
+// reads them from shared memory:   sf[g][kb][rt][ (r % 32) * 16 + ((r % 128) / 32) * 4 + (k % 128) / 32 ]
 // with kb = k / 128, rt = r / 128 - one 512-byte atom per 128 rows x 128 K elements, so a CTA stages the scales of a
 // whole operand tile with a single bulk copy.  Rows are padded to a multiple of 128 (pad scales are 0 = 2^-127).
 inline long long mx_sf_bytes(int groups, long long rows, long long k) {
@@ -38,9 +38,9 @@ struct MxGemmProblem {
   const void* aux = nullptr;     // MX_EPI_RELU_BWD: bf16 [G, M, N] forward activation
   long long ld_aux = 0, aux_group_stride = 0;
   int epilogue = 0;              // MxEpilogue
-  int block_n = 0;               // 128 or 256 (0: 256 when N % 256 == 0)
-  int cta_group = 0;             // 1, or 2 = CTA pairs on 256 x 256 tiles (block_n 256 only); 0: auto
-  int max_ctas = 0;              // 0: one wave of resident CTAs
+  int block_n = 0;               // 0, 128 or 256: tile-shape hint of callers written for wider tiles; the kernel tiles 128 x 128
+  int cta_group = 0;             // 0, 1 or 2: likewise a hint only (Hopper has no CTA-pair MMA)
+  int max_ctas = 0;              // 0: one CTA per SM
 };
 
 cudaError_t mx_gemm_launch(const MxGemmProblem& p, cudaStream_t stream, const char** why = nullptr);

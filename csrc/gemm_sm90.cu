@@ -1,0 +1,842 @@
+// wgmma / TMA grouped GEMM for sm_90a (H100).
+//
+// Replaces the reference's cuBLAS `torch.matmul` expert GEMMs (tutel/experts/ffn.py:114-118,
+// tutel/experts/llama_ffn.py:38-41) and its host-synchronised per-expert loop
+// `sparse_bmm_infer` (tutel/custom/custom_kernel.cpp:874-889) with ONE persistent, warp-specialised kernel
+// (384 threads, 128 x 128 output tiles):
+//
+//   warp 0        TMA producer   cp.async.bulk.tensor (128B swizzle) -> smem ring, mbarrier complete_tx; the other
+//                                three warps of its warpgroup only give their registers away (setmaxnreg)
+//   warps 4..11   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async (m64n128, operands straight from
+//                                the swizzled ring, fp32 accumulator fragment in registers), one stage in flight; a stage is
+//                                handed back to the producer when the wgmma group that read it has retired.
+//                                Epilogue: every warp parks its 16 x 128 fragment in its own shared-memory rows and
+//                                reads it back with one lane per row and 32 consecutive columns per lane, applies the
+//                                fused bias / activation / activation-grad / GLU / bias-grad math in fp32 and writes 64
+//                                contiguous bytes per lane - locally or straight into PEER GPUs' memory plus a
+//                                release.sys counter bump (GEMM -> combine all-to-all fusion) - while the producer
+//                                already fills the ring for the next tile.
+//
+// The producer can also acquire system-scope "rows have arrived" counters before loading an A tile, which is
+// how the dispatch all-to-all is overlapped tile-by-tile with the first expert GEMM.
+#include "gemm_sm90.h"
+
+#include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include <cstdio>
+#include <cstdlib>
+#include <mutex>
+
+#include "ptx.cuh"
+
+namespace tb {
+
+struct GemmArgs {
+  int M, N, K, G;
+  int b_group_div;
+  int tiles_m, tiles_n;
+  long long num_tiles;
+
+  void* d;
+  long long ldd, d_group_stride;
+  const unsigned long long* d_ptr_table;
+  int out_dtype;
+
+  int epilogue;
+  float alpha;
+  const void* bias;
+  long long bias_group_stride;
+  int bias_is_fp32;
+  int bias_is_bf16;
+  const void* aux;
+  long long ld_aux, aux_group_stride;
+  const void* aux2;
+  void* d2;
+  void* d3;
+  int dual;        // EPI_GLU: B tile = 64 columns of tmB + the same 64 columns of tmB2
+  int act;
+  const float* scale_b2;
+
+  const int* row_counts;
+  float* colsum;  // [G / b_group_div, N] fp32: += column sums of the epilogue result (bias gradient), may be null
+  long long colsum_group_stride;
+  const float* scale_a;  // [G, M] per-row dequantisation scales (fp8 operands), may be null
+  long long scale_a_group_stride;
+  const float* scale_b;  // [G / b_group_div, N] per-column scales, may be null
+  long long scale_b_group_stride;
+
+  const uint32_t* wait_flags;
+  int wait_rows_per_flag, wait_flags_per_group;
+  uint32_t wait_target;
+  const unsigned long long* signal_ptr_table;
+  int group_rot, group_mod;  // tile order visits group (g/mod)*mod + (g%mod + rot)%mod  (own-rank segment first)
+};
+
+namespace {
+
+constexpr int kThreads = 384;        // producer warpgroup + two consumer warpgroups
+constexpr int kSwizzleBytes = 128;   // one swizzle row: 64 bf16 / 128 fp8
+constexpr int kSmemLimit = 232448;   // 227 KB
+
+struct Cfg {
+  static constexpr int BM = 128;
+  static constexpr int BN = 128;
+  static constexpr int A_BYTES = BM * kSwizzleBytes;
+  static constexpr int B_BYTES = BN * kSwizzleBytes;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  // Epilogue staging: per consumer warp 16 accumulator rows of BN floats; 8 floats of padding per row keep the
+  // fragment writes (float2, four rows per half-warp) free of bank conflicts.
+  static constexpr int EPI_PITCH = BN + 8;
+  static constexpr int EPI_WARP_BYTES = 16 * EPI_PITCH * 4;
+  static constexpr int EPI_BYTES = 8 * EPI_WARP_BYTES;
+  static constexpr int BAR_BYTES = 512;
+  static constexpr int STAGES = 4;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + BAR_BYTES + EPI_BYTES;
+  // 228 KB per SM, 1 KB reserved per resident block: a dispatch block (no shared memory of its own) must still fit
+  static_assert(SMEM_BYTES + 2 * 1024 <= 228 * 1024, "no room for the push kernel");
+  static_assert(SMEM_BYTES <= kSmemLimit, "");
+};
+
+struct TileCoord {
+  int g, m_blk, n_blk;
+};
+
+// Tiles are enumerated group-major; inside a group, bands of kBand row-blocks sweep all column blocks so that a
+// wave of CTAs re-uses both its A band and its B columns out of L2.
+template <int kBand>
+__device__ __forceinline__ TileCoord decode_tile(long long t, int tiles_m, int tiles_n) {
+  const int per_group = tiles_m * tiles_n;
+  TileCoord c;
+  c.g = static_cast<int>(t / per_group);
+  int r = static_cast<int>(t - static_cast<long long>(c.g) * per_group);
+  const int band_tiles = kBand * tiles_n;
+  const int band = r / band_tiles;
+  const int first_m = band * kBand;
+  const int rows_in_band = min(kBand, tiles_m - first_m);
+  r -= band * band_tiles;
+  c.m_blk = first_m + r % rows_in_band;
+  c.n_blk = r / rows_in_band;
+  return c;
+}
+
+// mod > 1: ascending from `rot`;  mod < -1: descending from `rot` (matches a sender that walks destinations upwards).
+__device__ __forceinline__ int rotate_group(int g, int rot, int mod) {
+  if (mod > 1) {
+    const int base = (g / mod) * mod;
+    return base + (g - base + rot) % mod;
+  }
+  if (mod < -1) {
+    const int m = -mod;
+    const int base = (g / m) * m;
+    return base + (rot + m - (g - base)) % m;
+  }
+  return g;
+}
+
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+__device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
+
+__device__ __forceinline__ void unpack8(const uint4& u, bool is_bf16, float* f) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    if (is_bf16) {
+      f[2 * i] = __uint_as_float(w[i] << 16);
+      f[2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+    } else {
+      const __half2 h = *reinterpret_cast<const __half2*>(&w[i]);
+      const float2 t = __half22float2(h);
+      f[2 * i] = t.x;
+      f[2 * i + 1] = t.y;
+    }
+  }
+}
+// 32 floats -> 16 packed words; the dtype branch is taken ONCE per segment (a per-element branch on a kernel argument
+// serialises the unrolled loop and costs all its instruction-level parallelism).
+template <bool BF16>
+__device__ __forceinline__ void pack32_t(const float* v, uint32_t* w) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    if constexpr (BF16) {
+      const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
+      w[i] = *reinterpret_cast<const uint32_t*>(&h);
+    } else {
+      const __half2 h = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
+      w[i] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+  }
+}
+__device__ __forceinline__ void pack32(const float* v, uint32_t* w, bool is_bf16) {
+  if (is_bf16) pack32_t<true>(v, w); else pack32_t<false>(v, w);
+}
+template <bool BF16>
+__device__ __forceinline__ void unpack32_t(const uint4* p, float* f) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const uint32_t w[4] = {p[q].x, p[q].y, p[q].z, p[q].w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      if constexpr (BF16) {
+        f[q * 8 + 2 * i] = __uint_as_float(w[i] << 16);
+        f[q * 8 + 2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+      } else {
+        const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+        f[q * 8 + 2 * i] = t.x;
+        f[q * 8 + 2 * i + 1] = t.y;
+      }
+    }
+  }
+}
+__device__ __forceinline__ void unpack32(const uint4* p, float* f, bool is_bf16) {
+  if (is_bf16) unpack32_t<true>(p, f); else unpack32_t<false>(p, f);
+}
+
+__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
+
+// GLU math on one 32-column segment, activation fixed at compile time (branch-free, fully interleavable).
+template <int ACT>
+__device__ __forceinline__ void glu_fwd_seg(const float* g, const float* u, float* o) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    float a;
+    if constexpr (ACT == ACT_RELU) a = fmaxf(g[j], 0.0f);
+    else if constexpr (ACT == ACT_GELU) a = gelu_erf(g[j]);
+    else a = g[j] * fast_sigmoid(g[j]);
+    o[j] = a * u[j];
+  }
+}
+// in: dh, g, u      out: o = d gate, u = d up
+template <int ACT>
+__device__ __forceinline__ void glu_bwd_seg(const float* r, const float* g, float* u, float* o) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float dh = r[j];
+    float a, da;
+    if constexpr (ACT == ACT_RELU) {
+      a = fmaxf(g[j], 0.0f);
+      da = g[j] > 0.0f ? 1.0f : 0.0f;
+    } else if constexpr (ACT == ACT_GELU) {
+      const float cdf = 0.5f * (1.0f + erff(g[j] * 0.70710678118654752f));
+      a = g[j] * cdf;
+      da = cdf + g[j] * 0.3989422804014327f * __expf(-0.5f * g[j] * g[j]);
+    } else {
+      const float sg = fast_sigmoid(g[j]);
+      a = g[j] * sg;
+      da = sg * (1.0f + g[j] * (1.0f - sg));
+    }
+    o[j] = dh * u[j] * da;
+    u[j] = dh * a;
+  }
+}
+
+// Resource budget (deliberate): 384 threads x 144 registers = 55296 of the SM's 65536 registers (the producer warpgroup
+// shrinks to 40 per thread, the two consumer warpgroups grow to 192: 128 x 40 + 256 x 192 = 54272) and 202 KB of its
+// 228 KB shared memory, so ONE 128-thread x 64-register block of the dispatch kernel (encode_rows, which needs no
+// shared memory) always fits next to a GEMM CTA.  That is what makes the dispatch+GEMM fusion deadlock-free: a GEMM
+// whose producer spins on arrival flags can never starve the kernel that publishes them, whichever gets the SMs first.
+template <bool A_MN, bool B_MN, int DT>
+__global__ void __maxnreg__(144)
+gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmB2, const GemmArgs args) {
+  using C = Cfg;
+  constexpr int BN = C::BN;
+  extern __shared__ uint8_t smem_raw[];
+
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);  // warp-uniform role id
+  const int lane = threadIdx.x & 31;
+
+  // ---- shared memory carve-up (operand ring must be 1024B aligned for the 128B swizzle) ----
+  const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
+  constexpr int stages = C::STAGES;
+  const uint32_t bar_base = smem_base + static_cast<uint32_t>(stages) * C::STAGE_BYTES;
+  auto smem_a = [&](int s) { return smem_base + s * C::STAGE_BYTES; };
+  auto smem_b = [&](int s) { return smem_base + s * C::STAGE_BYTES + C::A_BYTES; };
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
+  const uint32_t epi_base = bar_base + C::BAR_BYTES;
+  float* epi_ptr = reinterpret_cast<float*>(smem_raw + (epi_base - ptx::smem_u32(smem_raw)));
+
+  if (warp == 0 && ptx::elect_one()) {
+    ptx::prefetch_tensormap(&tmA);
+    ptx::prefetch_tensormap(&tmB);
+    if (args.dual) ptx::prefetch_tensormap(&tmB2);
+  }
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < stages; ++s) {
+      ptx::mbar_init(full_bar(s), 1);
+      ptx::mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
+    }
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+
+  constexpr int kEltBytes = (DT == DT_E4M3 || DT == DT_E5M2) ? 1 : 2;   // 2: wgmma k16   1: wgmma k32
+  static_assert(kEltBytes == 2 || (!A_MN && !B_MN), "8-bit operands are K-major only");
+  const int num_kb = (args.K * kEltBytes + kSwizzleBytes - 1) / kSwizzleBytes;
+  constexpr int bk_elems = kSwizzleBytes / kEltBytes;        // K elements per stage
+  const long long tile_step = gridDim.x;
+  const long long tile_first = blockIdx.x;
+  constexpr int kBand = 16;
+  const bool dual = args.dual != 0;
+  const int tile_n = dual ? BN / 2 : BN;   // output columns per tile
+
+  if (warp < 4) {
+    ptx::setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // =============================== TMA producer ===============================
+      int s = 0;
+      uint32_t ph = 0;
+      int seen_group = -1;
+      unsigned long long seen_mask = 0ull;
+      for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
+        TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
+        tc.g = rotate_group(tc.g, args.group_rot, args.group_mod);
+        if (args.row_counts != nullptr && tc.m_blk * C::BM >= args.row_counts[tc.g]) continue;
+        const int m0 = tc.m_blk * C::BM;
+        const int n0 = tc.n_blk * BN;   // (non-dual) first B column of this tile
+        const int gb = tc.g / args.b_group_div;
+        if (args.wait_flags != nullptr) {
+          // Dispatch fusion: rows of this tile are pushed by peer GPUs; acquire their release flags - once per
+          // (group, flag): consecutive tiles of a group share flags, so remember which ones were already seen.
+          if (tc.g != seen_group) { seen_group = tc.g; seen_mask = 0ull; }
+          const int f0 = (tc.m_blk * C::BM) / args.wait_rows_per_flag;
+          const int f1 = (min(tc.m_blk * C::BM + C::BM, args.M) - 1) / args.wait_rows_per_flag;
+          unsigned long long need = 0ull;
+          for (int f = f0; f <= f1; ++f) need |= 1ull << (f & 63);
+          if ((seen_mask & need) != need) {
+            if (lane == 0) {
+              for (int f = f0; f <= f1; ++f)
+                if (!((seen_mask >> (f & 63)) & 1ull))
+                  ptx::wait_flag_ge_sys_quiet(args.wait_flags + static_cast<long long>(tc.g) * args.wait_flags_per_group + f,
+                                        args.wait_target);
+              ptx::fence_proxy_async_global();  // order the upcoming async-proxy (TMA) reads after the acquire
+            }
+            __syncwarp();
+            seen_mask |= need;
+          }
+        }
+        for (int kb = 0; kb < num_kb; ++kb) {
+          ptx::mbar_wait_quiet(empty_bar(s), ph ^ 1u);
+          if (ptx::elect_one()) {
+            const uint32_t fb = full_bar(s);
+            ptx::mbar_expect_tx(fb, C::STAGE_BYTES);
+            const int k0 = kb * bk_elems;
+            constexpr int chunk_elems = kSwizzleBytes / kEltBytes;    // MN-major: one 128-byte chunk of the MN axis ...
+            constexpr int chunk_bytes = bk_elems * kSwizzleBytes;     // ... times the stage's K rows
+            // ---- A ----
+            if constexpr (!A_MN) {
+              ptx::tma_load_3d(smem_a(s), &tmA, fb, k0, m0, tc.g);
+            } else {
+              for (int c = 0; c < C::BM / chunk_elems; ++c)
+                ptx::tma_load_3d(smem_a(s) + c * chunk_bytes, &tmA, fb, m0 + c * chunk_elems, k0, tc.g);
+            }
+            // ---- B ----
+            if (!dual) {
+              if constexpr (!B_MN) {
+                ptx::tma_load_3d(smem_b(s), &tmB, fb, k0, n0, gb);
+              } else {
+                for (int c = 0; c < BN / chunk_elems; ++c)
+                  ptx::tma_load_3d(smem_b(s) + c * chunk_bytes, &tmB, fb, n0 + c * chunk_elems, k0, gb);
+              }
+            } else {
+              // GLU: accumulator columns [0, BN/2) come from B, [BN/2, BN) from B2, both at weight columns nb0...
+              const int nb0 = tc.n_blk * (BN / 2);
+              if constexpr (!B_MN) {
+                ptx::tma_load_3d(smem_b(s), &tmB, fb, k0, nb0, gb);
+                ptx::tma_load_3d(smem_b(s) + (BN / 2) * kSwizzleBytes, &tmB2, fb, k0, nb0, gb);
+              } else {
+                constexpr int half_chunks = (BN / 2) / chunk_elems;
+                for (int c = 0; c < 2 * half_chunks; ++c)
+                  ptx::tma_load_3d(smem_b(s) + c * chunk_bytes, c < half_chunks ? &tmB : &tmB2, fb,
+                                   nb0 + (c % half_chunks) * chunk_elems, k0, gb);
+              }
+            }
+          }
+          __syncwarp();
+          if (++s == stages) { s = 0; ph ^= 1u; }
+        }
+      }
+    }
+  } else {
+    ptx::setmaxnreg_inc<192>();
+    // =============================== consumers: wgmma main loop + epilogue ===============================
+    const int cw = warp - 4;          // consumer warp 0..7 owns tile rows [16 cw, 16 cw + 16)
+    const int wg = cw >> 2;           // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    int s = 0;
+    uint32_t ph = 0;
+    // Descriptor = constant high word + low word {start>>4, lbo>>4}.  Advancing along K inside a stage and
+    // from stage to stage only adds to the 14-bit start-address field (smem < 256 KB, so it never carries).
+    constexpr uint32_t kMnChunkBytes = 64u * kSwizzleBytes;           // BK rows * 128 B (16-bit operands)
+    constexpr uint32_t kMnKStep = 16u * kSwizzleBytes;                // 16 K rows * 128 B
+    constexpr uint32_t a_lbo = A_MN ? kMnChunkBytes : 16u;
+    constexpr uint32_t b_lbo = B_MN ? kMnChunkBytes : 16u;
+    constexpr uint32_t a_kstep = (A_MN ? kMnKStep : 32u) >> 4;
+    constexpr uint32_t b_kstep = (B_MN ? kMnKStep : 32u) >> 4;
+    constexpr uint32_t desc_hi = (1024u >> 4) | (1u << 30);           // SBO | SWIZZLE_128B
+    // this warpgroup's 64 rows of A: K-major 64 rows x 128 B, MN-major one 64-element chunk - 8 KB either way
+    const uint32_t a_lo0 = (((smem_a(0) + static_cast<uint32_t>(wg) * 8192u) >> 4) & 0x3FFFu) | ((a_lbo >> 4) << 16);
+    const uint32_t b_lo0 = ((smem_b(0) >> 4) & 0x3FFFu) | ((b_lbo >> 4) << 16);
+
+    const bool out16 = (args.out_dtype != DT_FP32);
+    const bool out_bf16 = (args.out_dtype == DT_BF16);
+    const bool glu = args.epilogue == EPI_GLU || args.epilogue == EPI_GLU_BWD;
+    // Epilogue geometry: lane l works on accumulator row (l % 16) of this warp and on 32 consecutive columns, the
+    // lower half-warp on the first and the upper half-warp on the second half of every 64-column chunk.
+    float* epi_warp = epi_ptr + cw * 16 * C::EPI_PITCH;
+    const float* epi_row = epi_warp + (lane & 15) * C::EPI_PITCH;
+    const int col_half = (lane >> 4) * 32;
+    auto load_acc = [&](int col, float* v) {
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float4 t4 = *reinterpret_cast<const float4*>(epi_row + col + q * 4);
+        v[q * 4] = t4.x; v[q * 4 + 1] = t4.y; v[q * 4 + 2] = t4.z; v[q * 4 + 3] = t4.w;
+      }
+    };
+
+    for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
+      TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
+      tc.g = rotate_group(tc.g, args.group_rot, args.group_mod);
+      int m_valid = args.M;
+      if (args.row_counts != nullptr) {
+        m_valid = min(args.M, args.row_counts[tc.g]);
+        if (tc.m_blk * C::BM >= m_valid) continue;
+      }
+      // ------------------------------- main loop -------------------------------
+      float acc[64];
+      int prev_s = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        ptx::mbar_wait_quiet(full_bar(s), ph);
+        const uint32_t a_lo = a_lo0 + static_cast<uint32_t>(s) * (C::STAGE_BYTES >> 4);
+        const uint32_t b_lo = b_lo0 + static_cast<uint32_t>(s) * (C::STAGE_BYTES >> 4);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t ad = (static_cast<uint64_t>(desc_hi) << 32) | (a_lo + k * a_kstep);
+          const uint64_t bd = (static_cast<uint64_t>(desc_hi) << 32) | (b_lo + k * b_kstep);
+          ptx::wgmma_m64n128<DT, A_MN, B_MN>(acc, ad, bd, (kb | k) != 0);
+        }
+        ptx::wgmma_commit();
+        if (kb > 0) {
+          ptx::wgmma_wait<1>();                                   // the group that read the previous stage has retired
+          if (wg_leader) ptx::mbar_arrive(empty_bar(prev_s));
+        }
+        prev_s = s;
+        if (++s == stages) { s = 0; ph ^= 1u; }
+      }
+      ptx::wgmma_wait<0>();
+      if (wg_leader) ptx::mbar_arrive(empty_bar(prev_s));
+
+      // ------------------------------- epilogue -------------------------------
+      {
+        const int fr = lane >> 2, fc = (lane & 3) * 2;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          *reinterpret_cast<float2*>(epi_warp + fr * C::EPI_PITCH + j * 8 + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(epi_warp + (fr + 8) * C::EPI_PITCH + j * 8 + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      __syncwarp();
+
+      const int m = tc.m_blk * C::BM + cw * 16 + (lane & 15);
+      const bool row_ok = m < m_valid;
+      const int gb = tc.g / args.b_group_div;
+      uint8_t* d_base = (args.d_ptr_table != nullptr)
+                            ? reinterpret_cast<uint8_t*>(args.d_ptr_table[tc.g])
+                            : reinterpret_cast<uint8_t*>(args.d) +
+                                  static_cast<long long>(tc.g) * args.d_group_stride * (out16 ? 2 : 4);
+      uint8_t* d_row = d_base + static_cast<long long>(m) * args.ldd * (out16 ? 2 : 4);
+      const uint8_t* aux_row = nullptr;
+      if (args.aux != nullptr)
+        aux_row = reinterpret_cast<const uint8_t*>(args.aux) +
+                  (static_cast<long long>(tc.g) * args.aux_group_stride + static_cast<long long>(m) * args.ld_aux) * 2;
+      const uint8_t* aux2_row = nullptr;
+      if (args.aux2 != nullptr)
+        aux2_row = reinterpret_cast<const uint8_t*>(args.aux2) +
+                   (static_cast<long long>(tc.g) * args.aux_group_stride + static_cast<long long>(m) * args.ld_aux) * 2;
+      const uint8_t* bias_g = nullptr;
+      if (args.bias != nullptr)
+        bias_g = reinterpret_cast<const uint8_t*>(args.bias) +
+                 static_cast<long long>(gb) * args.bias_group_stride * (args.bias_is_fp32 ? 4 : 2);
+
+      // One 32-column segment of this lane's row -> global memory (local or a peer's): 64 contiguous bytes in 16 bit.
+      // ncols (a multiple of 8) may be <= 0 for segments past the last column: nothing is touched then.
+      auto store_seg = [&](uint8_t* row, int n, int ncols, const float* v) {
+        if (!row_ok) return;
+        if (out16) {
+          uint32_t w[16];
+          pack32(v, w, out_bf16);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            if (q * 8 < ncols) {
+              *reinterpret_cast<uint4*>(row + (n + q * 8) * 2) = make_uint4(w[q * 4], w[q * 4 + 1], w[q * 4 + 2], w[q * 4 + 3]);
+            }
+          }
+        } else {
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            if (q * 4 < ncols) {
+              float4 o = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
+              *reinterpret_cast<float4*>(row + (n + q * 4) * 4) = o;
+            }
+          }
+        }
+      };
+      // 32 values of a 16-bit [.., ld] side input (zeros for rows / columns past the end)
+      auto load_seg16 = [&](const uint8_t* row, int n, int ncols, float* f) {
+        uint4 p[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          p[q] = (row_ok && q * 8 < ncols) ? ptx::ld_nc_v4(row + (n + q * 8) * 2) : make_uint4(0u, 0u, 0u, 0u);
+        unpack32(p, f, out_bf16);
+      };
+
+      if (glu) {
+        // ---------------- gated-linear-unit epilogues ----------------
+        const bool fwd = args.epilogue == EPI_GLU;
+        const long long row_off = (static_cast<long long>(tc.g) * args.d_group_stride + static_cast<long long>(m) * args.ldd) * 2;
+        uint8_t* d2_row = args.d2 != nullptr ? reinterpret_cast<uint8_t*>(args.d2) + row_off : nullptr;
+        uint8_t* d3_row = args.d3 != nullptr ? reinterpret_cast<uint8_t*>(args.d3) + row_off : nullptr;
+        const float sa = (args.scale_a != nullptr && row_ok)
+                             ? args.scale_a[static_cast<long long>(tc.g) * args.scale_a_group_stride + m] : 1.0f;
+#pragma unroll 1
+        for (int c = 0; c < tile_n / 64; ++c) {
+          const int col = c * 64 + col_half;
+          const int n = tc.n_blk * tile_n + col;
+          const int ncols = min(32, args.N - n);
+          float g[32], u[32], o[32];
+          if (fwd) {
+            load_acc(col, g);
+            load_acc(BN / 2 + col, u);
+            if (args.scale_a != nullptr || args.scale_b != nullptr) {
+              const float* sb = args.scale_b != nullptr ? args.scale_b + static_cast<long long>(gb) * args.scale_b_group_stride + n : nullptr;
+              const float* sb2 = args.scale_b2 != nullptr ? args.scale_b2 + static_cast<long long>(gb) * args.scale_b_group_stride + n : nullptr;
+#pragma unroll
+              for (int j = 0; j < 32; ++j) {
+                g[j] *= (sb != nullptr && j < ncols) ? sa * sb[j] : sa;
+                u[j] *= (sb2 != nullptr && j < ncols) ? sa * sb2[j] : sa;
+              }
+            }
+            if (d2_row != nullptr) {       // training: keep the pre-activations for the backward pass
+              store_seg(d2_row, n, ncols, g);
+              store_seg(d3_row, n, ncols, u);
+            }
+            if (args.act == ACT_RELU) glu_fwd_seg<ACT_RELU>(g, u, o);
+            else if (args.act == ACT_GELU) glu_fwd_seg<ACT_GELU>(g, u, o);
+            else glu_fwd_seg<ACT_SILU>(g, u, o);
+            store_seg(d_row, n, ncols, o);
+          } else {
+            float dh[32];
+            load_acc(col, dh);
+            if (args.scale_a != nullptr || args.scale_b != nullptr) {     // fp8 operands: dh = acc * sa[m] * sb[n]
+              const float* sb = args.scale_b != nullptr ? args.scale_b + static_cast<long long>(gb) * args.scale_b_group_stride + n : nullptr;
+#pragma unroll
+              for (int j = 0; j < 32; ++j) dh[j] *= (sb != nullptr && j < ncols) ? sa * sb[j] : sa;
+            }
+            load_seg16(aux_row, n, ncols, g);
+            load_seg16(aux2_row, n, ncols, u);
+            if (args.act == ACT_RELU) glu_bwd_seg<ACT_RELU>(dh, g, u, o);
+            else if (args.act == ACT_GELU) glu_bwd_seg<ACT_GELU>(dh, g, u, o);
+            else glu_bwd_seg<ACT_SILU>(dh, g, u, o);
+            store_seg(d_row, n, ncols, o);
+            store_seg(d2_row, n, ncols, u);
+          }
+        }
+      } else {
+#pragma unroll 1
+      for (int c = 0; c < BN / 64; ++c) {
+        const int col = c * 64 + col_half;
+        const int n = tc.n_blk * BN + col;
+        float v[32];
+        load_acc(col, v);
+        const int ncols = min(32, args.N - n);  // multiple of 8, <= 0 past the last column
+        if (args.scale_a != nullptr || args.scale_b != nullptr) {
+          // fp8 operands were quantised with one scale per A row and per B column: D = acc * sa[m] * sb[n]
+          const float sa = (args.scale_a != nullptr && row_ok)
+                               ? args.scale_a[static_cast<long long>(tc.g) * args.scale_a_group_stride + m] : 1.0f;
+          const float* sb = args.scale_b != nullptr ? args.scale_b + static_cast<long long>(gb) * args.scale_b_group_stride + n : nullptr;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] *= (sb != nullptr && j < ncols) ? sa * sb[j] : sa;
+        }
+
+        if (args.epilogue == EPI_NONE) {
+          if (args.alpha != 1.0f) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] *= args.alpha;
+          }
+        } else if (args.epilogue == EPI_RELU_BWD || args.epilogue == EPI_ADD || args.epilogue == EPI_ACT_BWD) {
+          float f[32];
+          load_seg16(aux_row, n, ncols, f);
+          if (args.epilogue == EPI_RELU_BWD) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = f[j] > 0.0f ? v[j] : 0.0f;
+          } else if (args.epilogue == EPI_ADD) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] += f[j];
+          } else if (args.act == ACT_GELU) {      // f = pre-activation: d/dx [x * Phi(x)] = Phi(x) + x * phi(x)
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              const float cdf = 0.5f * (1.0f + erff(f[j] * 0.70710678118654752f));
+              v[j] *= cdf + f[j] * 0.3989422804014327f * __expf(-0.5f * f[j] * f[j]);
+            }
+          } else if (args.act == ACT_SILU) {      // d/dx [x * s(x)] = s(x) * (1 + x * (1 - s(x)))
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              const float sg = fast_sigmoid(f[j]);
+              v[j] *= sg * (1.0f + f[j] * (1.0f - sg));
+            }
+          } else {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = f[j] > 0.0f ? v[j] : 0.0f;
+          }
+        } else {
+          if (bias_g != nullptr) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              if (q * 8 < ncols) {
+                float f[8];
+                if (args.bias_is_fp32) {
+                  const float4 b0 = *reinterpret_cast<const float4*>(bias_g + (n + q * 8) * 4);
+                  const float4 b1 = *reinterpret_cast<const float4*>(bias_g + (n + q * 8 + 4) * 4);
+                  f[0] = b0.x; f[1] = b0.y; f[2] = b0.z; f[3] = b0.w;
+                  f[4] = b1.x; f[5] = b1.y; f[6] = b1.z; f[7] = b1.w;
+                } else {
+                  unpack8(*reinterpret_cast<const uint4*>(bias_g + (n + q * 8) * 2), args.bias_is_bf16 != 0, f);
+                }
+#pragma unroll
+                for (int j = 0; j < 8; ++j) v[q * 8 + j] += f[j];
+              }
+            }
+          }
+          if (args.d2 != nullptr && (args.epilogue == EPI_BIAS_GELU || args.epilogue == EPI_BIAS_SILU)) {
+            // training: the backward pass needs the pre-activation (ReLU gets by with the sign of its output)
+            uint8_t* d2_row = reinterpret_cast<uint8_t*>(args.d2) +
+                              (static_cast<long long>(tc.g) * args.d_group_stride + static_cast<long long>(m) * args.ldd) * 2;
+            store_seg(d2_row, n, ncols, v);
+          }
+          if (args.epilogue == EPI_BIAS_RELU) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.0f);
+          } else if (args.epilogue == EPI_BIAS_GELU) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
+          } else if (args.epilogue == EPI_BIAS_SILU) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = silu(v[j]);
+          }
+        }
+
+        if (args.colsum != nullptr) {
+          // Bias gradient fused into the epilogue: transpose-reduce each half-warp's 16 rows x 32 columns with 30
+          // shuffles (afterwards lane l holds the sums of columns 2 (l % 16) + {0, 1}) and add them to the fp32
+          // accumulator in global memory.
+          float s[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) s[j] = row_ok ? v[j] : 0.0f;
+#pragma unroll
+          for (int off = 8; off >= 1; off >>= 1) {
+            const bool upper = (lane & off) != 0;
+#pragma unroll
+            for (int i = 0; i < 2 * off; ++i) {
+              const float send = upper ? s[i] : s[i + 2 * off];
+              const float recv = __shfl_xor_sync(0xffffffffu, send, off);
+              s[i] = (upper ? s[i + 2 * off] : s[i]) + recv;
+            }
+          }
+          const int cc = 2 * (lane & 15);
+          float* cs = args.colsum + static_cast<long long>(gb) * args.colsum_group_stride + n + cc;
+          if (cc < ncols) {
+            atomicAdd(cs, s[0]);
+            atomicAdd(cs + 1, s[1]);
+          }
+        }
+        store_seg(d_row, n, ncols, v);
+      }
+      }
+      __syncwarp();   // every lane has read its row before the next tile's fragment overwrites the staging rows
+      if (args.signal_ptr_table != nullptr) {
+        // Combine fusion: all 256 consumer threads' (possibly remote) stores -> one release.sys counter bump.
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (cw == 0 && lane == 0) {
+          ptx::fence_acq_rel_sys();
+          ptx::red_add_release_sys(reinterpret_cast<uint32_t*>(args.signal_ptr_table[tc.g]), 1u);
+        }
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// host side
+// ------------------------------------------------------------------------------------------------
+using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeTiledFn get_encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  });
+  return fn;
+}
+
+bool make_operand_map(CUtensorMap* map, const void* base, int dtype, bool mn_major, long long rows_mn,
+                      long long k, long long ld, long long group_stride, int groups, int box_mn_kmajor,
+                      const char** why) {
+  EncodeTiledFn enc = get_encode_fn();
+  if (enc == nullptr) { *why = "cuTensorMapEncodeTiled unavailable"; return false; }
+  const int eb = (dtype == DT_E4M3 || dtype == DT_E5M2) ? 1 : 2;
+  CUtensorMapDataType dt = eb == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                   : (dtype == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * eb) & 15) || ((group_stride * eb) & 15)) {
+    *why = "operand base/stride must be 16-byte aligned";
+    return false;
+  }
+  cuuint64_t dims[3];
+  cuuint64_t strides[2];
+  cuuint32_t box[3];
+  cuuint32_t estr[3] = {1, 1, 1};
+  const cuuint32_t row_elems = kSwizzleBytes / eb;
+  if (!mn_major) {
+    dims[0] = static_cast<cuuint64_t>(k); dims[1] = static_cast<cuuint64_t>(rows_mn);
+    box[0] = row_elems; box[1] = static_cast<cuuint32_t>(box_mn_kmajor);
+  } else {
+    dims[0] = static_cast<cuuint64_t>(rows_mn); dims[1] = static_cast<cuuint64_t>(k);
+    box[0] = row_elems; box[1] = row_elems;  // BK k-rows x one 128-byte MN chunk
+  }
+  dims[2] = static_cast<cuuint64_t>(groups);
+  box[2] = 1;
+  strides[0] = static_cast<cuuint64_t>(ld) * eb;
+  strides[1] = static_cast<cuuint64_t>(groups > 1 ? group_stride : (mn_major ? k : rows_mn) * ld) * eb;
+  if (strides[1] == 0) strides[1] = strides[0];
+  CUresult r = enc(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { *why = "cuTensorMapEncodeTiled failed"; return false; }
+  return true;
+}
+
+template <bool A_MN, bool B_MN, int DT>
+cudaError_t launch_inst(const CUtensorMap& ta, const CUtensorMap& tb_, const CUtensorMap& tb2, const GemmArgs& args,
+                        int grid, cudaStream_t stream) {
+  auto* kern = gemm_sm90_kernel<A_MN, B_MN, DT>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  kern<<<grid, kThreads, Cfg::SMEM_BYTES, stream>>>(ta, tb_, tb2, args);
+  return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const char** why_out) {
+  const char* why_local = nullptr;
+  const char** why = why_out ? why_out : &why_local;
+  *why = nullptr;
+  if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.G <= 0) return cudaSuccess;
+  const int eb = (p.in_dtype == DT_E4M3 || p.in_dtype == DT_E5M2) ? 1 : 2;
+  if (p.N % 8 != 0) { *why = "N must be a multiple of 8"; return cudaErrorInvalidValue; }
+  const int ob = p.out_dtype == DT_FP32 ? 4 : 2;
+  if ((reinterpret_cast<uintptr_t>(p.d) & 15) || ((p.ldd * ob) & 15) || ((p.d_group_stride * ob) & 15)) {
+    *why = "output base/stride must be 16-byte aligned";
+    return cudaErrorInvalidValue;
+  }
+
+  int dev = 0;
+  cudaGetDevice(&dev);
+  static int sm_count_cache[64] = {0};
+  if (sm_count_cache[dev & 63] == 0) cudaDeviceGetAttribute(&sm_count_cache[dev & 63], cudaDevAttrMultiProcessorCount, dev);
+  int sms = sm_count_cache[dev & 63];
+  if (p.max_ctas > 0) sms = p.max_ctas < sms ? p.max_ctas : sms;
+
+  const bool dual = p.epilogue == EPI_GLU;
+  if (dual && (p.b2 == nullptr || p.out_dtype == DT_FP32)) { *why = "EPI_GLU needs b2 and a 16-bit output"; return cudaErrorInvalidValue; }
+  if (p.epilogue == EPI_GLU_BWD && (p.aux == nullptr || p.aux2 == nullptr || p.d2 == nullptr || p.out_dtype == DT_FP32)) {
+    *why = "EPI_GLU_BWD needs aux, aux2, d2 and a 16-bit output";
+    return cudaErrorInvalidValue;
+  }
+  if ((p.epilogue == EPI_GLU || p.epilogue == EPI_GLU_BWD) && p.d_ptr_table != nullptr) { *why = "GLU epilogues write local outputs only"; return cudaErrorInvalidValue; }
+  const bool uses_aux = p.epilogue == EPI_RELU_BWD || p.epilogue == EPI_ADD || p.epilogue == EPI_GLU_BWD || p.epilogue == EPI_ACT_BWD;
+  if (uses_aux && (p.aux == nullptr || p.out_dtype == DT_FP32 ||
+                   ((reinterpret_cast<uintptr_t>(p.aux) | reinterpret_cast<uintptr_t>(p.aux2)) & 15) || ((p.ld_aux * 2) & 15) ||
+                   ((p.aux_group_stride * 2) & 15))) {
+    *why = "this epilogue needs a 16-byte aligned 16-bit aux operand";
+    return cudaErrorInvalidValue;
+  }
+  if (p.cta_group < 0 || p.cta_group > 2) { *why = "cta_group must be 0, 1 or 2"; return cudaErrorInvalidValue; }
+  if (p.block_n != 0 && p.block_n != 128 && p.block_n != 256) { *why = "block_n must be 0, 128 or 256"; return cudaErrorInvalidValue; }
+
+  constexpr int bm = Cfg::BM, bn = Cfg::BN;
+  GemmArgs a{};
+  a.M = p.M; a.N = p.N; a.K = p.K; a.G = p.G;
+  a.b_group_div = p.b_group_div > 0 ? p.b_group_div : 1;
+  a.tiles_m = (p.M + bm - 1) / bm;
+  a.tiles_n = dual ? (p.N + bn / 2 - 1) / (bn / 2) : (p.N + bn - 1) / bn;
+  a.num_tiles = static_cast<long long>(a.tiles_m) * a.tiles_n * p.G;
+  a.d = p.d; a.ldd = p.ldd; a.d_group_stride = p.d_group_stride; a.d_ptr_table = p.d_ptr_table;
+  a.out_dtype = p.out_dtype;
+  a.epilogue = p.epilogue; a.alpha = p.alpha;
+  a.bias = p.bias; a.bias_group_stride = p.bias_group_stride; a.bias_is_fp32 = 0;
+  a.bias_is_bf16 = (eb == 2) ? (p.in_dtype == DT_BF16) : (p.out_dtype == DT_BF16);
+  a.aux = p.aux; a.ld_aux = p.ld_aux; a.aux_group_stride = p.aux_group_stride;
+  a.aux2 = p.aux2; a.d2 = p.d2; a.d3 = p.d3; a.dual = dual ? 1 : 0; a.act = p.act; a.scale_b2 = p.scale_b2;
+  a.row_counts = p.row_counts;
+  a.colsum = p.colsum; a.colsum_group_stride = p.colsum_group_stride;
+  a.scale_a = p.scale_a; a.scale_a_group_stride = p.scale_a_group_stride;
+  a.scale_b = p.scale_b; a.scale_b_group_stride = p.scale_b_group_stride;
+  a.wait_flags = p.wait_flags; a.wait_rows_per_flag = p.wait_rows_per_flag > 0 ? p.wait_rows_per_flag : bm;
+  a.wait_flags_per_group = p.wait_flags_per_group; a.wait_target = p.wait_target;
+  a.signal_ptr_table = p.signal_ptr_table;
+  a.group_rot = p.group_rot; a.group_mod = p.group_mod;
+
+  CUtensorMap ta, tb_;
+  const int gB = (p.G + a.b_group_div - 1) / a.b_group_div;
+  if (!make_operand_map(&ta, p.a, p.in_dtype, p.a_mn_major, p.M, p.K, p.lda, p.a_group_stride, p.G, bm, why))
+    return cudaErrorInvalidValue;
+  const int b_box = dual ? bn / 2 : bn;
+  if (!make_operand_map(&tb_, p.b, p.in_dtype, p.b_mn_major, p.N, p.K, p.ldb, p.b_group_stride, gB, b_box, why))
+    return cudaErrorInvalidValue;
+  CUtensorMap tb2 = tb_;
+  if (dual && !make_operand_map(&tb2, p.b2, p.in_dtype, p.b_mn_major, p.N, p.K, p.ldb, p.b_group_stride, gB, b_box, why))
+    return cudaErrorInvalidValue;
+
+  const int grid = static_cast<int>(a.num_tiles < sms ? a.num_tiles : sms);
+
+  if (eb == 1) {
+    if (p.a_mn_major || p.b_mn_major) { *why = "fp8 operands must be K-major"; return cudaErrorInvalidValue; }
+    const bool xact = p.epilogue == EPI_BIAS_GELU || p.epilogue == EPI_BIAS_SILU || p.epilogue == EPI_ACT_BWD;
+    if (xact) { *why = "GELU / SiLU epilogues need 16-bit operands"; return cudaErrorInvalidValue; }
+    if (p.in_dtype == DT_E4M3) return launch_inst<false, false, DT_E4M3>(ta, tb_, tb2, a, grid, stream);
+    return launch_inst<false, false, DT_E5M2>(ta, tb_, tb2, a, grid, stream);
+  }
+#define TB_SWITCH_MAJOR(DTv)                                                                                   \
+  do {                                                                                                         \
+    if (!p.a_mn_major && !p.b_mn_major) return launch_inst<false, false, DTv>(ta, tb_, tb2, a, grid, stream);   \
+    if (!p.a_mn_major && p.b_mn_major) return launch_inst<false, true, DTv>(ta, tb_, tb2, a, grid, stream);     \
+    if (p.a_mn_major && !p.b_mn_major) return launch_inst<true, false, DTv>(ta, tb_, tb2, a, grid, stream);     \
+    return launch_inst<true, true, DTv>(ta, tb_, tb2, a, grid, stream);                                        \
+  } while (0)
+  if (p.in_dtype == DT_BF16) TB_SWITCH_MAJOR(DT_BF16);
+  if (p.in_dtype == DT_FP16) TB_SWITCH_MAJOR(DT_FP16);
+#undef TB_SWITCH_MAJOR
+  *why = "unsupported operand dtype";
+  return cudaErrorInvalidValue;
+}
+
+// run-time spin-wait limit of this translation unit's kernels (ptx.cuh)
+cudaError_t set_spin_timeout_gemm(unsigned long long ns) {
+  return cudaMemcpyToSymbol(tb_spin_timeout_ns, &ns, sizeof(ns));
+}
+
+}  // namespace tb
+

@@ -1,4 +1,4 @@
-// Routing and sparse dispatch/combine kernels for sm_100a.
+// Routing and sparse dispatch/combine kernels for sm_90a.
 //
 // Functional counterpart of the reference's SIMT JIT kernels (tutel/jit_kernels/sparse.py:17-134), its
 // `tutel_ops.cumsum` Blelloch scan (tutel/custom/custom_kernel.cpp:822-872) and the ~15 small torch kernels of
@@ -194,7 +194,7 @@ __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return
 // encode: slot-centric row gather (+ optional remote push and release counters)
 // ------------------------------------------------------------------------------------------------
 constexpr int kEncThreads = 256;      // local gather
-constexpr int kEncPushThreads = 128;  // remote push: 128 x 64 registers fit next to a resident GEMM CTA (gemm_sm100.cu)
+constexpr int kEncPushThreads = 128;  // remote push: 128 x 64 registers fit next to a resident GEMM CTA (gemm_sm90.cu)
 
 template <typename T, bool VEC, int THREADS>
 __global__ void __launch_bounds__(THREADS, 65536 / (THREADS * 64))
@@ -396,7 +396,7 @@ gate_grad_kernel(const T* __restrict__ a, const T* __restrict__ buf, const int* 
 }
 
 // ------------------------------------------------------------------------------------------------
-// per-row e4m3 quantisation (activations / K-major weights for the fp8 tcgen05 GEMM): one warp per row
+// per-row e4m3 quantisation (activations / K-major weights for the fp8 wgmma GEMM): one warp per row
 // ------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256)

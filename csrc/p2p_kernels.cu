@@ -1,4 +1,4 @@
-// Peer-to-peer collectives written as plain CUDA kernels over NVLink-mapped memory: the B200-native replacement
+// Peer-to-peer collectives written as plain CUDA kernels over NVLink-mapped memory: the H100-native replacement
 // for the reference's grouped ncclSend/ncclRecv all-to-alls (tutel/custom/custom_kernel.cpp:463-518, 520-654)
 // and c10d all_to_all_single (tutel/impls/communicate.py:181-192).  One launch = handshake + payload + completion:
 //
@@ -20,7 +20,7 @@ namespace tb {
 namespace {
 
 constexpr int kPushThreadsBig = 512;
-constexpr int kPushThreadsSmall = 128;   // 128 threads x <= 64 registers: fits next to a resident persistent GEMM CTA (gemm_sm100.cu)
+constexpr int kPushThreadsSmall = 128;   // 128 threads x <= 64 registers: fits next to a resident persistent GEMM CTA (gemm_sm90.cu)
 
 template <int kPushThreads>
 __global__ void __launch_bounds__(kPushThreads, kPushThreads == 128 ? 8 : 1)

@@ -1,4 +1,4 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM),
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma,
 // cluster helpers and system-scope acquire/release primitives used by the cross-GPU protocols.
 // Everything here is written against the PTX ISA for CUDA 12.9; nothing is borrowed from CUTLASS.
 #pragma once
@@ -97,6 +97,16 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// Same bound, no message: for kernels that issue wgmma (ptxas serialises the MMAs of a kernel that contains a call,
+// and printf is one).
+__device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const uint64_t t0 = globaltimer_ns();
+  while (!mbar_try_wait(bar, parity)) {
+    if (globaltimer_ns() - t0 > tb_spin_timeout_ns) __trap();
+  }
+}
+
 // ----------------------------------------------------------------------------------------------
 // proxies / fences
 // ----------------------------------------------------------------------------------------------
@@ -166,6 +176,16 @@ __device__ __forceinline__ void wait_flag_ge_sys(const uint32_t* p, uint32_t tar
   }
 }
 
+// Same without the message (see mbar_wait_quiet), for kernels that issue wgmma.
+__device__ __forceinline__ void wait_flag_ge_sys_quiet(const uint32_t* p, uint32_t target) {
+  if (static_cast<int32_t>(ld_acquire_sys(p) - target) >= 0) return;
+  const uint64_t t0 = globaltimer_ns();
+  while (static_cast<int32_t>(ld_acquire_sys(p) - target) < 0) {
+    __nanosleep(64);
+    if (globaltimer_ns() - t0 > tb_spin_timeout_ns) __trap();
+  }
+}
+
 // 16-byte streaming global access (peer or local); keeps L1 clean for one-touch data.
 __device__ __forceinline__ uint4 ld_nc_v4(const void* p) {
   uint4 r;
@@ -201,17 +221,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const void* tmap,
       "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// Same, for a CTA pair: data lands in this CTA's smem, bytes are credited to the LEADER CTA's mbarrier
-// (bit 24 of a shared::cluster address selects the odd CTA of the pair).
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t smem_dst, const void* tmap, uint32_t bar, int c0, int c1,
-                                                int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_dst),
-      "l"(tmap), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-
 // Ask the L2 to fetch `bytes` (multiple of 16) starting at a 16-byte aligned global address.
 __device__ __forceinline__ void prefetch_l2_bulk(const void* gptr, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gptr), "r"(bytes) : "memory");
@@ -225,107 +234,54 @@ __device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads
+// wgmma: warpgroup-wide asynchronous MMA, operands in shared memory, fp32 accumulator fragment in registers.
+// One m64n128 instruction leaves 64 floats per thread: d[4j + {0,1}] = row (warp % 4) * 16 + lane / 4, columns
+// 8j + 2 * (lane % 4) + {0,1};  d[4j + {2,3}] = the same columns eight rows further down.
 // ----------------------------------------------------------------------------------------------
-template <int CG>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  }
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers fp16 and bf16 inputs with fp32 accumulation.
-template <int CG>
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  if constexpr (CG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-// kind::f8f6f4: e4m3/e5m2 inputs (plain, not block-scaled), fp32 accumulation, K = 32 per instruction.
-template <int CG>
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  if constexpr (CG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
+enum WgmmaType : int { WG_BF16 = 0, WG_FP16 = 1, WG_E4M3 = 3, WG_E5M2 = 4 };   // values of tb::GemmDtype
 
-// Make `bar` (this CTA, or both CTAs of the pair when CG==2) observe completion of all MMAs issued so far.
-template <int CG>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
-  } else {
-    const uint16_t mask = 0x3;
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            bar),
-        "h"(mask)
-        : "memory");
-  }
-}
+#define TB_ACC8(d, o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+#define TB_ACC64(d) TB_ACC8(d, 0), TB_ACC8(d, 8), TB_ACC8(d, 16), TB_ACC8(d, 24), TB_ACC8(d, 32), TB_ACC8(d, 40), TB_ACC8(d, 48), TB_ACC8(d, 56)
+#define TB_D64 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define TB_WGMMA16(TYPES)                                                                                       \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPES " " TB_D64 ", %64, %65, p, 1, 1, %67, %68;\n\t}\n" \
+               : TB_ACC64(d)                                                                                    \
+               : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA ? 1 : 0), "n"(TB ? 1 : 0))
+#define TB_WGMMA8(TYPES)                                                                                        \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n128k32.f32." TYPES " " TB_D64 ", %64, %65, p, 1, 1;\n\t}\n"      \
+               : TB_ACC64(d)                                                                                    \
+               : "l"(adesc), "l"(bdesc), "r"(accumulate))
 
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread t owns TMEM lane base+t).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// d (+)= A[64 x K] * B[K x 128], K = 16 (16-bit types) or 32 (8-bit types, K-major only).  TA / TB: the operand is
+// MN-major in shared memory (16-bit types only).
+template <int T, bool TA, bool TB>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  static_assert(T == WG_BF16 || T == WG_FP16 || (!TA && !TB), "8-bit operands are K-major only");
+  if constexpr (T == WG_BF16) TB_WGMMA16("bf16.bf16");
+  else if constexpr (T == WG_FP16) TB_WGMMA16("f16.f16");
+  else if constexpr (T == WG_E4M3) TB_WGMMA8("e4m3.e4m3");
+  else TB_WGMMA8("e5m2.e5m2");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+#undef TB_WGMMA16
+#undef TB_WGMMA8
+#undef TB_D64
+#undef TB_ACC64
+#undef TB_ACC8
+
+template <int NREG> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(NREG)); }
+template <int NREG> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(NREG)); }
 
 // ----------------------------------------------------------------------------------------------
-// UMMA shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle.
+// wgmma shared-memory matrix descriptor, 128-byte swizzle.
 //   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1      bits [61,64) layout (2 = SWIZZLE_128B)
+//   bits [32,46) stride byte offset >> 4 bits [62,64) layout (1 = SWIZZLE_128B)
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
                                                          uint32_t sbo_bytes) {
@@ -333,8 +289,7 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uin
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 

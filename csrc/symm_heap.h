@@ -1,5 +1,5 @@
 // Symmetric heap: one cudaMalloc'd arena per rank, exported with CUDA IPC and mapped into every peer process on the
-// node, so that kernels can address any rank's buffers directly over NVLink.  B200-native replacement for the
+// node, so that kernels can address any rank's buffers directly over NVLink.  H100-native replacement for the
 // reference's private NCCL communicators (tutel/custom/custom_kernel.cpp:327-431).
 #pragma once
 #include <cstddef>

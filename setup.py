@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Packaging of tutel_b200.  The native runtime is built ahead of time for sm_100a by tutel_b200/_build.py
+"""Packaging of tutel_b200.  The native runtime is built ahead of time for sm_90a by tutel_b200/_build.py
 (`python setup.py build_ext --inplace` or `pip install -e .` trigger it; set NO_CUDA=1 to skip the CUDA kernels'
 compilation check when nvcc is absent - the pure-PyTorch CPU paths keep working)."""
 import os
@@ -15,7 +15,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 
 def build_native():
     if int(os.environ.get('NO_CUDA', '0')):
-        print('NO_CUDA=1: skipping the native sm_100a extension')
+        print('NO_CUDA=1: skipping the native sm_90a extension')
         return
     sys.path.insert(0, ROOT)
     from tutel_b200 import _build
@@ -50,7 +50,7 @@ class Tester(Command):
 setup(
     name='tutel_b200',
     version='0.1.0',
-    description='B200-native Mixture-of-Experts framework with the capabilities of microsoft/tutel',
+    description='H100-native Mixture-of-Experts framework with the capabilities of microsoft/tutel',
     packages=find_packages(include=['tutel_b200', 'tutel_b200.*']),
     package_data={'tutel_b200': ['_C*.so', 'examples/README.md', 'examples/fairseq_moe/*']},
     python_requires='>=3.9',

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: test needs a CUDA GPU (B200); run with `pytest -m gpu`')
+    config.addinivalue_line('markers', 'gpu: test needs a CUDA GPU (H100); run with `pytest -m gpu`')
 
 
 def pytest_collection_modifyitems(config, items):
@@ -28,16 +28,7 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope='session')
 def golden():
-    """Reference golden loss curves (tests/test_baseline.json of the reference; numbers only, read at test time)."""
+    """Golden loss curves recorded from the reference's helloworld driver (tests/golden/losses.json; numbers only)."""
     import json
-    path = '/root/reference/tests/test_baseline.json'
-    local = os.path.join(ROOT, 'tests', 'golden_losses.json')
-    if os.path.exists(local):
-        with open(local) as f:
-            return json.load(f)
-    if os.path.exists(path):
-        with open(path) as f:
-            data = json.load(f)
-        return [{'top': d['top'], 'dtype': d['dtype'], 'num_local_experts': d['num_local_experts'],
-                 'losses': [float(v) for v in d['losses'][:12]]} for d in data]
-    pytest.skip('golden losses unavailable')
+    with open(os.path.join(ROOT, 'tests', 'golden', 'losses.json')) as f:
+        return json.load(f)

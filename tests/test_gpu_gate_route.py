@@ -1,5 +1,5 @@
 """Fused gate + routing kernels, column sums and the public column scan against plain PyTorch fp32 references
-(csrc/gate_route.cu; run with `pytest -m gpu` on a B200)."""
+(csrc/gate_route.cu; run with `pytest -m gpu` on an H100)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -162,7 +162,7 @@ def test_dropless_layer_without_host_sync_matches_padded_path(monkeypatch):
 
 @pytest.mark.parametrize('act', ['gelu', 'silu', 'relu'])
 def test_fused_act_ffn_matches_autograd(act):
-    """GELU / SiLU experts on the tcgen05 kernel: the forward epilogue also stores the pre-activation, the dgrad epilogue
+    """GELU / SiLU experts on the wgmma kernel: the forward epilogue also stores the pre-activation, the dgrad epilogue
     applies act'(pre) - checked against plain fp32 autograd."""
     from tutel_b200.ops import gemm as G
     torch.manual_seed(12)

@@ -1,4 +1,4 @@
-"""Numerics of every native CUDA kernel against plain PyTorch fp32 references (run with `pytest -m gpu` on a B200)."""
+"""Numerics of every native CUDA kernel against plain PyTorch fp32 references (run with `pytest -m gpu` on an H100)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -251,7 +251,7 @@ def _act(name, t):
 @pytest.mark.parametrize('act', ['silu', 'relu', 'gelu'])
 @pytest.mark.parametrize('M,b_mn', [(96, True), (328, True), (328, False), (1000, True)])
 def test_glu_dual_b_gemm_forward_and_backward_epilogues(C, act, M, b_mn):
-    """h = act(x@W1) * (x@W2) from ONE launch (gate/up halves share a TMEM tile), and the dh GEMM that emits dg/du."""
+    """h = act(x@W1) * (x@W2) from ONE launch (gate/up halves share an accumulator tile), and the dh GEMM that emits dg/du."""
     from tutel_b200.ops import gemm as G
     torch.manual_seed(3)
     Gn, K, N = 2, 264, 328          # N not a multiple of the 128-column half tile
@@ -268,7 +268,7 @@ def test_glu_dual_b_gemm_forward_and_backward_epilogues(C, act, M, b_mn):
     h_only, _, _ = G.glu_gemm(x, b1, b2, b_mn=b_mn, act=act)
     assert torch.equal(h_only, h)
 
-    # backward epilogue: dh = dy @ W3^T stays in TMEM, the epilogue writes dg and du
+    # backward epilogue: dh = dy @ W3^T stays in registers, the epilogue writes dg and du
     Mo = 136
     dy = (torch.randn(Gn, M, Mo, device='cuda') * 0.5).bfloat16()
     w3 = (torch.randn(Gn, N, Mo, device='cuda') * 0.1).bfloat16()

@@ -7,7 +7,7 @@ pytestmark = pytest.mark.gpu
 
 def _need_gpu():
     if not torch.cuda.is_available():
-        pytest.skip('needs a B200')
+        pytest.skip('needs an H100')
 
 
 @pytest.mark.parametrize('shape', [(1, 128, 256), (2, 300, 512), (3, 64, 1024)])
@@ -29,7 +29,7 @@ def test_mx_quantize_kernel_matches_definition(shape, dtype):
 def test_mx_gemm_is_exact_on_exactly_representable_operands(G, M, N, K, bn, cg):
     """Small integers x powers of two: every product and partial sum is exact in fp32, so the tensor-core result must
     equal the fp32 matmul of the dequantised operands bit for bit (after the bf16 rounding of the output) - this pins
-    the scale layout (row -> TMEM lane / column, K block -> byte) and the descriptors."""
+    the scale layout (row / column -> word of the atom, K block -> byte) and the descriptors."""
     _need_gpu()
     from tutel_b200.ops import mx
     g = torch.Generator().manual_seed(M + N)

@@ -1,4 +1,4 @@
-"""MX block-scaled fp8 number format (CPU): the PyTorch definition the sm_100a kernels are tested against."""
+"""MX block-scaled fp8 number format (CPU): the PyTorch definition the sm_90a kernels are tested against."""
 import pytest
 import torch
 

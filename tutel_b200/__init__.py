@@ -1,7 +1,7 @@
-"""tutel_b200 - a B200-native (sm_100a, NVLink 5) Mixture-of-Experts framework with the capabilities and API of
+"""tutel_b200 - a H100-native (sm_90a, NVLink 4) Mixture-of-Experts framework with the capabilities and API of
 microsoft/tutel: ``moe.moe_layer`` with top-k gating and dynamic capacity, switchable DP / EP / sharded-expert
 parallelism, all-to-all / FFN pipelining, 2DH, a dropless Megablocks path, ragged collectives, ZeRO helpers,
-re-shardable checkpoints - built on hand-written tcgen05 / TMA kernels and in-kernel NVLink peer-to-peer transfers.
+re-shardable checkpoints - built on hand-written wgmma / TMA kernels and in-kernel NVLink peer-to-peer transfers.
 
     from tutel_b200 import moe, net, system, jit
     # or, to run code written against the reference unchanged:

@@ -1,8 +1,8 @@
-"""In-tree ahead-of-time build of the native runtime (``tutel_b200/_C*.so``) for sm_100a.
+"""In-tree ahead-of-time build of the native runtime (``tutel_b200/_C*.so``) for sm_90a.
 
 The reference compiles its kernels at run time by fork/exec of nvcc (tutel/custom/custom_kernel.cpp:94-125) and
 builds one C++ extension through setuptools (setup.py:123-130).  Here every kernel is compiled ahead of time with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo`` (cross-compiles without a GPU) and linked into a single
+``-gencode arch=compute_90a,code=sm_90a -lineinfo`` (cross-compiles without a GPU) and linked into a single
 extension that lives next to the Python sources, so it travels to the GPU box with the snapshot.
 
 Usage:  python -m tutel_b200._build [--force] [--verbose]
@@ -23,10 +23,10 @@ BUILD = os.path.join(ROOT, 'build', 'obj')
 EXT_SUFFIX = sysconfig.get_config_var('EXT_SUFFIX') or '.so'
 TARGET = os.path.join(ROOT, 'tutel_b200', '_C' + EXT_SUFFIX)
 
-CUDA_SOURCES = ['gemm_sm100.cu', 'gemm_mx.cu', 'moe_kernels.cu', 'gate_route.cu', 'p2p_kernels.cu', 'skinny_gemm.cu']
+CUDA_SOURCES = ['gemm_sm90.cu', 'gemm_mx.cu', 'moe_kernels.cu', 'gate_route.cu', 'p2p_kernels.cu', 'skinny_gemm.cu']
 CPP_SOURCES = ['bindings.cpp', 'cpu_kernels.cpp', 'symm_heap.cpp', 'jit_nvrtc.cpp']
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '--expt-relaxed-constexpr', '-Xcompiler', '-fPIC', '-DTORCH_EXTENSION_NAME=_C']
 
 
@@ -37,7 +37,7 @@ def _cuda_home():
     nvcc = shutil.which('nvcc')
     if nvcc:
         return os.path.dirname(os.path.dirname(nvcc))
-    raise RuntimeError('nvcc not found: tutel_b200 needs the CUDA toolkit to build its sm_100a kernels')
+    raise RuntimeError('nvcc not found: tutel_b200 needs the CUDA toolkit to build its sm_90a kernels')
 
 
 def _digest(paths, extra=''):

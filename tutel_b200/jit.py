@@ -1,6 +1,6 @@
 """Run-time CUDA kernel creation (mirrors tutel/jit.py:4, tutel/impls/jit_compiler.py:24-55).
 
-The source is compiled with NVRTC for the device's architecture (``sm_100a`` on B200) inside the native runtime
+The source is compiled with NVRTC for the device's architecture (``sm_90a`` on H100) inside the native runtime
 (csrc/jit_nvrtc.cpp); launch extents come from ``// [thread_extent] blockIdx.x = N`` comments exactly like the
 reference's kernel strings, and ``@key@`` placeholders are substituted from ``keyword_dict``.
 """

@@ -6,7 +6,7 @@ dicts, the re-sharding tools and the golden loss curves carry over:
     batched_fc1_w    [El, H/Sh, M]        batched_fc1_bias [El, H/Sh]
     batched_fc2_w    [El, H/Sh, Mout]     batched_fc2_bias [El, ceil(Mout/Sh)]
 
-The compute path differs: on B200 both GEMMs (and their backward GEMMs) run on the tcgen05 grouped kernel with
+The compute path differs: on H100 both GEMMs (and their backward GEMMs) run on the wgmma grouped kernel with
 bias/ReLU fused into the epilogue (:mod:`tutel_b200.ops.gemm`); the dropless "Megablocks" mode passes the per-expert
 token counts to the kernel as a device tensor, so empty row tiles are skipped without the reference's host
 synchronisation (tutel/custom/custom_kernel.cpp:874-889).
@@ -148,7 +148,7 @@ class FusedExpertsNetwork(torch.nn.Module):
             return G.skinny_linear(y, w2, b2, 'kn', row_counts)
         if self.mx and self._act_kind == 'relu' and row_counts is None and MX.can_use_mx(x, w1, w2):
             y = MX.fused_relu_ffn_mx(x, w1, b1, w2, b2)
-        elif self._act_kind in G.FWD_EPILOGUE and G.can_use_tcgen05(x, w1) and G.can_use_tcgen05(x, w2):
+        elif self._act_kind in G.FWD_EPILOGUE and G.can_use_wgmma(x, w1) and G.can_use_wgmma(x, w2):
             if self.fp8 and self._act_kind == 'relu' and x.size(-1) % 16 == 0 and w1.size(1) % 16 == 0:
                 y = G.fused_relu_ffn_fp8(x, w1, b1, w2, b2, row_counts)
             else:

@@ -1,7 +1,7 @@
 """SwiGLU ("LLaMA") experts with flat-sharded parameters (reference: tutel/experts/llama_ffn.py:7-48).
 
 Each of the three matrices is stored as one flat shard of ``ceil(El*M*H / Sh)`` elements per GPU and re-assembled
-over the ``Sh`` sharers each forward (ZeRO-style; gradient = reduce-scatter).  The three GEMMs run on the tcgen05
+over the ``Sh`` sharers each forward (ZeRO-style; gradient = reduce-scatter).  The three GEMMs run on the wgmma
 grouped kernel when the dtype allows.
 """
 import torch
@@ -47,8 +47,8 @@ class LlamaFFNNetwork(torch.nn.Module):
         if x.dim() > 3:
             x = x.reshape(x.size(0), x.size(1), -1)
         kind = G.classify_activation(self.activation_fn)
-        if kind in G.ACT_CODES and G.can_use_tcgen05(x, w1) and w3.size(-1) % 8 == 0:
-            # gate/up GEMMs + activation + multiply in one dual-B tcgen05 launch; backward without elementwise passes
+        if kind in G.ACT_CODES and G.can_use_wgmma(x, w1) and w3.size(-1) % 8 == 0:
+            # gate/up GEMMs + activation + multiply in one dual-B wgmma launch; backward without elementwise passes
             return G.fused_glu_ffn(x, w1, w2, w3, kind, self.fp8 and x.size(-1) % 16 == 0 and w3.size(1) % 16 == 0)
         y1 = G.grouped_linear(x, w1, None, 'kn', fp8=self.fp8)
         y2 = G.grouped_linear(x, w2, None, 'kn', fp8=self.fp8)

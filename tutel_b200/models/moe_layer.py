@@ -8,7 +8,7 @@ loading.  The execution engine underneath is new:
     routing   fused histogram/scan/rank kernels          (ops/routing.py, csrc/moe_kernels.cu)
     dispatch  slot-centric gather, native bf16/fp16      (ops/dispatch.py)
     exchange  in-kernel NVLink peer-to-peer pushes       (parallel/p2p.py)  or NCCL / Gloo
-    experts   tcgen05 grouped GEMMs with fused epilogues (ops/gemm.py, csrc/gemm_sm100.cu)
+    experts   wgmma grouped GEMMs with fused epilogues (ops/gemm.py, csrc/gemm_sm90.cu)
     fused     dispatch+GEMM1 / GEMM2+combine over peer memory, tile-granular flags (parallel/fused.py)
 """
 from __future__ import annotations
@@ -70,7 +70,7 @@ def _parse_parallel_type(parallel_type: str, sharded_count: int, valid_rs):
 
 
 class MOELayer(torch.nn.Module):
-    """Mixture-of-Experts layer with switchable parallelism (B200-native engine)."""
+    """Mixture-of-Experts layer with switchable parallelism (H100-native engine)."""
 
     # ------------------------------------------------------------------------------------------------ statics
     @staticmethod

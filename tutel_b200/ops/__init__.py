@@ -1,1 +1,1 @@
-"""Operator layer: routing, sparse dispatch/combine, grouped expert GEMMs (native sm_100a kernels + CPU paths)."""
+"""Operator layer: routing, sparse dispatch/combine, grouped expert GEMMs (native sm_90a kernels + CPU paths)."""

@@ -1,6 +1,6 @@
 """Loading of the native runtime and kernel-path selection.
 
-On a GPU box the sm_100a extension is mandatory: ops fail loudly instead of silently falling back to eager PyTorch
+On a GPU box the sm_90a extension is mandatory: ops fail loudly instead of silently falling back to eager PyTorch
 (set ``TUTEL_B200_ALLOW_FALLBACK=1`` to permit a fallback, e.g. when debugging on another architecture).
 """
 from __future__ import annotations
@@ -45,7 +45,7 @@ def ext():
 def require_ext():
     _load()
     if _C is None:
-        raise RuntimeError('tutel_b200: the native sm_100a extension (tutel_b200/_C*.so) is missing: %r. '
+        raise RuntimeError('tutel_b200: the native sm_90a extension (tutel_b200/_C*.so) is missing: %r. '
                            'Run `python -m tutel_b200._build`.' % (_ERR,))
     return _C
 
@@ -58,16 +58,16 @@ def allow_fallback() -> bool:
     return bool(int(os.environ.get('TUTEL_B200_ALLOW_FALLBACK', '0')))
 
 
-_SM100 = {}
+_SM90 = {}
 
 
-def is_sm100(device=None) -> bool:
+def is_sm90(device=None) -> bool:
     if not torch.cuda.is_available():
         return False
     idx = torch.cuda.current_device() if device is None or getattr(device, 'index', None) is None else device.index
-    if idx not in _SM100:
-        _SM100[idx] = torch.cuda.get_device_capability(idx)[0] == 10
-    return _SM100[idx]
+    if idx not in _SM90:
+        _SM90[idx] = torch.cuda.get_device_capability(idx) == (9, 0)
+    return _SM90[idx]
 
 
 def has_cuda_ext() -> bool:
@@ -81,13 +81,13 @@ def has_cuda_ext() -> bool:
     return True
 
 
-def use_tcgen05(t: torch.Tensor) -> bool:
-    """Expert GEMMs go to the hand-written tcgen05 kernel for fp16/bf16 CUDA tensors on sm_100."""
+def use_wgmma(t: torch.Tensor) -> bool:
+    """Expert GEMMs go to the hand-written wgmma kernel for fp16/bf16 CUDA tensors on sm_90."""
     if not (t.is_cuda and t.dtype in (torch.bfloat16, torch.float16)):
         return False
-    if os.environ.get('TUTEL_B200_GEMM', 'tcgen05').lower() in ('cublas', 'torch'):
+    if os.environ.get('TUTEL_B200_GEMM', 'wgmma').lower() in ('cublas', 'torch'):
         return False
-    return has_cuda_ext() and is_sm100(t.device)
+    return has_cuda_ext() and is_sm90(t.device)
 
 
 # ---- native launch accounting (bench.py reports it as `gpu_launches`) ----------------------------------------------

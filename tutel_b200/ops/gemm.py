@@ -1,8 +1,8 @@
-"""Grouped expert GEMMs on the hand-written tcgen05 kernel (csrc/gemm_sm100.cu) with autograd.
+"""Grouped expert GEMMs on the hand-written wgmma kernel (csrc/gemm_sm90.cu) with autograd.
 
 The reference runs its experts through ``torch.matmul`` -> cuBLAS (tutel/experts/ffn.py:114-118) followed by separate
 bias / activation kernels.  Here forward, data-gradient and weight-gradient are all launches of one persistent
-tcgen05/TMEM/TMA kernel; bias, ReLU and the ReLU gradient mask are fused into its epilogue, operands are consumed in
+wgmma/TMA kernel; bias, ReLU and the ReLU gradient mask are fused into its epilogue, operands are consumed in
 whatever major-ness they already have (no transposes are materialised).
 
 Shapes (G = groups / local experts):
@@ -89,13 +89,13 @@ def _aligned(*dims: int) -> bool:
     return all(d % 8 == 0 for d in dims)
 
 
-def can_use_tcgen05(x: torch.Tensor, w: torch.Tensor) -> bool:
-    return (backend.use_tcgen05(x) and w.dtype == x.dtype and w.is_cuda and x.dim() == 3 and w.dim() == 3 and
+def can_use_wgmma(x: torch.Tensor, w: torch.Tensor) -> bool:
+    return (backend.use_wgmma(x) and w.dtype == x.dtype and w.is_cuda and x.dim() == 3 and w.dim() == 3 and
             _aligned(x.size(-1), w.size(-1), w.size(-2)))
 
 
 class GroupedLinear(torch.autograd.Function):
-    """y[g] = x[g] @ W[g]^T (+ b)  for ``w_layout == 'nk'``  or  x[g] @ W[g] (+ b)  for ``'kn'`` - all on tcgen05."""
+    """y[g] = x[g] @ W[g]^T (+ b)  for ``w_layout == 'nk'``  or  x[g] @ W[g] (+ b)  for ``'kn'`` - all on wgmma."""
 
     @staticmethod
     def forward(ctx: Any, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], w_layout: str,
@@ -138,7 +138,7 @@ def _zero_tail(t: torch.Tensor, counts: torch.Tensor) -> torch.Tensor:
 def grouped_linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, w_layout: str = 'nk',
                    row_counts: Optional[torch.Tensor] = None, fp8: bool = False) -> torch.Tensor:
     """Batched per-expert linear layer; falls back to ``torch.matmul`` for dtypes/devices the kernel does not cover."""
-    if can_use_tcgen05(x, w) and (bias is None or bias.numel() == w.size(0) * (w.size(1) if w_layout == 'nk' else w.size(2))):
+    if can_use_wgmma(x, w) and (bias is None or bias.numel() == w.size(0) * (w.size(1) if w_layout == 'nk' else w.size(2))):
         b = None if bias is None else bias.reshape(w.size(0), -1)
         fp8 = fp8 and x.size(-1) % 16 == 0
         return GroupedLinear.apply(x, w, b, w_layout, row_counts, fp8)
@@ -410,8 +410,8 @@ def _glu_extra(kw):
 
 def glu_gemm(a, b, b2, *, b_mn, act, save_pre=False, scale_a=None, scale_b=None, scale_b2=None, row_counts=None,
              out_dtype=None, **kw):
-    """h = act(a @ B) * (a @ B2) in ONE tcgen05 launch (each CTA of a pair stages one of the two weight tiles; the
-    gate/up halves meet in the TMEM accumulator).  ``save_pre`` also returns the pre-activations (g, u)."""
+    """h = act(a @ B) * (a @ B2) in ONE wgmma launch (the two weight tiles share one stage of the operand ring; the
+    gate/up halves meet in the accumulator fragment).  ``save_pre`` also returns the pre-activations (g, u)."""
     C = backend.require_ext()
     a, b, b2 = _prep(a), _prep(b), _prep(b2)
     if b2.stride() != b.stride():
@@ -426,7 +426,7 @@ def glu_gemm(a, b, b2, *, b_mn, act, save_pre=False, scale_a=None, scale_b=None,
 
 
 def glu_gemm_bwd(dy, w, g, u, *, b_mn, act, row_counts=None, scale_a=None, scale_b=None, **kw):
-    """(dg, du) for h = act(g) * u with dh = dy @ W formed in TMEM only (never written to memory); dy / W may be e4m3
+    """(dg, du) for h = act(g) * u with dh = dy @ W formed in registers only (never written to memory); dy / W may be e4m3
     with per-row scales."""
     C = backend.require_ext()
     dy, w = _prep(dy), _prep(w)

@@ -1,9 +1,9 @@
 """MX block-scaled fp8 (OCP Microscaling: e4m3 elements, one UE8M0 power-of-two scale per 32 consecutive K elements).
 
-The scales are consumed by the tensor core itself (``tcgen05.mma.kind::mxf8f6f4.block_scale``, csrc/gemm_mx.cu), so the
+The scales are applied to the fp32 partial sum of every 32-element K block (one e4m3 ``wgmma`` each, csrc/gemm_mx.cu), so the
 finer granularity costs no epilogue work.  The reference has no reduced-precision expert path (its experts run
 ``torch.matmul`` in the model dtype, tutel/experts/ffn.py); the framework's fused engine uses the row-scaled e4m3 GEMM of
-csrc/gemm_sm100.cu, this module is the finer-grained alternative for GEMMs whose rows carry outliers.
+csrc/gemm_sm90.cu, this module is the finer-grained alternative for GEMMs whose rows carry outliers.
 
 Everything here also has a pure PyTorch definition (``*_reference``) that runs on CPU: the tests compare the kernels
 against it, and it documents the number format:

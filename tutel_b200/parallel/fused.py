@@ -1,15 +1,15 @@
 """NVLink-fused expert-parallel engine: dispatch+GEMM1 and GEMM2+combine with no separate all-to-all.
 
-This is the B200-native replacement of the reference's ``all_to_all -> experts -> all_to_all`` sequence
+This is the H100-native replacement of the reference's ``all_to_all -> experts -> all_to_all`` sequence
 (tutel/impls/moe_layer.py:329-357) and of its chunked NCCL overlap scheduler (tutel/impls/overlap.py,
 tutel/custom/custom_kernel.cpp:520-654).  Per forward pass and rank (W ranks, El local experts, capacity C):
 
   comm stream   encode kernel: gathers this rank's tokens slot by slot and *stores them straight into the
                 destination expert GPU's receive buffer* ``IN[El, W(src), C, M]`` over NVLink, publishing an
                 epoch flag per row chunk with ``st.release.sys``                       (csrc/moe_kernels.cu)
-  main stream   GEMM1 (tcgen05): its TMA producer ``ld.acquire.sys``-polls the flags of exactly the rows of the
+  main stream   GEMM1 (wgmma): its TMA producer ``ld.acquire.sys``-polls the flags of exactly the rows of the
                 tile it is about to load, so tiles are multiplied as they arrive - own-rank rows first.
-                GEMM2 (tcgen05): the epilogue stores every output tile *directly into the source GPU's* combine
+                GEMM2 (wgmma): the epilogue stores every output tile *directly into the source GPU's* combine
                 buffer ``OUT[E, C, Mout]`` and bumps a ``red.release.sys`` counter per expert.
                 decode kernel: acquires the counters of the experts a token used and sums its k rows.
 
@@ -228,12 +228,9 @@ class FusedEngine:
 
     @staticmethod
     def tile_counts(C: int, N: int):
-        """(cta_group, block_n, completion signals per group) of a combine GEMM over [C, N] outputs.  EVERY CTA signals once
-        per tile it finishes - both CTAs of a pair do (each owns 128 of the tile's 256 rows) - so a group of
-        ceil(C / (128 * cg)) * ceil(N / bn) tiles raises its counter by that number times cg."""
-        cg = 2 if C > 128 else 1
-        bn = 256 if N > 128 else 128
-        return cg, bn, (-(-C // (128 * cg))) * (-(-N // bn)) * cg
+        """(cta_group, block_n, completion signals per group) of a combine GEMM over [C, N] outputs.  A CTA signals once
+        per 128 x 128 tile it finishes, so a group of ceil(C / 128) * ceil(N / 128) tiles raises its counter by that number."""
+        return 1, 128, (-(-C // 128)) * (-(-N // 128))
 
 
 def _engine(transport) -> FusedEngine:
@@ -399,7 +396,7 @@ def _virtual_gates(gates_f32: torch.Tensor, geo: _Geometry) -> torch.Tensor:
 # ----------------------------------------------------------------------------------------------------------------
 def engine_for(layer, x: torch.Tensor, crit, d: int):
     """Return a runnable fused call for this forward, or None when the generic path must be used."""
-    if not _enabled() or not backend.use_tcgen05(x):
+    if not _enabled() or not backend.use_wgmma(x):
         return None
     ex = layer.experts
     from ..models.experts.ffn import FusedExpertsNetwork
@@ -689,7 +686,7 @@ class _FusedGLUMoE(torch.autograd.Function):
         else:
             ev = tx.push(dout, gates_f32 if is_postscore else None, Mo)
             dy_recv = tx.recv_view(Mo)
-            # dh = dy @ W3^T stays in TMEM; the epilogue emits dg and du as the gradient rows arrive
+            # dh = dy @ W3^T stays in registers; the epilogue emits dg and du as the gradient rows arrive
             dg, du = G.glu_gemm_bwd(dy_recv, w3, g, u, b_mn=False, act=act, cta_group=cg, **tx.wait_kwargs())
             if need_dx:
                 ck = tx.combine_kwargs(M)

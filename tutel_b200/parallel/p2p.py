@@ -1,6 +1,6 @@
 """NVLink peer-to-peer transport: symmetric heap + in-kernel collectives.
 
-This is the B200-native counterpart of the reference's private NCCL communicators and grouped ``ncclSend/ncclRecv``
+This is the H100-native counterpart of the reference's private NCCL communicators and grouped ``ncclSend/ncclRecv``
 all-to-alls (tutel/custom/custom_kernel.cpp:327-518).  Every rank owns an arena (``_C.SymmHeap``, CUDA IPC mapped into
 all peers on the node); collectives are single kernels that *store* into the destination GPU's arena over NVLink and
 publish completion with ``red.release.sys`` counters (csrc/p2p_kernels.cu).  ``torch.distributed`` is only used to
