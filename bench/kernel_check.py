@@ -45,6 +45,8 @@ def gemm_cases():
     cases.append(dict(kind='gemm', M=8192, N=8192, K=8192, G=1, a_mn=False, b_mn=False, cg=1, bn=256, perf=True))
     cases.append(dict(kind='fp8', M=16384, N=14336, K=4096, G=1, cg=2))
     cases.append(dict(kind='fp8', M=16384, N=4096, K=14336, G=1, cg=2))
+    # the six GEMMs of one flagship training step, issued as FusedReluFFN issues them
+    cases.append(dict(kind='flagship', G=8, T=2048, D=4096, H=14336, perf=True))
     return cases
 
 
@@ -306,7 +308,74 @@ def run_fp8(c):
                 quantize_GBps=(a.numel() * 3) / tq * 1e-6)
 
 
-RUNNERS = dict(fp8=run_fp8, gemm=run_gemm, route=run_route, dispatch=run_dispatch, gate=run_gate, jit=run_jit)
+def run_flagship(c):
+    """The six expert GEMMs of the flagship step (G experts, T = capacity rows, D = model_dim, H = hidden) with the
+    layouts, epilogues and fused bias gradient of FusedReluFFN.  Each is timed three ways, interleaved round by round:
+    block_n=128 (the 128 x 128 configuration of the fused multi-GPU engine), block_n=0 (the launcher's choice) and
+    torch.matmul on the same operands (matmul only, no epilogue)."""
+    import torch
+    from tutel_b200.ops import gemm as GM
+    Gn, T, D, H = c['G'], c['T'], c['D'], c['H']
+    dev = 'cuda'
+    g = torch.Generator(device=dev).manual_seed(4321)
+    rnd = lambda *s, sc=1.0: (torch.randn(*s, device=dev, generator=g) * sc).bfloat16()
+    x, dy = rnd(Gn, T, D), rnd(Gn, T, D, sc=0.01)
+    w1, w2 = rnd(Gn, H, D, sc=D ** -0.5), rnd(Gn, H, D, sc=H ** -0.5)
+    b1, b2 = rnd(Gn, H, sc=0.1), rnd(Gn, D, sc=0.1)
+    act = GM.raw_gemm(x, w1, epilogue=GM.EPI_BIAS_RELU, bias=b1)
+    db1 = torch.zeros(Gn, H, device=dev)
+    dh = GM.raw_gemm(dy, w2, epilogue=GM.EPI_RELU_BWD, aux=act, colsum=db1)
+    tr = lambda t: t.transpose(1, 2)
+    # name: (M, N, K, native call(block_n, out), torch call(out))
+    calls = {
+        'fc1 bias_relu': (T, H, D, lambda bn, o: GM.raw_gemm(x, w1, epilogue=GM.EPI_BIAS_RELU, bias=b1, out=o, block_n=bn),
+                          lambda o: torch.matmul(x, tr(w1), out=o)),
+        'fc2 bias': (T, D, H, lambda bn, o: GM.raw_gemm(act, w2, b_mn=True, epilogue=GM.EPI_BIAS, bias=b2, out=o, block_n=bn),
+                     lambda o: torch.matmul(act, w2, out=o)),
+        'dh relu_bwd+colsum': (T, H, D, lambda bn, o: GM.raw_gemm(dy, w2, epilogue=GM.EPI_RELU_BWD, aux=act, colsum=db1, out=o,
+                                                                   block_n=bn),
+                               lambda o: torch.matmul(dy, tr(w2), out=o)),
+        'dw2 wgrad': (H, D, T, lambda bn, o: GM.raw_gemm(act, dy, a_mn=True, b_mn=True, out=o, block_n=bn),
+                      lambda o: torch.matmul(tr(act), dy, out=o)),
+        'dx dgrad': (T, D, H, lambda bn, o: GM.raw_gemm(dh, w1, b_mn=True, out=o, block_n=bn),
+                     lambda o: torch.matmul(dh, w1, out=o)),
+        'dw1 wgrad': (H, D, T, lambda bn, o: GM.raw_gemm(dh, x, a_mn=True, b_mn=True, out=o, block_n=bn),
+                      lambda o: torch.matmul(tr(dh), x, out=o)),
+    }
+    ev = lambda: torch.cuda.Event(enable_timing=True)
+    res, ok = {}, True
+    for name, (M, N, K, native, ref) in calls.items():
+        outs = {v: torch.empty(Gn, M, N, device=dev, dtype=torch.bfloat16) for v in ('narrow', 'auto', 'torch')}
+        fns = {'narrow': lambda: native(128, outs['narrow']), 'auto': lambda: native(0, outs['auto']),
+               'torch': lambda: ref(outs['torch'])}
+        for fn in fns.values():
+            fn(); fn()
+        times = {v: [] for v in fns}
+        for _ in range(5):
+            for v, fn in fns.items():
+                s, e = ev(), ev()
+                s.record()
+                for _ in range(4):
+                    fn()
+                e.record()
+                torch.cuda.synchronize()
+                times[v].append(s.elapsed_time(e) / 4)
+        flops = 2.0 * Gn * M * N * K
+        r = {'M': M, 'N': N, 'K': K}
+        for v, ts in times.items():
+            ms = sorted(ts)[len(ts) // 2]
+            r[v + '_ms'] = round(ms, 4)
+            r[v + '_tflops'] = round(flops / ms * 1e-9, 1)
+        # narrow and automatic configurations against each other: same epilogue math, same K order per element
+        na, au = outs['narrow'].float(), outs['auto'].float()
+        r['auto_vs_narrow_rel'] = ((na - au).abs().max() / (na.abs().max() + 1e-6)).item()
+        ok = ok and r['auto_vs_narrow_rel'] < 1e-2 and bool(torch.isfinite(au).all())
+        res[name] = r
+    res['ok'] = ok
+    return res
+
+
+RUNNERS = dict(flagship=run_flagship, fp8=run_fp8, gemm=run_gemm, route=run_route, dispatch=run_dispatch, gate=run_gate, jit=run_jit)
 
 
 def main():

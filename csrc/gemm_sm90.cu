@@ -3,14 +3,16 @@
 // Replaces the reference's cuBLAS `torch.matmul` expert GEMMs (tutel/experts/ffn.py:114-118,
 // tutel/experts/llama_ffn.py:38-41) and its host-synchronised per-expert loop
 // `sparse_bmm_infer` (tutel/custom/custom_kernel.cpp:874-889) with ONE persistent, warp-specialised kernel
-// (384 threads, 128 x 128 output tiles):
+// (384 threads, 128 x 256 output tiles; 128 x 128 for the fused multi-GPU engine, the GLU epilogues and block_n=128,
+// see Cfg and gemm_sm90_launch):
 //
 //   warp 0        TMA producer   cp.async.bulk.tensor (128B swizzle) -> smem ring, mbarrier complete_tx; the other
 //                                three warps of its warpgroup only give their registers away (setmaxnreg)
-//   warps 4..11   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async (m64n128, operands straight from
-//                                the swizzled ring, fp32 accumulator fragment in registers), one stage in flight; a stage is
-//                                handed back to the producer when the wgmma group that read it has retired.
-//                                Epilogue: every warp parks its 16 x 128 fragment in its own shared-memory rows and
+//   warps 4..11   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async (m64n256 / m64n128, operands
+//                                straight from the swizzled ring, fp32 accumulator fragment in registers), one stage in
+//                                flight; a stage is handed back to the producer when the wgmma group that read it has retired.
+//                                Epilogue: every warp parks 16 x 128 of its fragment (one pass per 128 columns) in its
+//                                own shared-memory rows and
 //                                reads it back with one lane per row and 32 consecutive columns per lane, applies the
 //                                fused bias / activation / activation-grad / GLU / bias-grad math in fp32 and writes 64
 //                                contiguous bytes per lane - locally or straight into PEER GPUs' memory plus a
@@ -80,23 +82,38 @@ constexpr int kThreads = 384;        // producer warpgroup + two consumer warpgr
 constexpr int kSwizzleBytes = 128;   // one swizzle row: 64 bf16 / 128 fp8
 constexpr int kSmemLimit = 232448;   // 227 KB
 
+// Two configurations of the same kernel (tiles of BM x BN):
+//   BN 128  4 stages of 32 KB, 144 registers per thread.  The fused multi-GPU engine runs this one (see the resource
+//           budget above gemm_sm90_kernel).
+//   BN 256  m64n256 wgmma per consumer warpgroup (128 fp32 accumulators per thread): 48 KB of operands per 64-deep K
+//           block for twice the FLOPs of a 128 x 128 tile's 32 KB, and each warpgroup's B reads from shared memory
+//           serve 256 instead of 128 columns.  3 stages of 48 KB plus the 68 KB epilogue staging (214 KB), 168
+//           registers per thread (producer warpgroup 40, consumers 232), one CTA per SM.
+template <int BN_>
 struct Cfg {
   static constexpr int BM = 128;
-  static constexpr int BN = 128;
+  static constexpr int BN = BN_;
+  static constexpr bool WIDE = BN_ == 256;
   static constexpr int A_BYTES = BM * kSwizzleBytes;
   static constexpr int B_BYTES = BN * kSwizzleBytes;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // Epilogue staging: per consumer warp 16 accumulator rows of BN floats; 8 floats of padding per row keep the
-  // fragment writes (float2, four rows per half-warp) free of bank conflicts.
-  static constexpr int EPI_PITCH = BN + 8;
+  // Epilogue staging: per consumer warp 16 accumulator rows of 128 floats (the accumulator is staged in passes of 128
+  // columns); 8 floats of padding per row keep the fragment writes (float2, four rows per half-warp) free of bank
+  // conflicts.
+  static constexpr int EPI_COLS = 128;
+  static constexpr int PASSES = BN / EPI_COLS;
+  static constexpr int EPI_PITCH = EPI_COLS + 8;
   static constexpr int EPI_WARP_BYTES = 16 * EPI_PITCH * 4;
   static constexpr int EPI_BYTES = 8 * EPI_WARP_BYTES;
   static constexpr int BAR_BYTES = 512;
-  static constexpr int STAGES = 4;
+  static constexpr int STAGES = WIDE ? 3 : 4;
+  static constexpr int MAXNREG = WIDE ? 168 : 144;
+  static constexpr int CONSUMER_REGS = WIDE ? 232 : 192;   // producer warpgroup: 40
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + BAR_BYTES + EPI_BYTES;
   // 228 KB per SM, 1 KB reserved per resident block: a dispatch block (no shared memory of its own) must still fit
-  static_assert(SMEM_BYTES + 2 * 1024 <= 228 * 1024, "no room for the push kernel");
+  static_assert(WIDE || SMEM_BYTES + 2 * 1024 <= 228 * 1024, "no room for the push kernel");
   static_assert(SMEM_BYTES <= kSmemLimit, "");
+  static_assert(128 * 40 + 256 * CONSUMER_REGS <= 65536 && 384 * MAXNREG <= 65536, "register budget");
 };
 
 struct TileCoord {
@@ -236,11 +253,12 @@ __device__ __forceinline__ void glu_bwd_seg(const float* r, const float* g, floa
 // 228 KB shared memory, so ONE 128-thread x 64-register block of the dispatch kernel (encode_rows, which needs no
 // shared memory) always fits next to a GEMM CTA.  That is what makes the dispatch+GEMM fusion deadlock-free: a GEMM
 // whose producer spins on arrival flags can never starve the kernel that publishes them, whichever gets the SMs first.
-template <bool A_MN, bool B_MN, int DT>
-__global__ void __maxnreg__(144)
+// (This is the BN = 128 configuration; the BN = 256 one takes the whole SM and is never used by the fused engine.)
+template <int BN_, bool A_MN, bool B_MN, int DT>
+__global__ void __maxnreg__(Cfg<BN_>::MAXNREG)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmB2, const GemmArgs args) {
-  using C = Cfg;
+  using C = Cfg<BN_>;
   constexpr int BN = C::BN;
   extern __shared__ uint8_t smem_raw[];
 
@@ -279,7 +297,9 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const long long tile_step = gridDim.x;
   const long long tile_first = blockIdx.x;
   constexpr int kBand = 16;
-  const bool dual = args.dual != 0;
+  // The GLU epilogues run on the 128 x 128 configuration only: with 64 accumulator columns still in registers, their
+  // 32-column gate / up / gradient segments do not fit the consumers' 232 registers.
+  const bool dual = !C::WIDE && args.dual != 0;
   const int tile_n = dual ? BN / 2 : BN;   // output columns per tile
 
   if (warp < 4) {
@@ -360,7 +380,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   } else {
-    ptx::setmaxnreg_inc<192>();
+    ptx::setmaxnreg_inc<C::CONSUMER_REGS>();
     // =============================== consumers: wgmma main loop + epilogue ===============================
     const int cw = warp - 4;          // consumer warp 0..7 owns tile rows [16 cw, 16 cw + 16)
     const int wg = cw >> 2;           // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
@@ -382,7 +402,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
     const bool out16 = (args.out_dtype != DT_FP32);
     const bool out_bf16 = (args.out_dtype == DT_BF16);
-    const bool glu = args.epilogue == EPI_GLU || args.epilogue == EPI_GLU_BWD;
+    const bool glu = !C::WIDE && (args.epilogue == EPI_GLU || args.epilogue == EPI_GLU_BWD);
     // Epilogue geometry: lane l works on accumulator row (l % 16) of this warp and on 32 consecutive columns, the
     // lower half-warp on the first and the upper half-warp on the second half of every 64-column chunk.
     float* epi_warp = epi_ptr + cw * 16 * C::EPI_PITCH;
@@ -405,7 +425,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (tc.m_blk * C::BM >= m_valid) continue;
       }
       // ------------------------------- main loop -------------------------------
-      float acc[64];
+      float acc[BN / 2];
       int prev_s = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         ptx::mbar_wait_quiet(full_bar(s), ph);
@@ -416,7 +436,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int k = 0; k < 4; ++k) {
           const uint64_t ad = (static_cast<uint64_t>(desc_hi) << 32) | (a_lo + k * a_kstep);
           const uint64_t bd = (static_cast<uint64_t>(desc_hi) << 32) | (b_lo + k * b_kstep);
-          ptx::wgmma_m64n128<DT, A_MN, B_MN>(acc, ad, bd, (kb | k) != 0);
+          if constexpr (BN == 256) ptx::wgmma_m64n256<DT, A_MN, B_MN>(acc, ad, bd, (kb | k) != 0);
+          else ptx::wgmma_m64n128<DT, A_MN, B_MN>(acc, ad, bd, (kb | k) != 0);
         }
         ptx::wgmma_commit();
         if (kb > 0) {
@@ -430,12 +451,17 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (wg_leader) ptx::mbar_arrive(empty_bar(prev_s));
 
       // ------------------------------- epilogue -------------------------------
+      // The accumulator goes through the staging rows in passes of EPI_COLS columns: pass p stages columns
+      // [128 p, 128 p + 128) and runs the segment epilogue on them (the GLU epilogues: one pass, 128 x 128 only).
+#pragma unroll
+      for (int pass = 0; pass < C::PASSES; ++pass) {
       {
         const int fr = lane >> 2, fc = (lane & 3) * 2;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          *reinterpret_cast<float2*>(epi_warp + fr * C::EPI_PITCH + j * 8 + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(epi_warp + (fr + 8) * C::EPI_PITCH + j * 8 + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        for (int jj = 0; jj < C::EPI_COLS / 8; ++jj) {
+          const int j = pass * (C::EPI_COLS / 8) + jj;
+          *reinterpret_cast<float2*>(epi_warp + fr * C::EPI_PITCH + jj * 8 + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(epi_warp + (fr + 8) * C::EPI_PITCH + jj * 8 + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
       }
       __syncwarp();
@@ -546,9 +572,9 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       } else {
 #pragma unroll 1
-      for (int c = 0; c < BN / 64; ++c) {
+      for (int c = 0; c < C::EPI_COLS / 64; ++c) {
         const int col = c * 64 + col_half;
-        const int n = tc.n_blk * BN + col;
+        const int n = tc.n_blk * BN + pass * C::EPI_COLS + col;
         float v[32];
         load_acc(col, v);
         const int ncols = min(32, args.N - n);  // multiple of 8, <= 0 past the last column
@@ -655,7 +681,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         store_seg(d_row, n, ncols, v);
       }
       }
-      __syncwarp();   // every lane has read its row before the next tile's fragment overwrites the staging rows
+      __syncwarp();   // every lane has read its row before the next pass / tile overwrites the staging rows
+      }
       if (args.signal_ptr_table != nullptr) {
         // Combine fusion: all 256 consumer threads' (possibly remote) stores -> one release.sys counter bump.
         asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -723,17 +750,17 @@ bool make_operand_map(CUtensorMap* map, const void* base, int dtype, bool mn_maj
   return true;
 }
 
-template <bool A_MN, bool B_MN, int DT>
+template <int BN, bool A_MN, bool B_MN, int DT>
 cudaError_t launch_inst(const CUtensorMap& ta, const CUtensorMap& tb_, const CUtensorMap& tb2, const GemmArgs& args,
                         int grid, cudaStream_t stream) {
-  auto* kern = gemm_sm90_kernel<A_MN, B_MN, DT>;
+  auto* kern = gemm_sm90_kernel<BN, A_MN, B_MN, DT>;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES);
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  kern<<<grid, kThreads, Cfg::SMEM_BYTES, stream>>>(ta, tb_, tb2, args);
+  kern<<<grid, kThreads, Cfg<BN>::SMEM_BYTES, stream>>>(ta, tb_, tb2, args);
   return cudaGetLastError();
 }
 
@@ -776,7 +803,13 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
   if (p.cta_group < 0 || p.cta_group > 2) { *why = "cta_group must be 0, 1 or 2"; return cudaErrorInvalidValue; }
   if (p.block_n != 0 && p.block_n != 128 && p.block_n != 256) { *why = "block_n must be 0, 128 or 256"; return cudaErrorInvalidValue; }
 
-  constexpr int bm = Cfg::BM, bn = Cfg::BN;
+  // 128 x 256 tiles unless the caller is the fused multi-GPU engine (flags, peer stores and per-128 x 128-tile
+  // completion signals are built around the 128 x 128 configuration) or pins that configuration with block_n == 128.
+  // The GLU epilogues always take the 128 x 128 configuration (see gemm_sm90_kernel).
+  const bool wide = p.block_n != 128 && p.wait_flags == nullptr && p.signal_ptr_table == nullptr && p.d_ptr_table == nullptr &&
+                    p.epilogue != EPI_GLU && p.epilogue != EPI_GLU_BWD;
+  constexpr int bm = 128;
+  const int bn = wide ? 256 : 128;
   GemmArgs a{};
   a.M = p.M; a.N = p.N; a.K = p.K; a.G = p.G;
   a.b_group_div = p.b_group_div > 0 ? p.b_group_div : 1;
@@ -816,18 +849,22 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
     if (p.a_mn_major || p.b_mn_major) { *why = "fp8 operands must be K-major"; return cudaErrorInvalidValue; }
     const bool xact = p.epilogue == EPI_BIAS_GELU || p.epilogue == EPI_BIAS_SILU || p.epilogue == EPI_ACT_BWD;
     if (xact) { *why = "GELU / SiLU epilogues need 16-bit operands"; return cudaErrorInvalidValue; }
-    if (p.in_dtype == DT_E4M3) return launch_inst<false, false, DT_E4M3>(ta, tb_, tb2, a, grid, stream);
-    return launch_inst<false, false, DT_E5M2>(ta, tb_, tb2, a, grid, stream);
+    if (wide) {
+      if (p.in_dtype == DT_E4M3) return launch_inst<256, false, false, DT_E4M3>(ta, tb_, tb2, a, grid, stream);
+      return launch_inst<256, false, false, DT_E5M2>(ta, tb_, tb2, a, grid, stream);
+    }
+    if (p.in_dtype == DT_E4M3) return launch_inst<128, false, false, DT_E4M3>(ta, tb_, tb2, a, grid, stream);
+    return launch_inst<128, false, false, DT_E5M2>(ta, tb_, tb2, a, grid, stream);
   }
-#define TB_SWITCH_MAJOR(DTv)                                                                                   \
-  do {                                                                                                         \
-    if (!p.a_mn_major && !p.b_mn_major) return launch_inst<false, false, DTv>(ta, tb_, tb2, a, grid, stream);   \
-    if (!p.a_mn_major && p.b_mn_major) return launch_inst<false, true, DTv>(ta, tb_, tb2, a, grid, stream);     \
-    if (p.a_mn_major && !p.b_mn_major) return launch_inst<true, false, DTv>(ta, tb_, tb2, a, grid, stream);     \
-    return launch_inst<true, true, DTv>(ta, tb_, tb2, a, grid, stream);                                        \
+#define TB_SWITCH_MAJOR(BNv, DTv)                                                                                  \
+  do {                                                                                                             \
+    if (!p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, false, false, DTv>(ta, tb_, tb2, a, grid, stream);   \
+    if (!p.a_mn_major && p.b_mn_major) return launch_inst<BNv, false, true, DTv>(ta, tb_, tb2, a, grid, stream);     \
+    if (p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, true, false, DTv>(ta, tb_, tb2, a, grid, stream);     \
+    return launch_inst<BNv, true, true, DTv>(ta, tb_, tb2, a, grid, stream);                                        \
   } while (0)
-  if (p.in_dtype == DT_BF16) TB_SWITCH_MAJOR(DT_BF16);
-  if (p.in_dtype == DT_FP16) TB_SWITCH_MAJOR(DT_FP16);
+  if (p.in_dtype == DT_BF16) { if (wide) TB_SWITCH_MAJOR(256, DT_BF16); TB_SWITCH_MAJOR(128, DT_BF16); }
+  if (p.in_dtype == DT_FP16) { if (wide) TB_SWITCH_MAJOR(256, DT_FP16); TB_SWITCH_MAJOR(128, DT_FP16); }
 #undef TB_SWITCH_MAJOR
   *why = "unsupported operand dtype";
   return cudaErrorInvalidValue;

@@ -91,8 +91,11 @@ struct GemmProblem {
   // rows it produced itself while the peers' rows are still in flight.
   int group_rot = 0, group_mod = 1;
 
-  // Tile-shape hints of callers written for CTA pairs / 256-wide tiles (cta_group 0, 1, 2; block_n 0, 128, 256):
-  // validated, but the kernel has ONE tile shape (128 x 128, one CTA) - Hopper has no CTA-pair MMA.
+  // Tile shape.  The launcher runs 128 x 256 tiles, except for the fused multi-GPU engine (wait_flags, signal_ptr_table
+  // or d_ptr_table set: its flags, peer stores and per-tile completion counts assume 128 x 128 tiles and a GEMM CTA
+  // that leaves room for one dispatch block per SM) and the GLU epilogues, which run 128 x 128 tiles.
+  // block_n == 128 pins the 128 x 128 configuration; 0 and 256 leave the choice to the launcher.
+  // cta_group (0, 1, 2) is validated and ignored: every tile is computed by one CTA.
   int cta_group = 0;
   int block_n = 0;
   int max_ctas = 0;  // 0 = all SMs

@@ -271,6 +271,34 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, ui
 }
 #undef TB_WGMMA16
 #undef TB_WGMMA8
+
+// m64n256: 128 floats per thread, same fragment layout with j = 0..31.
+#define TB_ACC64O(d, o) TB_ACC8(d, o), TB_ACC8(d, o + 8), TB_ACC8(d, o + 16), TB_ACC8(d, o + 24), TB_ACC8(d, o + 32), TB_ACC8(d, o + 40), TB_ACC8(d, o + 48), TB_ACC8(d, o + 56)
+#define TB_D128 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
+#define TB_WGMMA16(TYPES)                                                                                        \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n256k16.f32." TYPES " " TB_D128 ", %128, %129, p, 1, 1, %131, %132;\n\t}\n" \
+               : TB_ACC64O(d, 0), TB_ACC64O(d, 64)                                                               \
+               : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA ? 1 : 0), "n"(TB ? 1 : 0))
+#define TB_WGMMA8(TYPES)                                                                                         \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n256k32.f32." TYPES " " TB_D128 ", %128, %129, p, 1, 1;\n\t}\n"      \
+               : TB_ACC64O(d, 0), TB_ACC64O(d, 64)                                                               \
+               : "l"(adesc), "l"(bdesc), "r"(accumulate))
+
+// d (+)= A[64 x K] * B[K x 256]; operand rules of wgmma_m64n128.
+template <int T, bool TA, bool TB>
+__device__ __forceinline__ void wgmma_m64n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  static_assert(T == WG_BF16 || T == WG_FP16 || (!TA && !TB), "8-bit operands are K-major only");
+  if constexpr (T == WG_BF16) TB_WGMMA16("bf16.bf16");
+  else if constexpr (T == WG_FP16) TB_WGMMA16("f16.f16");
+  else if constexpr (T == WG_E4M3) TB_WGMMA8("e4m3.e4m3");
+  else TB_WGMMA8("e5m2.e5m2");
+}
+#undef TB_WGMMA16
+#undef TB_WGMMA8
+#undef TB_D128
+#undef TB_ACC64O
 #undef TB_D64
 #undef TB_ACC64
 #undef TB_ACC8
