@@ -3,19 +3,24 @@
 // Replaces the reference's cuBLAS `torch.matmul` expert GEMMs (tutel/experts/ffn.py:114-118,
 // tutel/experts/llama_ffn.py:38-41) and its host-synchronised per-expert loop
 // `sparse_bmm_infer` (tutel/custom/custom_kernel.cpp:874-889) with ONE persistent, warp-specialised kernel
-// (384 threads, 128 x 256 output tiles; 128 x 128 for the fused multi-GPU engine, the GLU epilogues and block_n=128,
-// see Cfg and gemm_sm90_launch):
+// (384 threads, 128 x 256 output tiles; 128 x 128 for the fused multi-GPU engine, the GLU epilogues, fp32 outputs and
+// block_n=128, see Cfg and gemm_sm90_launch):
 //
 //   warp 0        TMA producer   cp.async.bulk.tensor (128B swizzle) -> smem ring, mbarrier complete_tx; the other
-//                                three warps of its warpgroup only give their registers away (setmaxnreg)
+//                                three warps of its warpgroup only give their registers away (setmaxnreg).  128 x 256:
+//                                also loads the tile's aux operand (ReLU / activation gradient, add) into the output
+//                                tile while the main loop runs.
 //   warps 4..11   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async (m64n256 / m64n128, operands
 //                                straight from the swizzled ring, fp32 accumulator fragment in registers), one stage in
 //                                flight; a stage is handed back to the producer when the wgmma group that read it has retired.
-//                                Epilogue: every warp parks 16 x 128 of its fragment (one pass per 128 columns) in its
-//                                own shared-memory rows and
-//                                reads it back with one lane per row and 32 consecutive columns per lane, applies the
-//                                fused bias / activation / activation-grad / GLU / bias-grad math in fp32 and writes 64
-//                                contiguous bytes per lane - locally or straight into PEER GPUs' memory plus a
+//                                128 x 256 epilogue: scales / bias / activation / aux math on the fragment in registers,
+//                                packed into the 16-bit output tile in the TMA box layout, bias-gradient column sums
+//                                reduced in the CTA; one thread issues the TMA store and all consumers go on to the next
+//                                tile's main loop while it drains (see wide_main and flush_out_tile).
+//                                128 x 128 epilogue: every warp parks 16 x 128 of its fragment in its own shared-memory
+//                                rows and reads it back with one lane per row and 32 consecutive columns per lane, applies
+//                                the fused bias / activation / activation-grad / GLU / bias-grad math in fp32 and writes
+//                                64 contiguous bytes per lane - locally or straight into PEER GPUs' memory plus a
 //                                release.sys counter bump (GEMM -> combine all-to-all fusion) - while the producer
 //                                already fills the ring for the next tile.
 //
@@ -87,8 +92,10 @@ constexpr int kSmemLimit = 232448;   // 227 KB
 //           budget above gemm_sm90_kernel).
 //   BN 256  m64n256 wgmma per consumer warpgroup (128 fp32 accumulators per thread): 48 KB of operands per 64-deep K
 //           block for twice the FLOPs of a 128 x 128 tile's 32 KB, and each warpgroup's B reads from shared memory
-//           serve 256 instead of 128 columns.  3 stages of 48 KB plus the 68 KB epilogue staging (214 KB), 168
-//           registers per thread (producer warpgroup 40, consumers 232), one CTA per SM.
+//           serve 256 instead of 128 columns.  16-bit output only.  3 stages of 48 KB, the 64 KB output tile, barriers
+//           and two 1 KB bias-gradient rows (212 KB), 168 registers per thread (producer warpgroup 40, consumers 232),
+//           one CTA per SM.  The epilogue works on the accumulator fragment in registers and hands the tile to a TMA
+//           store, so the consumers start the next tile's main loop while the store drains (see wide_epilogue).
 template <int BN_>
 struct Cfg {
   static constexpr int BM = 128;
@@ -97,19 +104,23 @@ struct Cfg {
   static constexpr int A_BYTES = BM * kSwizzleBytes;
   static constexpr int B_BYTES = BN * kSwizzleBytes;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // Epilogue staging: per consumer warp 16 accumulator rows of 128 floats (the accumulator is staged in passes of 128
-  // columns); 8 floats of padding per row keep the fragment writes (float2, four rows per half-warp) free of bank
-  // conflicts.
+  // 128 x 128 epilogue staging: per consumer warp 16 accumulator rows of 128 floats; 8 floats of padding per row keep
+  // the fragment writes (float2, four rows per half-warp) free of bank conflicts.
   static constexpr int EPI_COLS = 128;
-  static constexpr int PASSES = BN / EPI_COLS;
   static constexpr int EPI_PITCH = EPI_COLS + 8;
   static constexpr int EPI_WARP_BYTES = 16 * EPI_PITCH * 4;
-  static constexpr int EPI_BYTES = 8 * EPI_WARP_BYTES;
+  static constexpr int EPI_BYTES = WIDE ? 0 : 8 * EPI_WARP_BYTES;
+  // 128 x 256 output tile in 16 bit, as the TMA boxes of the output tensor map: four boxes of 128 rows x 64 columns
+  // (128 B per row, 128-byte swizzle).  It also receives the tile's aux operand, and its bias-gradient rows.
+  static constexpr int OUT_BOX_BYTES = BM * kSwizzleBytes;
+  static constexpr int OUT_TILE_BYTES = WIDE ? BM * BN * 2 : 0;
+  static constexpr int COLSUM_BYTES = WIDE ? 2 * BN * 4 : 0;   // double-buffered: tile i+2 reuses tile i's row
   static constexpr int BAR_BYTES = 512;
   static constexpr int STAGES = WIDE ? 3 : 4;
   static constexpr int MAXNREG = WIDE ? 168 : 144;
   static constexpr int CONSUMER_REGS = WIDE ? 232 : 192;   // producer warpgroup: 40
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + BAR_BYTES + EPI_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + OUT_TILE_BYTES + BAR_BYTES + EPI_BYTES + COLSUM_BYTES;
+  static_assert((STAGES * STAGE_BYTES) % 1024 == 0, "the output tile must stay 1024B aligned for the 128B swizzle");
   // 228 KB per SM, 1 KB reserved per resident block: a dispatch block (no shared memory of its own) must still fit
   static_assert(WIDE || SMEM_BYTES + 2 * 1024 <= 228 * 1024, "no room for the push kernel");
   static_assert(SMEM_BYTES <= kSmemLimit, "");
@@ -152,8 +163,31 @@ __device__ __forceinline__ int rotate_group(int g, int rot, int mod) {
   return g;
 }
 
+// Per-element epilogue formulas.  Both configurations call these, so that they produce the same bits per element.
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 __device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
+__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
+// v = upstream gradient, x = forward activation output (ReLU) or pre-activation (GELU / SiLU)
+__device__ __forceinline__ float relu_bwd(float v, float x) { return x > 0.0f ? v : 0.0f; }
+__device__ __forceinline__ float gelu_bwd(float v, float x) {   // d/dx [x * Phi(x)] = Phi(x) + x * phi(x)
+  const float cdf = 0.5f * (1.0f + erff(x * 0.70710678118654752f));
+  return v * (cdf + x * 0.3989422804014327f * __expf(-0.5f * x * x));
+}
+__device__ __forceinline__ float silu_bwd(float v, float x) {   // d/dx [x * s(x)] = s(x) * (1 + x * (1 - s(x)))
+  const float sg = fast_sigmoid(x);
+  return v * (sg * (1.0f + x * (1.0f - sg)));
+}
+// two floats <-> one word of two 16-bit values; both conversions are computed and one is selected, so a run-time dtype
+// costs no branch inside an unrolled loop
+__device__ __forceinline__ uint32_t pack2(float a, float b, bool bf16) {
+  const __nv_bfloat162 hb = __floats2bfloat162_rn(a, b);
+  const __half2 hh = __floats2half2_rn(a, b);
+  return bf16 ? *reinterpret_cast<const uint32_t*>(&hb) : *reinterpret_cast<const uint32_t*>(&hh);
+}
+__device__ __forceinline__ float2 unpack2(uint32_t w, bool bf16) {
+  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&w));
+  return bf16 ? make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xFFFF0000u)) : h;
+}
 
 __device__ __forceinline__ void unpack8(const uint4& u, bool is_bf16, float* f) {
   const uint32_t w[4] = {u.x, u.y, u.z, u.w};
@@ -210,8 +244,6 @@ __device__ __forceinline__ void unpack32(const uint4* p, float* f, bool is_bf16)
   if (is_bf16) unpack32_t<true>(p, f); else unpack32_t<false>(p, f);
 }
 
-__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-
 // GLU math on one 32-column segment, activation fixed at compile time (branch-free, fully interleavable).
 template <int ACT>
 __device__ __forceinline__ void glu_fwd_seg(const float* g, const float* u, float* o) {
@@ -248,6 +280,149 @@ __device__ __forceinline__ void glu_bwd_seg(const float* r, const float* g, floa
   }
 }
 
+// ---- 128 x 256 epilogue, on the accumulator fragment in registers ----
+// A consumer thread (warp cw, lane l) holds tile rows r0 = 16 cw + l / 4 (acc[4j], acc[4j + 1]) and r0 + 8 (acc[4j + 2],
+// acc[4j + 3]) at columns 8j + 2 (l % 4) + {0, 1}, j = 0..31.  In the 16-bit output tile, column block j lies in box
+// j / 8 at 16-byte chunk j % 8 of its row, which the 128-byte swizzle moves to chunk (j % 8) ^ (row % 8), and row % 8 is
+// l / 4 for both rows of a thread: each fragment word has one fixed shared-memory word, and the 32 lanes' words of one
+// j cover 8 rows x 16 bytes in 32 distinct banks.
+enum WideMain : int { WM_NONE, WM_BIAS, WM_RELU_BWD, WM_ADD, WM_GELU_BWD, WM_SILU_BWD };
+
+__device__ __forceinline__ uint32_t out_tile_off(int j, int swz) {
+  return static_cast<uint32_t>((j >> 3) * (128 * kSwizzleBytes) + (((j & 7) ^ swz) << 4));
+}
+
+// fp8 operands: acc *= scale_a[m] * scale_b[n]  (sb: this group's column scales or null)
+__device__ __forceinline__ void wide_scale(float (&acc)[128], float sa0, float sa1, const float* sb, int n_lane, int N) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const int n = n_lane + 8 * j;
+    if (sb != nullptr && n < N) {
+      const float2 s = *reinterpret_cast<const float2*>(sb + n);
+      acc[4 * j] *= sa0 * s.x; acc[4 * j + 1] *= sa0 * s.y;
+      acc[4 * j + 2] *= sa1 * s.x; acc[4 * j + 3] *= sa1 * s.y;
+    } else {
+      acc[4 * j] *= sa0; acc[4 * j + 1] *= sa0;
+      acc[4 * j + 2] *= sa1; acc[4 * j + 3] *= sa1;
+    }
+  }
+}
+
+// alpha / bias / aux math.  The aux operand is read from the output tile (this thread's words at row0 and row0 + 8 rows).
+template <int WM>
+__device__ __forceinline__ void wide_main(float (&acc)[128], const uint8_t* row0, int swz, const uint8_t* bias_g,
+                                          bool bias_f32, bool bias_bf16, int n_lane, int N, bool out_bf16, float alpha) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    if constexpr (WM == WM_NONE) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) acc[4 * j + c] *= alpha;
+    } else if constexpr (WM == WM_BIAS) {
+      const int n = n_lane + 8 * j;
+      float2 b = make_float2(0.0f, 0.0f);
+      if (n < N)
+        b = bias_f32 ? *reinterpret_cast<const float2*>(bias_g + n * 4)
+                     : unpack2(*reinterpret_cast<const uint32_t*>(bias_g + n * 2), bias_bf16);
+      acc[4 * j] += b.x; acc[4 * j + 1] += b.y;
+      acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
+    } else {
+      const uint32_t o = out_tile_off(j, swz);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float2 f = unpack2(*reinterpret_cast<const uint32_t*>(row0 + h * 8 * kSwizzleBytes + o), out_bf16);
+        float& v0 = acc[4 * j + 2 * h];
+        float& v1 = acc[4 * j + 2 * h + 1];
+        if constexpr (WM == WM_RELU_BWD) { v0 = relu_bwd(v0, f.x); v1 = relu_bwd(v1, f.y); }
+        else if constexpr (WM == WM_ADD) { v0 += f.x; v1 += f.y; }
+        else if constexpr (WM == WM_GELU_BWD) { v0 = gelu_bwd(v0, f.x); v1 = gelu_bwd(v1, f.y); }
+        else { v0 = silu_bwd(v0, f.x); v1 = silu_bwd(v1, f.y); }
+      }
+    }
+  }
+}
+
+template <int ACT>
+__device__ __forceinline__ void wide_act(float (&acc)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) {
+    if constexpr (ACT == ACT_RELU) acc[i] = fmaxf(acc[i], 0.0f);
+    else if constexpr (ACT == ACT_GELU) acc[i] = gelu_erf(acc[i]);
+    else acc[i] = silu(acc[i]);
+  }
+}
+
+__device__ __forceinline__ void wide_stage(const float (&acc)[128], uint8_t* row0, int swz, bool out_bf16) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const uint32_t o = out_tile_off(j, swz);
+    *reinterpret_cast<uint32_t*>(row0 + o) = pack2(acc[4 * j], acc[4 * j + 1], out_bf16);
+    *reinterpret_cast<uint32_t*>(row0 + 8 * kSwizzleBytes + o) = pack2(acc[4 * j + 2], acc[4 * j + 3], out_bf16);
+  }
+}
+
+// Bias gradient: this thread's two rows (those below the valid row count) summed per column, then reduced over the
+// eight lanes that share its columns (lane bits 2..4) by halving exchanges, 32 + 16 + 8 shuffles: afterwards lane l
+// holds the warp's sums of columns 32 (l / 4) + 8 i + 2 (l % 4) + {0, 1}, i = 0..3, which go into the CTA's shared row.
+__device__ __forceinline__ void wide_colsum(const float (&acc)[128], bool ok0, bool ok1, int lane, float* colrow) {
+  float s[64];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+#pragma unroll
+    for (int c = 0; c < 2; ++c) s[2 * j + c] = (ok0 ? acc[4 * j + c] : 0.0f) + (ok1 ? acc[4 * j + 2 + c] : 0.0f);
+  }
+#pragma unroll
+  for (int off = 16; off >= 4; off >>= 1) {
+    const bool upper = (lane & off) != 0;
+#pragma unroll
+    for (int i = 0; i < 2 * off; ++i) {
+      const float send = upper ? s[i] : s[i + 2 * off];
+      const float recv = __shfl_xor_sync(0xffffffffu, send, off);
+      s[i] = (upper ? s[i + 2 * off] : s[i]) + recv;
+    }
+  }
+  float* base = colrow + 32 * (lane >> 2) + 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) atomicAdd(base + 8 * (i >> 1) + (i & 1), s[i]);
+}
+
+// The 128 x 256 output tile of group g at rows m0.., columns n0.. -> global memory.
+struct OutTileStore {
+  const uint8_t* tile;
+  uint32_t tile_smem;
+  int m0, n0, m_valid, N, g;
+  long long group_stride, ld;
+  bool straddle;       // rows from m_valid on must stay untouched: row-guarded copy instead of TMA
+  int ct;              // consumer thread 0..255
+  bool writer;         // the thread that issues (and later waits for) the TMA stores
+};
+// All 256 consumer threads call this after writing their words of the tile.  One thread issues the TMA store and
+// everyone moves on; with wait_read the tile may be overwritten as soon as this returns.
+__device__ __forceinline__ void flush_out_tile(const OutTileStore& s, const CUtensorMap* map, uint8_t* dst, bool wait_read) {
+  constexpr int kChunks = 256 / 8;   // 16-byte chunks per tile row
+  ptx::fence_proxy_async_smem();     // this thread's tile writes -> visible to the async proxy (TMA)
+  ptx::named_bar_sync(1, 256);
+  if (s.straddle) {
+    for (int i = s.ct; i < 128 * kChunks; i += 256) {
+      const int r = i / kChunks, ch = i % kChunks;
+      const int m = s.m0 + r, n = s.n0 + ch * 8;
+      if (m < s.m_valid && n < s.N) {
+        const uint4 v = *reinterpret_cast<const uint4*>(s.tile + (ch >> 3) * (128 * kSwizzleBytes) + r * kSwizzleBytes +
+                                                        (((ch & 7) ^ (r & 7)) << 4));
+        *reinterpret_cast<uint4*>(dst + (static_cast<long long>(s.g) * s.group_stride + static_cast<long long>(m) * s.ld + n) * 2) = v;
+      }
+    }
+    ptx::named_bar_sync(1, 256);   // the tile has been read
+    return;
+  }
+  if (s.writer) {
+    for (int b = 0; b < 4; ++b)
+      if (s.n0 + 64 * b < s.N) ptx::tma_store_3d(map, s.tile_smem + b * (128 * kSwizzleBytes), s.n0 + 64 * b, s.m0, s.g);
+    ptx::bulk_commit_group();
+    if (wait_read) ptx::bulk_wait_group_read<0>();
+  }
+  if (wait_read) ptx::named_bar_sync(1, 256);
+}
+
 // Resource budget (deliberate): 384 threads x 144 registers = 55296 of the SM's 65536 registers (the producer warpgroup
 // shrinks to 40 per thread, the two consumer warpgroups grow to 192: 128 x 40 + 256 x 192 = 54272) and 202 KB of its
 // 228 KB shared memory, so ONE 128-thread x 64-register block of the dispatch kernel (encode_rows, which needs no
@@ -257,7 +432,9 @@ __device__ __forceinline__ void glu_bwd_seg(const float* r, const float* g, floa
 template <int BN_, bool A_MN, bool B_MN, int DT>
 __global__ void __maxnreg__(Cfg<BN_>::MAXNREG)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmB2, const GemmArgs args) {
+                 const __grid_constant__ CUtensorMap tmB2, const __grid_constant__ CUtensorMap tmD,
+                 const __grid_constant__ CUtensorMap tmAux, const __grid_constant__ CUtensorMap tmD2,
+                 const GemmArgs args) {
   using C = Cfg<BN_>;
   constexpr int BN = C::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -265,28 +442,44 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);  // warp-uniform role id
   const int lane = threadIdx.x & 31;
 
-  // ---- shared memory carve-up (operand ring must be 1024B aligned for the 128B swizzle) ----
+  // ---- shared memory carve-up (operand ring and output tile must be 1024B aligned for the 128B swizzle) ----
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr int stages = C::STAGES;
-  const uint32_t bar_base = smem_base + static_cast<uint32_t>(stages) * C::STAGE_BYTES;
+  const uint32_t out_base = smem_base + static_cast<uint32_t>(stages) * C::STAGE_BYTES;   // 128 x 256 only
+  const uint32_t bar_base = out_base + C::OUT_TILE_BYTES;
   auto smem_a = [&](int s) { return smem_base + s * C::STAGE_BYTES; };
   auto smem_b = [&](int s) { return smem_base + s * C::STAGE_BYTES + C::A_BYTES; };
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
+  // 128 x 256: the aux operand has landed in the output tile / the TMA store has finished reading the output tile
+  const uint32_t aux_full = bar_base + 128u;
+  const uint32_t out_empty = bar_base + 136u;
   const uint32_t epi_base = bar_base + C::BAR_BYTES;
   float* epi_ptr = reinterpret_cast<float*>(smem_raw + (epi_base - ptx::smem_u32(smem_raw)));
+  uint8_t* out_tile = smem_raw + (out_base - ptx::smem_u32(smem_raw));
+  float* colsum_rows = epi_ptr;   // 128 x 256: two rows of BN floats (EPI_BYTES is 0)
+  // The 128 x 256 epilogue reads the aux operand of RELU_BWD / ADD / ACT_BWD from the output tile; the producer loads
+  // it there with TMA while the main loop runs.
+  const bool aux_tma = C::WIDE && (args.epilogue == EPI_RELU_BWD || args.epilogue == EPI_ADD || args.epilogue == EPI_ACT_BWD);
 
   if (warp == 0 && ptx::elect_one()) {
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmB);
     if (args.dual) ptx::prefetch_tensormap(&tmB2);
+    if (C::WIDE) ptx::prefetch_tensormap(&tmD);
+    if (aux_tma) ptx::prefetch_tensormap(&tmAux);
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < stages; ++s) {
       ptx::mbar_init(full_bar(s), 1);
       ptx::mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
     }
+    ptx::mbar_init(aux_full, 1);
+    ptx::mbar_init(out_empty, 1);
     ptx::fence_mbar_init();
+  }
+  if constexpr (C::WIDE) {
+    for (int i = threadIdx.x; i < 2 * BN; i += kThreads) colsum_rows[i] = 0.0f;
   }
   __syncthreads();
 
@@ -301,6 +494,10 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   // 32-column gate / up / gradient segments do not fit the consumers' 232 registers.
   const bool dual = !C::WIDE && args.dual != 0;
   const int tile_n = dual ? BN / 2 : BN;   // output columns per tile
+  // 128 x 256: in the main loop of tile i, once K block kb_out_free has been issued, the thread that stored tile i - 1
+  // waits until that store has read the output tile and releases the tile (out_empty); the producer then loads tile i's
+  // aux operand into it.  Late enough that the store has normally drained, early enough to hide the aux load.
+  const int kb_out_free = min(2, num_kb - 1);
 
   if (warp < 4) {
     ptx::setmaxnreg_dec<40>();
@@ -308,6 +505,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       // =============================== TMA producer ===============================
       int s = 0;
       uint32_t ph = 0;
+      uint32_t it = 0;   // tiles processed
       int seen_group = -1;
       unsigned long long seen_mask = 0ull;
       for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
@@ -376,7 +574,17 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
           __syncwarp();
           if (++s == stages) { s = 0; ph ^= 1u; }
+          if (aux_tma && kb == kb_out_free) {
+            ptx::mbar_wait_quiet(out_empty, (it & 1u) ^ 1u);   // tile it - 1's store has read the output tile
+            if (ptx::elect_one()) {
+              ptx::mbar_expect_tx(aux_full, C::OUT_TILE_BYTES);
+              for (int b = 0; b < BN / 64; ++b)
+                ptx::tma_load_3d(out_base + b * C::OUT_BOX_BYTES, &tmAux, aux_full, n0 + 64 * b, m0, tc.g);
+            }
+            __syncwarp();
+          }
         }
+        ++it;
       }
     }
   } else {
@@ -415,6 +623,19 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         v[q * 4] = t4.x; v[q * 4 + 1] = t4.y; v[q * 4 + 2] = t4.z; v[q * 4 + 3] = t4.w;
       }
     };
+    // 128 x 256 epilogue geometry (see wide_main): this thread's words of the output tile are at row0 + out_tile_off(j)
+    // and 8 rows further down.
+    const int ct = threadIdx.x - 128;       // consumer thread 0..255
+    const bool out_writer = ct == 0;        // issues the output tile's TMA stores and releases the tile (out_empty)
+    const int r0 = cw * 16 + (lane >> 2);
+    const int swz = lane >> 2;              // = r0 % 8
+    uint8_t* row0 = out_tile + r0 * kSwizzleBytes + (lane & 3) * 4;
+    const int wmain = args.epilogue == EPI_NONE ? WM_NONE
+                    : args.epilogue == EPI_ADD ? WM_ADD
+                    : args.epilogue == EPI_RELU_BWD ? WM_RELU_BWD
+                    : args.epilogue == EPI_ACT_BWD ? (args.act == ACT_GELU ? WM_GELU_BWD : args.act == ACT_SILU ? WM_SILU_BWD : WM_RELU_BWD)
+                    : WM_BIAS;
+    uint32_t it = 0;   // tiles processed
 
     for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
       TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
@@ -426,6 +647,12 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
       // ------------------------------- main loop -------------------------------
       float acc[BN / 2];
+      if constexpr (C::WIDE) {
+        // The first wgmma of a tile ignores the accumulator, but its register operands are read-write: without a fresh
+        // definition the previous tile's 128 values would stay live through the whole epilogue.
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      }
       int prev_s = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         ptx::mbar_wait_quiet(full_bar(s), ph);
@@ -440,6 +667,13 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           else ptx::wgmma_m64n128<DT, A_MN, B_MN>(acc, ad, bd, (kb | k) != 0);
         }
         ptx::wgmma_commit();
+        if constexpr (C::WIDE) {
+          if (out_writer && it > 0 && kb == kb_out_free) {
+            ptx::bulk_wait_group_read<0>();
+            ptx::mbar_arrive(out_empty);
+          }
+          __syncwarp();
+        }
         if (kb > 0) {
           ptx::wgmma_wait<1>();                                   // the group that read the previous stage has retired
           if (wg_leader) ptx::mbar_arrive(empty_bar(prev_s));
@@ -450,18 +684,83 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       ptx::wgmma_wait<0>();
       if (wg_leader) ptx::mbar_arrive(empty_bar(prev_s));
 
-      // ------------------------------- epilogue -------------------------------
-      // The accumulator goes through the staging rows in passes of EPI_COLS columns: pass p stages columns
-      // [128 p, 128 p + 128) and runs the segment epilogue on them (the GLU epilogues: one pass, 128 x 128 only).
-#pragma unroll
-      for (int pass = 0; pass < C::PASSES; ++pass) {
+      if constexpr (C::WIDE) {
+        // ------------------------- 128 x 256 epilogue -------------------------
+        const int m0 = tc.m_blk * C::BM, n0 = tc.n_blk * BN;
+        const int gb = tc.g / args.b_group_div;
+        const bool ok0 = m0 + r0 < m_valid, ok1 = m0 + r0 + 8 < m_valid;
+        const int n_lane = n0 + 2 * (lane & 3);
+        // a row block that straddles the group's row count (at most one per group) must not write past the count,
+        // which the output tensor map cannot express: it is copied out with row-guarded stores instead
+        const bool straddle = m0 + C::BM > m_valid && m_valid < args.M;
+        if (args.scale_a != nullptr || args.scale_b != nullptr) {
+          const float* sa = args.scale_a != nullptr ? args.scale_a + static_cast<long long>(tc.g) * args.scale_a_group_stride + m0 + r0 : nullptr;
+          const float sa0 = (sa != nullptr && ok0) ? sa[0] : 1.0f;
+          const float sa1 = (sa != nullptr && ok1) ? sa[8] : 1.0f;
+          const float* sb = args.scale_b != nullptr ? args.scale_b + static_cast<long long>(gb) * args.scale_b_group_stride : nullptr;
+          wide_scale(acc, sa0, sa1, sb, n_lane, args.N);
+        }
+        const uint8_t* bias_g = nullptr;
+        if (args.bias != nullptr)
+          bias_g = reinterpret_cast<const uint8_t*>(args.bias) +
+                   static_cast<long long>(gb) * args.bias_group_stride * (args.bias_is_fp32 ? 4 : 2);
+        const uint32_t out_free_parity = (it & 1u) ^ 1u;   // out_empty phase it - 1: tile it - 1's store has read the tile
+
+        const OutTileStore st{out_tile, out_base, m0, n0, m_valid, args.N, tc.g, args.d_group_stride, args.ldd, straddle, ct,
+                              out_writer};
+
+        if (wmain == WM_BIAS) {
+          if (bias_g != nullptr)
+            wide_main<WM_BIAS>(acc, row0, swz, bias_g, args.bias_is_fp32 != 0, args.bias_is_bf16 != 0, n_lane, args.N, out_bf16, 1.0f);
+          if (args.d2 != nullptr && (args.epilogue == EPI_BIAS_GELU || args.epilogue == EPI_BIAS_SILU)) {
+            // training: the backward pass needs the pre-activation (ReLU gets by with the sign of its output)
+            ptx::mbar_wait_quiet(out_empty, out_free_parity);
+            wide_stage(acc, row0, swz, out_bf16);
+            flush_out_tile(st, &tmD2, reinterpret_cast<uint8_t*>(args.d2), true);
+          }
+          if (args.epilogue == EPI_BIAS_RELU) wide_act<ACT_RELU>(acc);
+          else if (args.epilogue == EPI_BIAS_GELU) wide_act<ACT_GELU>(acc);
+          else if (args.epilogue == EPI_BIAS_SILU) wide_act<ACT_SILU>(acc);
+        } else if (wmain == WM_NONE) {
+          if (args.alpha != 1.0f) wide_main<WM_NONE>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, args.alpha);
+        } else {
+          ptx::mbar_wait_quiet(aux_full, it & 1u);   // this tile's aux operand is in the output tile
+          if (wmain == WM_RELU_BWD) wide_main<WM_RELU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
+          else if (wmain == WM_ADD) wide_main<WM_ADD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
+          else if (wmain == WM_GELU_BWD) wide_main<WM_GELU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
+          else wide_main<WM_SILU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
+        }
+        if (!aux_tma) ptx::mbar_wait_quiet(out_empty, out_free_parity);
+        wide_stage(acc, row0, swz, out_bf16);     // aux epilogues: each word overwrites the aux word it was computed from
+        float* colrow = colsum_rows + (it & 1u) * BN;
+        if (args.colsum != nullptr) wide_colsum(acc, ok0, ok1, lane, colrow);
+        flush_out_tile(st, &tmD, reinterpret_cast<uint8_t*>(args.d), false);
+        if (args.colsum != nullptr && ct < BN / 4) {
+          // one 4-column add per thread and tile: 64 global reductions instead of one per column and 16-row slice
+          float4* src = reinterpret_cast<float4*>(colrow) + ct;
+          const float4 v = *src;
+          *src = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+          const int n = n0 + 4 * ct;
+          if (n < args.N) {   // N is a multiple of 8: all four columns are in range
+            float* cs = args.colsum + static_cast<long long>(gb) * args.colsum_group_stride + n;
+            if ((reinterpret_cast<uintptr_t>(cs) & 15) == 0) {
+              ptx::red_add_v4_f32(cs, v.x, v.y, v.z, v.w);
+            } else {
+              atomicAdd(cs, v.x); atomicAdd(cs + 1, v.y); atomicAdd(cs + 2, v.z); atomicAdd(cs + 3, v.w);
+            }
+          }
+        }
+        ++it;
+        continue;
+      }
+
+      // ------------------------------- 128 x 128 epilogue -------------------------------
       {
         const int fr = lane >> 2, fc = (lane & 3) * 2;
 #pragma unroll
-        for (int jj = 0; jj < C::EPI_COLS / 8; ++jj) {
-          const int j = pass * (C::EPI_COLS / 8) + jj;
-          *reinterpret_cast<float2*>(epi_warp + fr * C::EPI_PITCH + jj * 8 + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(epi_warp + (fr + 8) * C::EPI_PITCH + jj * 8 + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        for (int j = 0; j < C::EPI_COLS / 8; ++j) {
+          *reinterpret_cast<float2*>(epi_warp + fr * C::EPI_PITCH + j * 8 + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(epi_warp + (fr + 8) * C::EPI_PITCH + j * 8 + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
       }
       __syncwarp();
@@ -574,7 +873,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll 1
       for (int c = 0; c < C::EPI_COLS / 64; ++c) {
         const int col = c * 64 + col_half;
-        const int n = tc.n_blk * BN + pass * C::EPI_COLS + col;
+        const int n = tc.n_blk * BN + col;
         float v[32];
         load_acc(col, v);
         const int ncols = min(32, args.N - n);  // multiple of 8, <= 0 past the last column
@@ -597,25 +896,19 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           load_seg16(aux_row, n, ncols, f);
           if (args.epilogue == EPI_RELU_BWD) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = f[j] > 0.0f ? v[j] : 0.0f;
+            for (int j = 0; j < 32; ++j) v[j] = relu_bwd(v[j], f[j]);
           } else if (args.epilogue == EPI_ADD) {
 #pragma unroll
             for (int j = 0; j < 32; ++j) v[j] += f[j];
-          } else if (args.act == ACT_GELU) {      // f = pre-activation: d/dx [x * Phi(x)] = Phi(x) + x * phi(x)
+          } else if (args.act == ACT_GELU) {      // f = pre-activation
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float cdf = 0.5f * (1.0f + erff(f[j] * 0.70710678118654752f));
-              v[j] *= cdf + f[j] * 0.3989422804014327f * __expf(-0.5f * f[j] * f[j]);
-            }
-          } else if (args.act == ACT_SILU) {      // d/dx [x * s(x)] = s(x) * (1 + x * (1 - s(x)))
+            for (int j = 0; j < 32; ++j) v[j] = gelu_bwd(v[j], f[j]);
+          } else if (args.act == ACT_SILU) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float sg = fast_sigmoid(f[j]);
-              v[j] *= sg * (1.0f + f[j] * (1.0f - sg));
-            }
+            for (int j = 0; j < 32; ++j) v[j] = silu_bwd(v[j], f[j]);
           } else {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = f[j] > 0.0f ? v[j] : 0.0f;
+            for (int j = 0; j < 32; ++j) v[j] = relu_bwd(v[j], f[j]);
           }
         } else {
           if (bias_g != nullptr) {
@@ -681,8 +974,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         store_seg(d_row, n, ncols, v);
       }
       }
-      __syncwarp();   // every lane has read its row before the next pass / tile overwrites the staging rows
-      }
+      __syncwarp();   // every lane has read its row before the next tile overwrites the staging rows
       if (args.signal_ptr_table != nullptr) {
         // Combine fusion: all 256 consumer threads' (possibly remote) stores -> one release.sys counter bump.
         asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -691,6 +983,9 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           ptx::red_add_release_sys(reinterpret_cast<uint32_t*>(args.signal_ptr_table[tc.g]), 1u);
         }
       }
+    }
+    if constexpr (C::WIDE) {
+      if (out_writer) ptx::bulk_wait_group<0>();   // the last tile's store has completed
     }
   }
 }
@@ -750,9 +1045,34 @@ bool make_operand_map(CUtensorMap* map, const void* base, int dtype, bool mn_maj
   return true;
 }
 
+// A 16-bit row-major [G][rows][cols] matrix (output, aux or pre-activation of the 128 x 256 epilogue) in boxes of
+// 128 rows x 64 columns, 128-byte swizzle: the layout of the kernel's output tile.  Loads past the end read zeros,
+// stores past the end are dropped.
+bool make_tile_map(CUtensorMap* map, const void* base, int dtype, long long rows, long long cols, long long ld,
+                   long long group_stride, int groups, const char** why) {
+  EncodeTiledFn enc = get_encode_fn();
+  if (enc == nullptr) { *why = "cuTensorMapEncodeTiled unavailable"; return false; }
+  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * 2) & 15) || ((group_stride * 2) & 15)) {
+    *why = "output / aux base and strides must be 16-byte aligned";
+    return false;
+  }
+  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(groups)};
+  cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 2,
+                           static_cast<cuuint64_t>(groups > 1 ? group_stride : rows * ld) * 2};
+  if (strides[1] == 0) strides[1] = strides[0];
+  const cuuint32_t box[3] = {64, 128, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, dtype == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { *why = "cuTensorMapEncodeTiled failed"; return false; }
+  return true;
+}
+
 template <int BN, bool A_MN, bool B_MN, int DT>
-cudaError_t launch_inst(const CUtensorMap& ta, const CUtensorMap& tb_, const CUtensorMap& tb2, const GemmArgs& args,
-                        int grid, cudaStream_t stream) {
+cudaError_t launch_inst(const CUtensorMap& ta, const CUtensorMap& tb_, const CUtensorMap& tb2, const CUtensorMap& td,
+                        const CUtensorMap& taux, const CUtensorMap& td2, const GemmArgs& args, int grid,
+                        cudaStream_t stream) {
   auto* kern = gemm_sm90_kernel<BN, A_MN, B_MN, DT>;
   static bool configured = false;
   if (!configured) {
@@ -760,7 +1080,7 @@ cudaError_t launch_inst(const CUtensorMap& ta, const CUtensorMap& tb_, const CUt
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  kern<<<grid, kThreads, Cfg<BN>::SMEM_BYTES, stream>>>(ta, tb_, tb2, args);
+  kern<<<grid, kThreads, Cfg<BN>::SMEM_BYTES, stream>>>(ta, tb_, tb2, td, taux, td2, args);
   return cudaGetLastError();
 }
 
@@ -805,9 +1125,10 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
 
   // 128 x 256 tiles unless the caller is the fused multi-GPU engine (flags, peer stores and per-128 x 128-tile
   // completion signals are built around the 128 x 128 configuration) or pins that configuration with block_n == 128.
-  // The GLU epilogues always take the 128 x 128 configuration (see gemm_sm90_kernel).
+  // The GLU epilogues (see gemm_sm90_kernel) and fp32 outputs (the 128 x 256 output tile is 16-bit) always take the
+  // 128 x 128 configuration.
   const bool wide = p.block_n != 128 && p.wait_flags == nullptr && p.signal_ptr_table == nullptr && p.d_ptr_table == nullptr &&
-                    p.epilogue != EPI_GLU && p.epilogue != EPI_GLU_BWD;
+                    p.epilogue != EPI_GLU && p.epilogue != EPI_GLU_BWD && p.out_dtype != DT_FP32;
   constexpr int bm = 128;
   const int bn = wide ? 256 : 128;
   GemmArgs a{};
@@ -842,6 +1163,16 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
   CUtensorMap tb2 = tb_;
   if (dual && !make_operand_map(&tb2, p.b2, p.in_dtype, p.b_mn_major, p.N, p.K, p.ldb, p.b_group_stride, gB, b_box, why))
     return cudaErrorInvalidValue;
+  // 128 x 256: the output (TMA store), the aux operand (TMA load) and the GELU / SiLU pre-activation (TMA store)
+  CUtensorMap td = tb_, taux = tb_, td2 = tb_;
+  if (wide) {
+    if (!make_tile_map(&td, p.d, p.out_dtype, p.M, p.N, p.ldd, p.d_group_stride, p.G, why)) return cudaErrorInvalidValue;
+    if (uses_aux && !make_tile_map(&taux, p.aux, p.out_dtype, p.M, p.N, p.ld_aux, p.aux_group_stride, p.G, why))
+      return cudaErrorInvalidValue;
+    if (p.d2 != nullptr && (p.epilogue == EPI_BIAS_GELU || p.epilogue == EPI_BIAS_SILU) &&
+        !make_tile_map(&td2, p.d2, p.out_dtype, p.M, p.N, p.ldd, p.d_group_stride, p.G, why))
+      return cudaErrorInvalidValue;
+  }
 
   const int grid = static_cast<int>(a.num_tiles < sms ? a.num_tiles : sms);
 
@@ -850,18 +1181,18 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
     const bool xact = p.epilogue == EPI_BIAS_GELU || p.epilogue == EPI_BIAS_SILU || p.epilogue == EPI_ACT_BWD;
     if (xact) { *why = "GELU / SiLU epilogues need 16-bit operands"; return cudaErrorInvalidValue; }
     if (wide) {
-      if (p.in_dtype == DT_E4M3) return launch_inst<256, false, false, DT_E4M3>(ta, tb_, tb2, a, grid, stream);
-      return launch_inst<256, false, false, DT_E5M2>(ta, tb_, tb2, a, grid, stream);
+      if (p.in_dtype == DT_E4M3) return launch_inst<256, false, false, DT_E4M3>(ta, tb_, tb2, td, taux, td2, a, grid, stream);
+      return launch_inst<256, false, false, DT_E5M2>(ta, tb_, tb2, td, taux, td2, a, grid, stream);
     }
-    if (p.in_dtype == DT_E4M3) return launch_inst<128, false, false, DT_E4M3>(ta, tb_, tb2, a, grid, stream);
-    return launch_inst<128, false, false, DT_E5M2>(ta, tb_, tb2, a, grid, stream);
+    if (p.in_dtype == DT_E4M3) return launch_inst<128, false, false, DT_E4M3>(ta, tb_, tb2, td, taux, td2, a, grid, stream);
+    return launch_inst<128, false, false, DT_E5M2>(ta, tb_, tb2, td, taux, td2, a, grid, stream);
   }
 #define TB_SWITCH_MAJOR(BNv, DTv)                                                                                  \
   do {                                                                                                             \
-    if (!p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, false, false, DTv>(ta, tb_, tb2, a, grid, stream);   \
-    if (!p.a_mn_major && p.b_mn_major) return launch_inst<BNv, false, true, DTv>(ta, tb_, tb2, a, grid, stream);     \
-    if (p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, true, false, DTv>(ta, tb_, tb2, a, grid, stream);     \
-    return launch_inst<BNv, true, true, DTv>(ta, tb_, tb2, a, grid, stream);                                        \
+    if (!p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, false, false, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);   \
+    if (!p.a_mn_major && p.b_mn_major) return launch_inst<BNv, false, true, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);     \
+    if (p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, true, false, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);     \
+    return launch_inst<BNv, true, true, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);                                        \
   } while (0)
   if (p.in_dtype == DT_BF16) { if (wide) TB_SWITCH_MAJOR(256, DT_BF16); TB_SWITCH_MAJOR(128, DT_BF16); }
   if (p.in_dtype == DT_FP16) { if (wide) TB_SWITCH_MAJOR(256, DT_FP16); TB_SWITCH_MAJOR(128, DT_FP16); }

@@ -93,7 +93,7 @@ struct GemmProblem {
 
   // Tile shape.  The launcher runs 128 x 256 tiles, except for the fused multi-GPU engine (wait_flags, signal_ptr_table
   // or d_ptr_table set: its flags, peer stores and per-tile completion counts assume 128 x 128 tiles and a GEMM CTA
-  // that leaves room for one dispatch block per SM) and the GLU epilogues, which run 128 x 128 tiles.
+  // that leaves room for one dispatch block per SM), the GLU epilogues and fp32 outputs, which run 128 x 128 tiles.
   // block_n == 128 pins the 128 x 128 configuration; 0 and 256 leave the choice to the launcher.
   // cta_group (0, 1, 2) is validated and ignored: every tile is computed by one CTA.
   int cta_group = 0;

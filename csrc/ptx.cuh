@@ -232,6 +232,23 @@ __device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src
                "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// Wait until at most N of this thread's bulk groups are still reading their shared-memory source ...
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// ... or are still in flight at all.
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// Named barrier over `count` threads (a multiple of 32), id 1..15 (0 is __syncthreads).
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// Four fp32 adds to consecutive, 16-byte aligned global words, result unused.
+__device__ __forceinline__ void red_add_v4_f32(float* p, float a, float b, float c, float d) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
 
 // ----------------------------------------------------------------------------------------------
 // wgmma: warpgroup-wide asynchronous MMA, operands in shared memory, fp32 accumulator fragment in registers.
