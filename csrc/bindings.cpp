@@ -76,10 +76,18 @@ void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn,
   TORCH_CHECK(p.out_dtype <= tb::DT_FP32, "tutel_b200.gemm: output must be bf16/fp16/fp32");
   p.epilogue = static_cast<int>(epilogue);
   p.alpha = static_cast<float>(alpha);
+  // groups of B (and rows of bias / scale_b / colsum) the kernel indexes: g / b_group_div for g < G
+  const int64_t gb = (p.G + p.b_group_div - 1) / p.b_group_div;
+  // The epilogues read bias 16 bytes at a time (128 x 128) and scale_b 8 bytes at a time (128 x 256), from the row of
+  // each B group: the base and the row stride must keep that alignment.
+  auto aligned_rows = [](const at::Tensor& t, int64_t bytes) {
+    return reinterpret_cast<uintptr_t>(t.data_ptr()) % bytes == 0 && (t.size(0) == 1 || (t.stride(0) * t.element_size()) % bytes == 0);
+  };
   if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->is_cuda() && bias->dim() == 2 && bias->stride(1) == 1 &&
+    TORCH_CHECK(bias->is_cuda() && bias->dim() == 2 && bias->stride(1) == 1 && bias->size(0) >= gb && bias->size(1) == p.N &&
                     (bias->scalar_type() == a.scalar_type() || (a.element_size() == 1 && bias->scalar_type() == d.scalar_type() && d.element_size() == 2)),
                 "tutel_b200.gemm: bias must be [Gb, N] of the input dtype (fp8 inputs: of the 16-bit output dtype)");
+    TORCH_CHECK(aligned_rows(*bias, 16), "tutel_b200.gemm: bias rows must start 16-byte aligned");
     p.bias = bias->data_ptr();
     p.bias_group_stride = bias->stride(0);
   }
@@ -103,13 +111,14 @@ void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn,
   }
   if (scale_b.has_value() && scale_b->defined()) {
     TORCH_CHECK(scale_b->is_cuda() && scale_b->scalar_type() == at::kFloat && scale_b->dim() == 2 && scale_b->stride(1) == 1 &&
-                scale_b->size(1) == p.N, "tutel_b200.gemm: scale_b must be float [Gb, N]");
+                scale_b->size(0) >= gb && scale_b->size(1) == p.N, "tutel_b200.gemm: scale_b must be float [Gb, N]");
+    TORCH_CHECK(aligned_rows(*scale_b, 8), "tutel_b200.gemm: scale_b rows must start 8-byte aligned");
     p.scale_b = scale_b->data_ptr<float>();
     p.scale_b_group_stride = scale_b->stride(0);
   }
   if (colsum.has_value() && colsum->defined()) {
     TORCH_CHECK(colsum->is_cuda() && colsum->scalar_type() == at::kFloat && colsum->dim() == 2 && colsum->stride(1) == 1 &&
-                colsum->size(1) == p.N, "tutel_b200.gemm: colsum must be float [Gb, N]");
+                colsum->size(0) >= gb && colsum->size(1) == p.N, "tutel_b200.gemm: colsum must be float [Gb, N]");
     p.colsum = colsum->data_ptr<float>();
     p.colsum_group_stride = colsum->stride(0);
   }

@@ -932,7 +932,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (args.d2 != nullptr && (args.epilogue == EPI_BIAS_GELU || args.epilogue == EPI_BIAS_SILU)) {
             // training: the backward pass needs the pre-activation (ReLU gets by with the sign of its output)
             uint8_t* d2_row = reinterpret_cast<uint8_t*>(args.d2) +
-                              (static_cast<long long>(tc.g) * args.d_group_stride + static_cast<long long>(m) * args.ldd) * 2;
+                              (static_cast<long long>(tc.g) * args.d_group_stride + static_cast<long long>(m) * args.ldd) * (out16 ? 2 : 4);
             store_seg(d2_row, n, ncols, v);
           }
           if (args.epilogue == EPI_BIAS_RELU) {
@@ -1120,6 +1120,22 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
     *why = "this epilogue needs a 16-byte aligned 16-bit aux operand";
     return cudaErrorInvalidValue;
   }
+  // A zero group stride (an expanded tensor) would be taken for "one group" by the tensor maps, so group g would start g
+  // rows into the matrix instead of at it: such operands must be materialised by the caller.
+  const int groups_b = (p.G + (p.b_group_div > 0 ? p.b_group_div : 1) - 1) / (p.b_group_div > 0 ? p.b_group_div : 1);
+  if ((p.G > 1 && (p.a_group_stride == 0 || (p.d_ptr_table == nullptr && p.d_group_stride == 0) ||
+                   (uses_aux && p.aux_group_stride == 0))) ||
+      (groups_b > 1 && p.b_group_stride == 0)) {
+    *why = "group strides of A, B, aux and the output must be nonzero when there is more than one group";
+    return cudaErrorInvalidValue;
+  }
+  // rotate_group permutes groups within blocks of |group_mod|; a partial block would map groups past G
+  const int mod_abs = p.group_mod < 0 ? -p.group_mod : p.group_mod;
+  if (mod_abs > 1 && (p.G % mod_abs != 0 || p.group_rot < 0)) {
+    *why = "G must be a multiple of |group_mod|, and group_rot must not be negative";
+    return cudaErrorInvalidValue;
+  }
+  if (p.alpha != 1.0f && p.epilogue != EPI_NONE) { *why = "alpha is applied by EPI_NONE only"; return cudaErrorInvalidValue; }
   if (p.cta_group < 0 || p.cta_group > 2) { *why = "cta_group must be 0, 1 or 2"; return cudaErrorInvalidValue; }
   if (p.block_n != 0 && p.block_n != 128 && p.block_n != 256) { *why = "block_n must be 0, 128 or 256"; return cudaErrorInvalidValue; }
 

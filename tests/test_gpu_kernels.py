@@ -222,7 +222,8 @@ def test_fp8_gemm_with_row_col_scales(C, cg):
     assert (deq - a.float()).abs().max() <= a.float().abs().amax() * 0.07
     d = G.raw_gemm(aq, bq, epilogue=G.EPI_BIAS_RELU, bias=bias, out_dtype=torch.bfloat16, scale_a=sa, scale_b=sb, cta_group=cg)
     ref_q = torch.relu(torch.matmul(deq, (bq.float() * sb.unsqueeze(-1)).transpose(1, 2)) + bias.float().unsqueeze(1))
-    assert torch.allclose(d.float(), ref_q, atol=0.06, rtol=2e-2)          # exact up to bf16 output rounding
+    assert torch.allclose(d.float(), ref_q, atol=0.06, rtol=2e-2)          # bf16 rounding + fp8 accumulation error
+    # (the fp8 wgmma accumulator keeps fewer bits than fp32: see C_ACC in tests/gemm_reference.py)
     ref = torch.relu(torch.matmul(a.float(), b.float().transpose(1, 2)) + bias.float().unsqueeze(1))
     assert (d.float() - ref).norm() / ref.norm() < 0.06                    # quantisation error budget
 

@@ -24,15 +24,27 @@ ACT_CODES = {'relu': 1, 'gelu': 2, 'silu': 3}
 
 
 def _ok_stride(t: torch.Tensor) -> bool:
+    # 16-byte aligned base and strides, and no expanded (stride 0) dimension: the kernel reads rows and groups through
+    # tensor maps, which would take a zero stride for "one row / one group"
     es = t.element_size()
-    return (t.stride(-1) == 1 and (t.stride(-2) * es) % 16 == 0 and (t.dim() < 3 or (t.stride(0) * es) % 16 == 0 or t.size(0) == 1)
-            and t.data_ptr() % 16 == 0)
+    return (t.stride(-1) == 1 and (t.stride(-2) * es) % 16 == 0 and (t.stride(-2) != 0 or t.size(-2) == 1) and
+            (t.dim() < 3 or t.size(0) == 1 or (t.stride(0) != 0 and (t.stride(0) * es) % 16 == 0)) and t.data_ptr() % 16 == 0)
 
 
 def _prep(t: torch.Tensor) -> torch.Tensor:
     if t.dim() == 2:
         t = t.unsqueeze(0)
     return t if _ok_stride(t) else t.contiguous()
+
+
+def _side(t: torch.Tensor, dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """A [rows, N] side input (bias, column scales) in ``dtype`` whose rows start 16-byte aligned, as the epilogues'
+    vector loads need; a view at another offset is copied (``contiguous()`` alone would keep the offset)."""
+    t = t if dtype is None else t.to(dtype)
+    es = t.element_size()
+    if t.stride(-1) == 1 and t.data_ptr() % 16 == 0 and (t.size(0) == 1 or (t.stride(0) * es) % 16 == 0):
+        return t
+    return t.clone(memory_format=torch.contiguous_format)
 
 
 def raw_gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False, epilogue: int = EPI_NONE,
@@ -59,10 +71,9 @@ def raw_gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool
         out = torch.empty([G, M, N], dtype=out_dtype, device=a.device)
     d = out if out.dim() == 3 else out.unsqueeze(0)
     if bias is not None:
-        bias = bias.reshape(b.size(0), N)
-        want = a.dtype if a.element_size() > 1 else out.dtype
-        if bias.stride(-1) != 1 or bias.dtype != want:
-            bias = bias.to(want).contiguous()
+        bias = _side(bias.reshape(b.size(0), N), a.dtype if a.element_size() > 1 else out.dtype)
+    if scale_b is not None:
+        scale_b = _side(scale_b)
     if aux is not None:
         aux = _prep(aux)
     backend.count_launch()
