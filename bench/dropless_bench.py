@@ -4,7 +4,18 @@
 
     python bench/dropless_bench.py --impl ours      --megablocks_size 1
     python bench/dropless_bench.py --impl reference --megablocks_size 1
-Device-timed forward latency (CUDA events, L2 flushed between iterations), one JSON line.
+    python bench/dropless_bench.py --expert_type llama_ffn --experts 8 --dim 4096 --hidden 14336 --top_k 2 \\
+        --tokens 1 --dtype bfloat16                                   # Mixtral-like SwiGLU decode step
+
+`--megablocks_size 0` times the padded path (the capacity is read back to the host, every expert computes the whole
+buffer).  With `--megablocks_size 1` only the experts that received tokens cost anything: up to 64 rows per expert the
+whole expert is one weight-streaming launch (`ffn`: skinny_ffn_kernel, `llama_ffn`: skinny_glu_ffn_kernel), above that
+the wgmma kernels skip rows past the device-side counts.
+Device-timed forward latency (CUDA events, L2 flushed between iterations), one JSON line with the number of active
+experts (experts that received at least one token), the weight bytes those experts hold, and those bytes over the median
+time (`active_weight_GBps`: the weight bandwidth the dropless path needs, whatever the path actually read).  The expert
+module alone is timed the same way on the dispatch buffer of one call (`experts_median_ms`,
+`experts_active_weight_GBps`), and the output is compared with the padded path (`rel_err_vs_padded`).
 """
 import argparse
 import json
@@ -15,13 +26,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ap = argparse.ArgumentParser()
 ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
 ap.add_argument('--megablocks_size', type=int, default=1)
+ap.add_argument('--expert_type', default='ffn', choices=['ffn', 'llama_ffn'])
 ap.add_argument('--experts', type=int, default=128)
 ap.add_argument('--tokens', type=int, default=32)
+ap.add_argument('--top_k', type=int, default=1)
 ap.add_argument('--dim', type=int, default=2048)
+ap.add_argument('--hidden', type=int, default=0, help='hidden size per expert (default: --dim)')
 ap.add_argument('--dtype', default='float32')
 ap.add_argument('--iters', type=int, default=50)
 ap.add_argument('--graph', action='store_true', help='ours only: replay the forward as one CUDA graph (tutel_b200.utils.graph)')
 args = ap.parse_args()
+hidden = args.hidden or args.dim
 if args.impl == 'reference':
     sys.path.insert(0, os.path.join(ROOT, 'baseline', '_ref'))
     from tutel import moe, system
@@ -35,27 +50,53 @@ env = system.init_data_model_parallel(backend='nccl')
 dev = env.local_device
 torch.set_default_dtype(getattr(torch, args.dtype))
 torch.manual_seed(0)
-layer = moe.moe_layer(gate_type={'type': 'top', 'k': 1, 'capacity_factor': 0.0}, model_dim=args.dim,
-                      experts={'type': 'ffn', 'num_experts_per_device': args.experts, 'hidden_size_per_expert': args.dim,
-                               'activation_fn': lambda x: F.relu(x)}, seeds=(1, 1, 1)).to(dev).eval()
+experts = {'type': args.expert_type, 'num_experts_per_device': args.experts, 'hidden_size_per_expert': hidden}
+if args.expert_type == 'ffn':
+    experts['activation_fn'] = lambda x: F.relu(x)
+with torch.device(dev):        # initialise the (multi-GB) weights on the GPU
+    layer = moe.moe_layer(gate_type={'type': 'top', 'k': args.top_k, 'capacity_factor': 0.0}, model_dim=args.dim,
+                          experts=experts, seeds=(1, 1, 1)).eval()
 x = torch.randn(1, args.tokens, args.dim, device=dev)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-call = (lambda t: layer(t, megablocks_size=args.megablocks_size)) if args.megablocks_size > 0 else (lambda t: layer(t))
+eager = (lambda t: layer(t, megablocks_size=args.megablocks_size)) if args.megablocks_size > 0 else (lambda t: layer(t))
+call = eager
 if args.graph and args.impl == 'ours':
     from tutel_b200.utils.graph import GraphedForward
-    call = GraphedForward(call, x)
-times = []
-with torch.no_grad():
-    for i in range(args.iters + 5):
+    call = GraphedForward(eager, x)
+
+
+def timed(fn, iters):
+    times = []
+    for i in range(iters + 5):
         flush.zero_()
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
-        y = call(x)
+        out = fn()
         e.record()
         torch.cuda.synchronize()
         if i >= 5:
             times.append(s.elapsed_time(e))
-times.sort()
-print(json.dumps({'impl': args.impl, 'config': 'dropless cf=0 top-1 E=%d tokens=%d dim=%d %s megablocks_size=%d%s' % (
-    args.experts, args.tokens, args.dim, args.dtype, args.megablocks_size, ' cuda-graph' if args.graph and args.impl == 'ours' else ''), 'median_ms': times[len(times) // 2], 'min_ms': times[0],
+    return out, sorted(times)
+
+
+with torch.no_grad():
+    y, times = timed(lambda: call(x), args.iters)
+    y = y.clone()
+    active = int((layer.dispatch_count > 0).sum())       # counts of the timed call (a graph replay refreshes them too)
+    # the experts alone (no gate, routing, encode, decode), on the dispatch buffer of one eager call of the same mode
+    bufs = []
+    hook = layer.experts.register_forward_pre_hook(lambda m, a: bufs.append(a[0]))
+    eager(x)
+    hook.remove()
+    _, expert_times = timed(lambda: layer.experts(bufs[-1], layer), args.iters)
+    padded = layer(x)
+bytes_per_expert = sum(p.numel() * p.element_size() for p in layer.experts.parameters()) // args.experts
+median, expert_median = times[len(times) // 2], expert_times[len(expert_times) // 2]
+print(json.dumps({'impl': args.impl, 'config': 'dropless cf=0 top-%d E=%d tokens=%d dim=%d hidden=%d %s %s megablocks_size=%d%s' % (
+    args.top_k, args.experts, args.tokens, args.dim, hidden, args.expert_type, args.dtype, args.megablocks_size,
+    ' cuda-graph' if args.graph and args.impl == 'ours' else ''), 'median_ms': median, 'min_ms': times[0], 'max_ms': times[-1],
+    'experts_median_ms': expert_median, 'active_experts': active, 'active_weight_bytes': active * bytes_per_expert,
+    'active_weight_GBps': active * bytes_per_expert / (median * 1e-3) / 1e9,
+    'experts_active_weight_GBps': active * bytes_per_expert / (expert_median * 1e-3) / 1e9,
+    'rel_err_vs_padded': float((y.float() - padded.float()).norm() / padded.float().norm()),
     'checksum': float(y.float().abs().sum())}))

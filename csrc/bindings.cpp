@@ -605,6 +605,30 @@ at::Tensor skinny_ffn(const at::Tensor& x, const at::Tensor& w1, const c10::opti
   return y;
 }
 
+// x [G, R, M], w1 / w2 [G, M, H], w3 [G, H, N], counts int [G] or None -> fp32 [G, R, N]
+at::Tensor skinny_glu_ffn(const at::Tensor& x, const at::Tensor& w1, const at::Tensor& w2, const at::Tensor& w3,
+                          const c10::optional<at::Tensor>& counts, int64_t act) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 3 && w1.dim() == 3 && w2.dim() == 3 && w3.dim() == 3 && x.is_contiguous() &&
+              w1.is_contiguous() && w2.is_contiguous() && w3.is_contiguous(), "skinny_glu_ffn: needs contiguous 3-d CUDA tensors");
+  TORCH_CHECK(x.scalar_type() == w1.scalar_type() && x.scalar_type() == w2.scalar_type() && x.scalar_type() == w3.scalar_type(),
+              "skinny_glu_ffn: x and the weights must have one dtype");
+  TORCH_CHECK(x.size(0) == w1.size(0) && x.size(0) == w2.size(0) && x.size(0) == w3.size(0), "skinny_glu_ffn: group count mismatch");
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int G = static_cast<int>(x.size(0)), R = static_cast<int>(x.size(1)), M = static_cast<int>(x.size(2));
+  const int H = static_cast<int>(w1.size(2)), N = static_cast<int>(w3.size(2));
+  TORCH_CHECK(w1.size(1) == M && w2.sizes() == w1.sizes() && w3.size(1) == H, "skinny_glu_ffn: weight shapes do not match");
+  TORCH_CHECK(act >= 1 && act <= 3, "skinny_glu_ffn: act must be 1 (relu), 2 (gelu) or 3 (silu)");
+  at::Tensor y = at::zeros({G, R, N}, x.options().dtype(at::kFloat));
+  const int* c = nullptr;
+  if (counts.has_value() && counts->defined()) {
+    TORCH_CHECK(counts->is_cuda() && counts->scalar_type() == at::kInt && counts->numel() >= G);
+    c = counts->data_ptr<int>();
+  }
+  TB_CHECK_CUDA(tb::skinny_grouped_glu_ffn(x.data_ptr(), w1.data_ptr(), w2.data_ptr(), w3.data_ptr(), y.data_ptr<float>(), c, G,
+                                           R, M, H, N, static_cast<int>(act), elem_type_of(x), cur_stream()));
+  return y;
+}
+
 }  // namespace
 
 void register_symm_bindings(pybind11::module& m);  // symm_heap.cpp / p2p bindings
@@ -629,6 +653,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cumsum_sub_one", &cumsum_sub_one);
   m.def("skinny_gemm", &skinny_gemm);
   m.def("skinny_ffn", &skinny_ffn);
+  m.def("skinny_glu_ffn", &skinny_glu_ffn);
   m.def("quantize_rows", &quantize_rows);
   m.def("dequant_rows", &dequant_rows);
   m.def("quantize_transpose", &quantize_transpose);

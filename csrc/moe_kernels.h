@@ -110,4 +110,12 @@ cudaError_t skinny_grouped_ffn(const void* x, const void* w1, const void* b1, co
                                const int* counts, int G, int rows_cap, int K, int H, int N, int act, int elem_type,
                                cudaStream_t stream);
 
+// Whole SwiGLU expert for a few rows per expert in ONE launch (dropless / decoder inference):
+//   y[g, r, :] += (act(x[g, r, :] @ W1[g]) * (x[g, r, :] @ W2[g])) @ W3[g]   for r < counts[g]
+// x [G, rows_cap, M], W1 / W2 [G, M, H], W3 [G, H, N] (LlamaFFNNetwork's layouts, last dims contiguous), y fp32
+// [G, rows_cap, N] ZERO-INITIALISED.  M, H, N multiples of 16 bytes' worth of elements; cudaErrorInvalidValue when the
+// staged rows of x do not fit in the same 200 KB of shared memory as skinny_grouped_ffn (M > 12224).  act: as above.
+cudaError_t skinny_grouped_glu_ffn(const void* x, const void* w1, const void* w2, const void* w3, float* y, const int* counts,
+                                   int G, int rows_cap, int M, int H, int N, int act, int elem_type, cudaStream_t stream);
+
 }  // namespace tb

@@ -139,6 +139,7 @@ cudaError_t launch(const void* x, const void* w, const void* bias, void* y, cons
 // per lane; experts without tokens cost one block exit.  No host synchronisation: counts are read on the device.
 constexpr int kHS = 64;         // hidden units per block
 constexpr int kFfnRows = 4;     // rows per pass (more rows re-stream the slice); keeps the kernel at <= 128 registers, 2 blocks / SM
+constexpr size_t kFfnSmemLimit = 200 * 1024;   // dynamic shared memory (staged x rows + slice buffers) per block
 
 template <typename T> struct WVec;
 template <> struct WVec<float> {
@@ -179,6 +180,71 @@ __device__ __forceinline__ float ffn_act(float v, int act) {
   if (act == 2) return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));
   if (act == 3) return v / (1.0f + __expf(-v));
   return v;
+}
+
+// Stage rows [r0, r0 + nr) of x[g] ([rows, K], fp32 in shared memory) for one pass.  Passes of 3-4 rows run the
+// kFfnRows specialisation, so its missing rows are zeroed (they then contribute zeros and are never stored).
+template <typename T>
+__device__ __forceinline__ void stage_rows(float* __restrict__ xs, const T* __restrict__ xrow0, int nr, int K) {
+  constexpr int V = WVec<T>::N;
+  __syncthreads();
+  for (int i = threadIdx.x * V; i < nr * K; i += 256 * V) {
+    float f[V];
+    WVec<T>::load(xrow0 + i, f);
+#pragma unroll
+    for (int q = 0; q < V; ++q) xs[i + q] = f[q];
+  }
+  if (nr > 2)
+    for (int i = threadIdx.x + nr * K; i < kFfnRows * K; i += 256) xs[i] = 0.0f;
+  __syncthreads();
+}
+
+// Second layer of a pass: yrow0[r, :] += hsm[r, :hs] @ w2g[:hs, :] (+ b2g) for r < nr, with fp32 atomics.  w2g points at
+// the block's hs rows of the [H, N] weight (N contiguous); each thread owns V output columns per pass and walks the rows.
+template <typename T, int ROWS>
+__device__ __forceinline__ void ffn_layer2(const float* __restrict__ hsm, const T* __restrict__ w2g, const T* __restrict__ b2g,
+                                           float* __restrict__ yrow0, int nr, int hs, int N, bool add_bias) {
+  constexpr int V = WVec<T>::N;
+  for (int n = threadIdx.x * V; n < N; n += 256 * V) {
+    float acc[ROWS][V];
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+      for (int q = 0; q < V; ++q) acc[r][q] = 0.0f;
+    for (int j = 0; j < hs; j += 8) {
+      float wv[8][V];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        if (j + u < hs) WVec<T>::load(w2g + static_cast<long long>(j + u) * N + n, wv[u]);
+        else {
+#pragma unroll
+          for (int q = 0; q < V; ++q) wv[u][q] = 0.0f;
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        if (j + u < hs) {
+#pragma unroll
+          for (int r = 0; r < ROWS; ++r) {
+            const float hv = hsm[r * kHS + j + u];
+#pragma unroll
+            for (int q = 0; q < V; ++q) acc[r][q] = fmaf(hv, wv[u][q], acc[r][q]);
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) {
+      if (r < nr) {
+#pragma unroll
+        for (int q = 0; q < V; ++q) {
+          float v = acc[r][q];
+          if (add_bias) v += ldf<T>(b2g + n + q);
+          atomicAdd(yrow0 + static_cast<long long>(r) * N + n + q, v);
+        }
+      }
+    }
+  }
 }
 
 // One pass over this block's weight slices for ROWS (compile-time) rows: the inner products cost ROWS shared-memory reads
@@ -230,47 +296,7 @@ __device__ __forceinline__ void ffn_pass(const float* __restrict__ xs, float* __
     }
   }
   __syncthreads();
-  // ---- layer 2: each thread owns V output columns per pass and walks the slice's rows of W2 ----
-  for (int n = threadIdx.x * V; n < N; n += 256 * V) {
-    float acc[ROWS][V];
-#pragma unroll
-    for (int r = 0; r < ROWS; ++r)
-#pragma unroll
-      for (int q = 0; q < V; ++q) acc[r][q] = 0.0f;
-    for (int j = 0; j < hs; j += 8) {
-      float wv[8][V];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        if (j + u < hs) WVec<T>::load(w2g + static_cast<long long>(j + u) * N + n, wv[u]);
-        else {
-#pragma unroll
-          for (int q = 0; q < V; ++q) wv[u][q] = 0.0f;
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        if (j + u < hs) {
-#pragma unroll
-          for (int r = 0; r < ROWS; ++r) {
-            const float hv = hsm[r * kHS + j + u];
-#pragma unroll
-            for (int q = 0; q < V; ++q) acc[r][q] = fmaf(hv, wv[u][q], acc[r][q]);
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int r = 0; r < ROWS; ++r) {
-      if (r < nr) {
-#pragma unroll
-        for (int q = 0; q < V; ++q) {
-          float v = acc[r][q];
-          if (add_bias) v += ldf<T>(b2g + n + q);
-          atomicAdd(yrow0 + static_cast<long long>(r) * N + n + q, v);
-        }
-      }
-    }
-  }
+  ffn_layer2<T, ROWS>(hsm, w2g, b2g, yrow0, nr, hs, N, add_bias);
 }
 
 template <typename T>
@@ -279,7 +305,6 @@ skinny_ffn_kernel(const T* __restrict__ x, const T* __restrict__ w1, const T* __
                   const T* __restrict__ b2, float* __restrict__ y, const int* __restrict__ counts, int rows_cap, int K,
                   int H, int N, int act) {
   extern __shared__ float sm[];                 // x rows [kFfnRows][K] | hidden slice [kFfnRows][kHS]
-  constexpr int V = WVec<T>::N;
   const int g = blockIdx.y;
   const int count = counts != nullptr ? min(counts[g], rows_cap) : rows_cap;
   if (count <= 0) return;
@@ -297,23 +322,11 @@ skinny_ffn_kernel(const T* __restrict__ x, const T* __restrict__ w1, const T* __
 
   for (int r0 = 0; r0 < count; r0 += kFfnRows) {
     const int nr = min(kFfnRows, count - r0);
-    __syncthreads();
-    for (int i = threadIdx.x * V; i < nr * K; i += 256 * V) {
-      const int r = i / K, k = i - r * K;
-      float f[V];
-      WVec<T>::load(xg + static_cast<long long>(r0 + r) * K + k, f);
-#pragma unroll
-      for (int q = 0; q < V; ++q) xs[i + q] = f[q];
-    }
-    __syncthreads();
+    stage_rows<T>(xs, xg + static_cast<long long>(r0) * K, nr, K);
     float* yrow0 = yg + static_cast<long long>(r0) * N;
     if (nr == 1) ffn_pass<T, 1>(xs, hsm, w1g, b1g, w2g, b2g, yrow0, nr, K, hs, N, act, add_bias);
     else if (nr == 2) ffn_pass<T, 2>(xs, hsm, w1g, b1g, w2g, b2g, yrow0, nr, K, hs, N, act, add_bias);
-    else {
-      for (int i = threadIdx.x + nr * K; i < kFfnRows * K; i += 256) xs[i] = 0.0f;       // rows [nr, 4) of the staged block
-      __syncthreads();
-      ffn_pass<T, kFfnRows>(xs, hsm, w1g, b1g, w2g, b2g, yrow0, nr, K, hs, N, act, add_bias);
-    }
+    else ffn_pass<T, kFfnRows>(xs, hsm, w1g, b1g, w2g, b2g, yrow0, nr, K, hs, N, act, add_bias);
   }
 }
 
@@ -323,7 +336,7 @@ cudaError_t launch_ffn(const void* x, const void* w1, const void* b1, const void
   constexpr int V = WVec<T>::N;
   if (K % V || N % V) return cudaErrorInvalidValue;
   const size_t smem = sizeof(float) * (static_cast<size_t>(kFfnRows) * K + kFfnRows * kHS);
-  if (smem > 200 * 1024) return cudaErrorInvalidValue;
+  if (smem > kFfnSmemLimit) return cudaErrorInvalidValue;
   auto* kern = skinny_ffn_kernel<T>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -332,6 +345,134 @@ cudaError_t launch_ffn(const void* x, const void* w1, const void* b1, const void
   dim3 grid((H + kHS - 1) / kHS, G);
   kern<<<grid, 256, smem, stream>>>(static_cast<const T*>(x), static_cast<const T*>(w1), static_cast<const T*>(b1),
                                     static_cast<const T*>(w2), static_cast<const T*>(b2), y, counts, rows_cap, K, H, N, act);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// SwiGLU expert for a few rows per expert in ONE launch:  y[g] += (act(x[g] @ W1[g]) * (x[g] @ W2[g])) @ W3[g]
+// ------------------------------------------------------------------------------------------------
+// W1, W2 are [G, M, H] and W3 [G, H, N], all with the last dim contiguous (LlamaFFNNetwork's parameters).  Block (g, s)
+// owns hidden units [s*kHS, s*kHS + kHS): in layer 1 it reads the kHS-wide column strip of every one of the M rows of
+// both W1 and W2 (64 contiguous elements: 256 bytes in fp32, 128 bytes in 16 bit, so every segment is whole 128-byte
+// lines).  Warps 0-3 stream W1 and warps 4-7 stream W2 over the same staged rows of x: kHS / V lanes cover one row
+// segment with 16-byte loads, the other lanes and warps stride M.  The gate and up partial sums are reduced across the
+// lanes of a warp with shuffles and across the four warps of each matrix in shared memory, where they become
+// act(gate) * up.  Layer 2 is the FFN kernel's W2 pass over the slice's kHS rows of W3.
+constexpr int kGluWarps = 8;                    // 4 warps per layer-1 matrix
+
+template <typename T, int ROWS>
+__device__ __forceinline__ void glu_pass(const float* __restrict__ xs, float* __restrict__ part, float* __restrict__ hsm,
+                                         const T* __restrict__ w1g, const T* __restrict__ w2g, const T* __restrict__ w3g,
+                                         float* __restrict__ yrow0, int nr, int M, int H, int hs, int N, int act) {
+  constexpr int V = WVec<T>::N;
+  constexpr int LPR = kHS / V;                  // lanes per row segment: 8 (16 bit) or 16 (fp32)
+  constexpr int KLW = 32 / LPR;                 // rows of one matrix per warp and load
+  constexpr int KL = 4 * KLW;                   // rows of one matrix per load over its four warps
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int c = (lane % LPR) * V;               // first hidden unit of this lane inside the slice
+  const int kl = (warp & 3) * KLW + lane / LPR;
+  const T* wg = (warp < 4 ? w1g : w2g) + c;
+  float acc[ROWS][V];
+#pragma unroll
+  for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+    for (int q = 0; q < V; ++q) acc[r][q] = 0.0f;
+  if (c < hs) {
+    for (int k = kl; k < M; k += KL * 4) {
+      float wv[4][V];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int kk = k + u * KL;
+        if (kk < M) WVec<T>::load(wg + static_cast<long long>(kk) * H, wv[u]);
+        else {
+#pragma unroll
+          for (int q = 0; q < V; ++q) wv[u][q] = 0.0f;
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int kk = k + u * KL;
+        if (kk < M) {
+#pragma unroll
+          for (int r = 0; r < ROWS; ++r) {
+            const float xv = xs[r * M + kk];
+#pragma unroll
+            for (int q = 0; q < V; ++q) acc[r][q] = fmaf(xv, wv[u][q], acc[r][q]);
+          }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+    for (int q = 0; q < V; ++q)
+#pragma unroll
+      for (int o = LPR; o < 32; o <<= 1) acc[r][q] += __shfl_xor_sync(0xffffffffu, acc[r][q], o);
+  if (lane < LPR) {
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+      for (int q = 0; q < V; ++q) part[(warp * kFfnRows + r) * kHS + c + q] = acc[r][q];
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < ROWS * kHS; i += 256) {
+    float gs = 0.0f, us = 0.0f;
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      gs += part[w * kFfnRows * kHS + i];
+      us += part[(w + 4) * kFfnRows * kHS + i];
+    }
+    hsm[i] = ffn_act(gs, act) * us;
+  }
+  __syncthreads();
+  ffn_layer2<T, ROWS>(hsm, w3g, nullptr, yrow0, nr, hs, N, false);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256, 2)
+skinny_glu_ffn_kernel(const T* __restrict__ x, const T* __restrict__ w1, const T* __restrict__ w2, const T* __restrict__ w3,
+                      float* __restrict__ y, const int* __restrict__ counts, int rows_cap, int M, int H, int N, int act) {
+  extern __shared__ float sm[];                 // x rows [kFfnRows][M] | hidden slice [kFfnRows][kHS] | partial sums
+  const int g = blockIdx.y;
+  const int count = counts != nullptr ? min(counts[g], rows_cap) : rows_cap;
+  if (count <= 0) return;
+  const int h0 = blockIdx.x * kHS;
+  const int hs = min(kHS, H - h0);
+  float* xs = sm;
+  float* hsm = xs + kFfnRows * M;
+  float* part = hsm + kFfnRows * kHS;           // [kGluWarps][kFfnRows][kHS]
+  const T* xg = x + static_cast<long long>(g) * rows_cap * M;
+  const T* w1g = w1 + static_cast<long long>(g) * M * H + h0;
+  const T* w2g = w2 + static_cast<long long>(g) * M * H + h0;
+  const T* w3g = w3 + (static_cast<long long>(g) * H + h0) * N;
+  float* yg = y + static_cast<long long>(g) * rows_cap * N;
+
+  for (int r0 = 0; r0 < count; r0 += kFfnRows) {
+    const int nr = min(kFfnRows, count - r0);
+    stage_rows<T>(xs, xg + static_cast<long long>(r0) * M, nr, M);
+    float* yrow0 = yg + static_cast<long long>(r0) * N;
+    if (nr == 1) glu_pass<T, 1>(xs, part, hsm, w1g, w2g, w3g, yrow0, nr, M, H, hs, N, act);
+    else if (nr == 2) glu_pass<T, 2>(xs, part, hsm, w1g, w2g, w3g, yrow0, nr, M, H, hs, N, act);
+    else glu_pass<T, kFfnRows>(xs, part, hsm, w1g, w2g, w3g, yrow0, nr, M, H, hs, N, act);
+  }
+}
+
+template <typename T>
+cudaError_t launch_glu_ffn(const void* x, const void* w1, const void* w2, const void* w3, float* y, const int* counts, int G,
+                           int rows_cap, int M, int H, int N, int act, cudaStream_t stream) {
+  constexpr int V = WVec<T>::N;
+  if (M % V || H % V || N % V) return cudaErrorInvalidValue;
+  const size_t smem = sizeof(float) * (static_cast<size_t>(kFfnRows) * M + (1 + kGluWarps) * kFfnRows * kHS);
+  if (smem > kFfnSmemLimit) return cudaErrorInvalidValue;
+  auto* kern = skinny_glu_ffn_kernel<T>;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+  }
+  dim3 grid((H + kHS - 1) / kHS, G);
+  kern<<<grid, 256, smem, stream>>>(static_cast<const T*>(x), static_cast<const T*>(w1), static_cast<const T*>(w2),
+                                    static_cast<const T*>(w3), y, counts, rows_cap, M, H, N, act);
   return cudaGetLastError();
 }
 
@@ -356,6 +497,19 @@ cudaError_t skinny_grouped_ffn(const void* x, const void* w1, const void* b1, co
     case ET_F32: return launch_ffn<float>(x, w1, b1, w2, b2, y, counts, G, rows_cap, K, H, N, act, stream);
     case ET_F16: return launch_ffn<__half>(x, w1, b1, w2, b2, y, counts, G, rows_cap, K, H, N, act, stream);
     case ET_BF16: return launch_ffn<__nv_bfloat16>(x, w1, b1, w2, b2, y, counts, G, rows_cap, K, H, N, act, stream);
+  }
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t skinny_grouped_glu_ffn(const void* x, const void* w1, const void* w2, const void* w3, float* y, const int* counts,
+                                   int G, int rows_cap, int M, int H, int N, int act, int elem_type, cudaStream_t stream) {
+  if (G <= 0 || rows_cap <= 0 || M <= 0 || H <= 0 || N <= 0) return cudaSuccess;
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w1) | reinterpret_cast<uintptr_t>(w2) |
+       reinterpret_cast<uintptr_t>(w3)) & 15) return cudaErrorInvalidValue;
+  switch (elem_type) {
+    case ET_F32: return launch_glu_ffn<float>(x, w1, w2, w3, y, counts, G, rows_cap, M, H, N, act, stream);
+    case ET_F16: return launch_glu_ffn<__half>(x, w1, w2, w3, y, counts, G, rows_cap, M, H, N, act, stream);
+    case ET_BF16: return launch_glu_ffn<__nv_bfloat16>(x, w1, w2, w3, y, counts, G, rows_cap, M, H, N, act, stream);
   }
   return cudaErrorInvalidValue;
 }

@@ -19,9 +19,12 @@ import torch.nn.functional as F
 from ...ops import gemm as G
 from ...ops import mx as MX
 from ...parallel import communicate as C
+from . import dropless_row_counts
 
 
 class FusedExpertsNetwork(torch.nn.Module):
+    rows_independent = True      # each output row depends on its input row alone: dispatch may skip the zero padding
+
     def __init__(self, model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count, activation_fn=None,
                  activation_fn_with_self=None, output_dim=None, has_fc1_bias=True, has_fc2_bias=True, fp8=None):
         super().__init__()
@@ -122,14 +125,7 @@ class FusedExpertsNetwork(torch.nn.Module):
     def forward(self, x, ctx):
         if self.skip_expert:
             return x
-        row_counts = None
-        if getattr(ctx, 'megablocks_size', 0) > 0:
-            mb = ctx.megablocks_size
-            if mb == 1 and ctx.dispatch_count.dtype == torch.int32:
-                row_counts = ctx.dispatch_count          # the kernels clamp to the buffer's rows themselves: no extra launches
-            else:
-                groups = torch.div(ctx.dispatch_count + (mb - 1), mb, rounding_mode='floor')
-                row_counts = (torch.clamp(groups, max=x.size(1) // mb) * mb).to(torch.int32)
+        row_counts = dropless_row_counts(x, ctx)
         w1, b1, w2, b2 = self.materialize(ctx)
         return self.compute(x, w1, b1, w2, b2, row_counts)
 

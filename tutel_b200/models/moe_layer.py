@@ -276,8 +276,9 @@ class MOELayer(torch.nn.Module):
                         bound = S
                 crit, l_aux = fused_extract_critical(logits_w_noise, top_k, cf, self.normalize_gate, alignment, self.group,
                                                      inequivalent_tokens, rows_bound=bound)
-                if getattr(crit, 'skip_padding', False) and not hasattr(self.experts, 'batched_fc1_w'):
-                    crit.skip_padding = False      # custom experts see every row of the buffer: keep the zero padding
+                if getattr(crit, 'skip_padding', False) and not getattr(self.experts, 'rows_independent', False):
+                    # experts that do not declare `rows_independent = True` may mix rows of the buffer: keep the zero padding
+                    crit.skip_padding = False
                 return logits.dtype, crit, l_aux
             # same formulas, op by op (CPU, batch-prioritised routing): one autograd node for softmax + top-k + loss
             fused_gate = fused_topk_gate(logits_w_noise, k_eff, self.normalize_gate, True)
@@ -337,6 +338,7 @@ class MOELayer(torch.nn.Module):
 
         self.megablocks_size = megablocks_size
         self.dispatch_count = get_dispatch_count(crit)
+        self.top_k = min(top_k, self.num_global_experts)      # choices per token of this call (experts size their paths by it)
         if adaptive_r is not None:
             self.adaptive_degree = adaptive_r
 

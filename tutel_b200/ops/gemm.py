@@ -266,6 +266,7 @@ def can_use_skinny(x: torch.Tensor, w: torch.Tensor) -> bool:
 
 
 _SKINNY_ACTS = {'relu': 1, 'gelu': 2, 'silu': 3}
+SKINNY_PASS_ROWS = 4        # rows of an expert per weight pass of the skinny FFN kernels (kFfnRows, csrc/skinny_gemm.cu)
 
 
 def can_use_skinny_ffn(x: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, act_kind) -> bool:
@@ -282,6 +283,23 @@ def skinny_ffn(x, w1, b1, w2, b2, row_counts, act_kind):
     b2 = None if b2 is None else b2.reshape(w2.size(0), -1).contiguous()
     y = backend.require_ext().skinny_ffn(x.contiguous(), w1.contiguous(), b1, w2.contiguous(), b2, row_counts,
                                          _SKINNY_ACTS[act_kind])
+    return y if y.dtype == x.dtype else y.to(x.dtype)
+
+
+def can_use_skinny_glu_ffn(x: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch.Tensor, act_kind) -> bool:
+    """The whole SwiGLU expert in one weight-streaming launch (csrc/skinny_gemm.cu: skinny_glu_ffn_kernel)."""
+    v = 16 // x.element_size()
+    return (can_use_skinny(x, w1) and act_kind in _SKINNY_ACTS and w2.dtype == w1.dtype and w3.dtype == w1.dtype and
+            w1.dim() == 3 and w1.size(1) == x.size(2) and w2.shape == w1.shape and w3.dim() == 3 and
+            w3.size(1) == w1.size(2) and x.size(2) % v == 0 and w1.size(2) % v == 0 and w3.size(2) % v == 0 and
+            16 * x.size(2) + 9 * 1024 <= 100 * 1024)
+
+
+def skinny_glu_ffn(x, w1, w2, w3, row_counts, act_kind):
+    """y[g, r] = (act(x[g, r] @ W1[g]) * (x[g, r] @ W2[g])) @ W3[g] for r < row_counts[g]; other rows are zero."""
+    backend.count_launch(2)          # zero-fill of the fp32 accumulator + the kernel
+    y = backend.require_ext().skinny_glu_ffn(x.contiguous(), w1.contiguous(), w2.contiguous(), w3.contiguous(), row_counts,
+                                             _SKINNY_ACTS[act_kind])
     return y if y.dtype == x.dtype else y.to(x.dtype)
 
 
@@ -454,29 +472,35 @@ class FusedGLUFFN(torch.autograd.Function):
     Here: 2 launches forward (dual-B GLU GEMM, down projection), 4-6 backward (dh GEMM whose epilogue emits dg and du,
     three wgrads, optionally two dgrads with the add fused), no elementwise kernels at all.
     ``w1, w2: [G, M, H]``, ``w3: [G, H, Mout]`` (all "kn", the reference's parameter layout).
+    ``row_counts`` (int32 [G], dropless inference only): rows at or past the count of a group are skipped and left
+    undefined in the result; there is no backward for it.
     """
 
     @staticmethod
-    def forward(ctx: Any, x, w1, w2, w3, act: str, fp8: bool):
+    def forward(ctx: Any, x, w1, w2, w3, act: str, fp8: bool, row_counts=None):
         need_grad = any(ctx.needs_input_grad[:4])
         if fp8:
             xq, sx = quantize_rows(x)
             (q1, s1), (q2, s2), (q3, s3) = fp8_weight(w1, 'kn'), fp8_weight(w2, 'kn'), fp8_weight(w3, 'kn')
             h, g, u = glu_gemm(xq, q1, q2, b_mn=False, act=act, save_pre=need_grad, scale_a=sx, scale_b=s1, scale_b2=s2,
-                               out_dtype=x.dtype)
+                               row_counts=row_counts, out_dtype=x.dtype)
             hq, sh = quantize_rows(h)
-            y = raw_gemm(hq, q3, out_dtype=x.dtype, scale_a=sh, scale_b=s3)
+            y = raw_gemm(hq, q3, row_counts=row_counts, out_dtype=x.dtype, scale_a=sh, scale_b=s3)
             ctx.fp8 = True
         else:
-            h, g, u = glu_gemm(x, w1, w2, b_mn=True, act=act, save_pre=need_grad)
-            y = raw_gemm(h, w3, b_mn=True)
+            h, g, u = glu_gemm(x, w1, w2, b_mn=True, act=act, save_pre=need_grad, row_counts=row_counts)
+            y = raw_gemm(h, w3, b_mn=True, row_counts=row_counts)
         ctx.act = act
+        ctx.has_row_counts = row_counts is not None
         if need_grad:
             ctx.save_for_backward(x, w1, w2, w3, g, u, h)
         return y
 
     @staticmethod
     def backward(ctx: Any, dy: torch.Tensor):
+        if ctx.has_row_counts:
+            raise RuntimeError('FusedGLUFFN: row_counts is for no-grad dropless inference; backward through it is not '
+                               'supported')
         x, w1, w2, w3, g, u, h = ctx.saved_tensors
         dy = dy if _ok_stride(dy) else dy.contiguous()
         if getattr(ctx, 'fp8', False):
@@ -498,8 +522,8 @@ class FusedGLUFFN(torch.autograd.Function):
         elif ctx.needs_input_grad[0]:
             dx = raw_gemm(dg, w1)                                            # [T,M] = dg @ W1^T
             dx = raw_gemm(du, w2, epilogue=EPI_ADD, aux=dx)                  # += du @ W2^T (add fused in the epilogue)
-        return dx, dw1, dw2, dw3, None, None
+        return dx, dw1, dw2, dw3, None, None, None
 
 
-def fused_glu_ffn(x, w1, w2, w3, act='silu', fp8=False):
-    return FusedGLUFFN.apply(x, w1, w2, w3, act, fp8)
+def fused_glu_ffn(x, w1, w2, w3, act='silu', fp8=False, row_counts=None):
+    return FusedGLUFFN.apply(x, w1, w2, w3, act, fp8, row_counts)
