@@ -6,17 +6,20 @@
 // (384 threads, 128 x 256 output tiles; 128 x 128 for the fused multi-GPU engine, the GLU epilogues, fp32 outputs and
 // block_n=128, see Cfg and gemm_sm90_launch):
 //
-//   warp 0        TMA producer   cp.async.bulk.tensor (128B swizzle) -> smem ring, mbarrier complete_tx; the other
-//                                three warps of its warpgroup only give their registers away (setmaxnreg).  128 x 256:
-//                                also loads the tile's aux operand (ReLU / activation gradient, add) into the output
-//                                tile while the main loop runs.
+//   warp 0        TMA producer   cp.async.bulk.tensor (128B swizzle) -> smem ring, mbarrier complete_tx.
+//   warp 1        store warp     (128 x 256 only) owns the output tile: TMA-stores each finished tile, then loads the next
+//                                tile's aux operand (ReLU / activation gradient, add) into it; bulk-copies every tile's
+//                                bias and fp8 column scales into shared memory while the main loop runs; adds up the
+//                                consumer warps' bias-gradient partial rows and issues the global reductions.
+//                                Warps 2, 3 (and warp 1 of the 128 x 128 configuration) only give their registers away
+//                                (setmaxnreg).
 //   warps 4..11   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async (m64n256 / m64n128, operands
 //                                straight from the swizzled ring, fp32 accumulator fragment in registers), one stage in
 //                                flight; a stage is handed back to the producer when the wgmma group that read it has retired.
 //                                128 x 256 epilogue: scales / bias / activation / aux math on the fragment in registers,
 //                                packed into the 16-bit output tile in the TMA box layout, bias-gradient column sums
-//                                reduced in the CTA; one thread issues the TMA store and all consumers go on to the next
-//                                tile's main loop while it drains (see wide_main and flush_out_tile).
+//                                reduced per warp; the tile is handed to the store warp (out_full) and the consumers go
+//                                straight on to the next tile's main loop (see wide_main and hand_over_tile).
 //                                128 x 128 epilogue: every warp parks 16 x 128 of its fragment in its own shared-memory
 //                                rows and reads it back with one lane per row and 32 consecutive columns per lane, applies
 //                                the fused bias / activation / activation-grad / GLU / bias-grad math in fp32 and writes
@@ -92,10 +95,11 @@ constexpr int kSmemLimit = 232448;   // 227 KB
 //           budget above gemm_sm90_kernel).
 //   BN 256  m64n256 wgmma per consumer warpgroup (128 fp32 accumulators per thread): 48 KB of operands per 64-deep K
 //           block for twice the FLOPs of a 128 x 128 tile's 32 KB, and each warpgroup's B reads from shared memory
-//           serve 256 instead of 128 columns.  16-bit output only.  3 stages of 48 KB, the 64 KB output tile, barriers
-//           and two 1 KB bias-gradient rows (212 KB), 168 registers per thread (producer warpgroup 40, consumers 232),
-//           one CTA per SM.  The epilogue works on the accumulator fragment in registers and hands the tile to a TMA
-//           store, so the consumers start the next tile's main loop while the store drains (see wide_epilogue).
+//           serve 256 instead of 128 columns.  16-bit output only.  3 stages of 48 KB, the 64 KB output tile, barriers,
+//           eight 1 KB bias-gradient partial rows (one per consumer warp) and two 2 KB side-input slots (bias and
+//           column scales of two consecutive tiles): 221.5 KB.  168 registers per thread (producer warpgroup 40,
+//           consumers 232), one CTA per SM.  The epilogue works on the accumulator fragment in registers and hands the
+//           tile to the store warp, so the consumers start the next tile's main loop while the store drains.
 template <int BN_>
 struct Cfg {
   static constexpr int BM = 128;
@@ -111,15 +115,19 @@ struct Cfg {
   static constexpr int EPI_WARP_BYTES = 16 * EPI_PITCH * 4;
   static constexpr int EPI_BYTES = WIDE ? 0 : 8 * EPI_WARP_BYTES;
   // 128 x 256 output tile in 16 bit, as the TMA boxes of the output tensor map: four boxes of 128 rows x 64 columns
-  // (128 B per row, 128-byte swizzle).  It also receives the tile's aux operand, and its bias-gradient rows.
+  // (128 B per row, 128-byte swizzle).  It also receives the tile's aux operand.
   static constexpr int OUT_BOX_BYTES = BM * kSwizzleBytes;
   static constexpr int OUT_TILE_BYTES = WIDE ? BM * BN * 2 : 0;
-  static constexpr int COLSUM_BYTES = WIDE ? 2 * BN * 4 : 0;   // double-buffered: tile i+2 reuses tile i's row
+  static constexpr int COLSUM_BYTES = WIDE ? 8 * BN * 4 : 0;      // per consumer warp one row of BN column sums
+  static constexpr int SIDE_BIAS_BYTES = BN * 4;                  // bias of one tile (16-bit or fp32) ...
+  static constexpr int SIDE_SLOT_BYTES = SIDE_BIAS_BYTES + BN * 4;   // ... and its fp32 column scales
+  static constexpr int SIDE_BYTES = WIDE ? 2 * SIDE_SLOT_BYTES : 0;  // double-buffered: tile i+1's lands during tile i
   static constexpr int BAR_BYTES = 512;
   static constexpr int STAGES = WIDE ? 3 : 4;
   static constexpr int MAXNREG = WIDE ? 168 : 144;
   static constexpr int CONSUMER_REGS = WIDE ? 232 : 192;   // producer warpgroup: 40
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + OUT_TILE_BYTES + BAR_BYTES + EPI_BYTES + COLSUM_BYTES;
+  static constexpr int SMEM_BYTES =
+      STAGES * STAGE_BYTES + 1024 + OUT_TILE_BYTES + BAR_BYTES + EPI_BYTES + COLSUM_BYTES + SIDE_BYTES;
   static_assert((STAGES * STAGE_BYTES) % 1024 == 0, "the output tile must stay 1024B aligned for the 128B swizzle");
   // 228 KB per SM, 1 KB reserved per resident block: a dispatch block (no shared memory of its own) must still fit
   static_assert(WIDE || SMEM_BYTES + 2 * 1024 <= 228 * 1024, "no room for the push kernel");
@@ -292,12 +300,13 @@ __device__ __forceinline__ uint32_t out_tile_off(int j, int swz) {
   return static_cast<uint32_t>((j >> 3) * (128 * kSwizzleBytes) + (((j & 7) ^ swz) << 4));
 }
 
-// fp8 operands: acc *= scale_a[m] * scale_b[n]  (sb: this group's column scales or null)
-__device__ __forceinline__ void wide_scale(float (&acc)[128], float sa0, float sa1, const float* sb, int n_lane, int N) {
+// fp8 operands: acc *= scale_a[m] * scale_b[n]  (sb: this tile's column scales in shared memory, or null).  Columns are
+// counted from the tile's first: n_lane = 2 (lane % 4), n_lim = N - n0.
+__device__ __forceinline__ void wide_scale(float (&acc)[128], float sa0, float sa1, const float* sb, int n_lane, int n_lim) {
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
     const int n = n_lane + 8 * j;
-    if (sb != nullptr && n < N) {
+    if (sb != nullptr && n < n_lim) {
       const float2 s = *reinterpret_cast<const float2*>(sb + n);
       acc[4 * j] *= sa0 * s.x; acc[4 * j + 1] *= sa0 * s.y;
       acc[4 * j + 2] *= sa1 * s.x; acc[4 * j + 3] *= sa1 * s.y;
@@ -308,10 +317,11 @@ __device__ __forceinline__ void wide_scale(float (&acc)[128], float sa0, float s
   }
 }
 
-// alpha / bias / aux math.  The aux operand is read from the output tile (this thread's words at row0 and row0 + 8 rows).
+// alpha / bias / aux math.  The aux operand is read from the output tile (this thread's words at row0 and row0 + 8 rows),
+// the bias from the tile's side-input slot (columns counted from the tile's first, as in wide_scale).
 template <int WM>
-__device__ __forceinline__ void wide_main(float (&acc)[128], const uint8_t* row0, int swz, const uint8_t* bias_g,
-                                          bool bias_f32, bool bias_bf16, int n_lane, int N, bool out_bf16, float alpha) {
+__device__ __forceinline__ void wide_main(float (&acc)[128], const uint8_t* row0, int swz, const uint8_t* bias_s,
+                                          bool bias_f32, bool bias_bf16, int n_lane, int n_lim, bool out_bf16, float alpha) {
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
     if constexpr (WM == WM_NONE) {
@@ -320,9 +330,9 @@ __device__ __forceinline__ void wide_main(float (&acc)[128], const uint8_t* row0
     } else if constexpr (WM == WM_BIAS) {
       const int n = n_lane + 8 * j;
       float2 b = make_float2(0.0f, 0.0f);
-      if (n < N)
-        b = bias_f32 ? *reinterpret_cast<const float2*>(bias_g + n * 4)
-                     : unpack2(*reinterpret_cast<const uint32_t*>(bias_g + n * 2), bias_bf16);
+      if (n < n_lim)
+        b = bias_f32 ? *reinterpret_cast<const float2*>(bias_s + n * 4)
+                     : unpack2(*reinterpret_cast<const uint32_t*>(bias_s + n * 2), bias_bf16);
       acc[4 * j] += b.x; acc[4 * j + 1] += b.y;
       acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
     } else {
@@ -360,9 +370,23 @@ __device__ __forceinline__ void wide_stage(const float (&acc)[128], uint8_t* row
   }
 }
 
+// One halving exchange of wide_colsum: lanes with bit OFF set keep the upper 2 OFF of the first 4 OFF sums, the others the
+// lower ones, each adding its partner's.  OFF is a compile-time constant so that every index of s is one, and s stays in
+// registers.
+template <int OFF>
+__device__ __forceinline__ void colsum_halve(float (&s)[64], int lane) {
+  const bool upper = (lane & OFF) != 0;
+#pragma unroll
+  for (int i = 0; i < 2 * OFF; ++i) {
+    const float lo = s[i], hi = s[i + 2 * OFF];
+    const float recv = __shfl_xor_sync(0xffffffffu, upper ? lo : hi, OFF);
+    s[i] = (upper ? hi : lo) + recv;
+  }
+}
 // Bias gradient: this thread's two rows (those below the valid row count) summed per column, then reduced over the
 // eight lanes that share its columns (lane bits 2..4) by halving exchanges, 32 + 16 + 8 shuffles: afterwards lane l
-// holds the warp's sums of columns 32 (l / 4) + 8 i + 2 (l % 4) + {0, 1}, i = 0..3, which go into the CTA's shared row.
+// holds the warp's sums of columns 32 (l / 4) + 8 i + 2 (l % 4) + {0, 1}, i = 0..3, which go into the warp's own row of
+// the partial sums (the store warp adds up the eight rows).
 __device__ __forceinline__ void wide_colsum(const float (&acc)[128], bool ok0, bool ok1, int lane, float* colrow) {
   float s[64];
 #pragma unroll
@@ -370,57 +394,37 @@ __device__ __forceinline__ void wide_colsum(const float (&acc)[128], bool ok0, b
 #pragma unroll
     for (int c = 0; c < 2; ++c) s[2 * j + c] = (ok0 ? acc[4 * j + c] : 0.0f) + (ok1 ? acc[4 * j + 2 + c] : 0.0f);
   }
-#pragma unroll
-  for (int off = 16; off >= 4; off >>= 1) {
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < 2 * off; ++i) {
-      const float send = upper ? s[i] : s[i + 2 * off];
-      const float recv = __shfl_xor_sync(0xffffffffu, send, off);
-      s[i] = (upper ? s[i + 2 * off] : s[i]) + recv;
-    }
-  }
+  colsum_halve<16>(s, lane);
+  colsum_halve<8>(s, lane);
+  colsum_halve<4>(s, lane);
   float* base = colrow + 32 * (lane >> 2) + 2 * (lane & 3);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) atomicAdd(base + 8 * (i >> 1) + (i & 1), s[i]);
+  for (int q = 0; q < 4; ++q) *reinterpret_cast<float2*>(base + 8 * q) = make_float2(s[2 * q], s[2 * q + 1]);
 }
 
-// The 128 x 256 output tile of group g at rows m0.., columns n0.. -> global memory.
-struct OutTileStore {
-  const uint8_t* tile;
-  uint32_t tile_smem;
-  int m0, n0, m_valid, N, g;
-  long long group_stride, ld;
-  bool straddle;       // rows from m_valid on must stay untouched: row-guarded copy instead of TMA
-  int ct;              // consumer thread 0..255
-  bool writer;         // the thread that issues (and later waits for) the TMA stores
-};
-// All 256 consumer threads call this after writing their words of the tile.  One thread issues the TMA store and
-// everyone moves on; with wait_read the tile may be overwritten as soon as this returns.
-__device__ __forceinline__ void flush_out_tile(const OutTileStore& s, const CUtensorMap* map, uint8_t* dst, bool wait_read) {
+// Consumers: hand the output tile of group g at rows m0.., columns n0.. to the store warp, called by all 256 consumer
+// threads after writing their words of the tile.  A tile that straddles the group's row count (rows from m_valid on must
+// stay untouched, which the output tensor map cannot express) is copied out here with row-guarded stores instead; the
+// store warp then only releases it.  Every warp arrives on out_full once it no longer reads the tile.
+__device__ __forceinline__ void hand_over_tile(const uint8_t* tile, bool straddle, int m0, int n0, int m_valid, int N, int g,
+                                               long long group_stride, long long ld, uint8_t* dst, int ct, int lane,
+                                               uint32_t out_full) {
   constexpr int kChunks = 256 / 8;   // 16-byte chunks per tile row
   ptx::fence_proxy_async_smem();     // this thread's tile writes -> visible to the async proxy (TMA)
-  ptx::named_bar_sync(1, 256);
-  if (s.straddle) {
-    for (int i = s.ct; i < 128 * kChunks; i += 256) {
+  if (straddle) {
+    ptx::named_bar_sync(1, 256);
+    for (int i = ct; i < 128 * kChunks; i += 256) {
       const int r = i / kChunks, ch = i % kChunks;
-      const int m = s.m0 + r, n = s.n0 + ch * 8;
-      if (m < s.m_valid && n < s.N) {
-        const uint4 v = *reinterpret_cast<const uint4*>(s.tile + (ch >> 3) * (128 * kSwizzleBytes) + r * kSwizzleBytes +
+      const int m = m0 + r, n = n0 + ch * 8;
+      if (m < m_valid && n < N) {
+        const uint4 v = *reinterpret_cast<const uint4*>(tile + (ch >> 3) * (128 * kSwizzleBytes) + r * kSwizzleBytes +
                                                         (((ch & 7) ^ (r & 7)) << 4));
-        *reinterpret_cast<uint4*>(dst + (static_cast<long long>(s.g) * s.group_stride + static_cast<long long>(m) * s.ld + n) * 2) = v;
+        *reinterpret_cast<uint4*>(dst + (static_cast<long long>(g) * group_stride + static_cast<long long>(m) * ld + n) * 2) = v;
       }
     }
-    ptx::named_bar_sync(1, 256);   // the tile has been read
-    return;
   }
-  if (s.writer) {
-    for (int b = 0; b < 4; ++b)
-      if (s.n0 + 64 * b < s.N) ptx::tma_store_3d(map, s.tile_smem + b * (128 * kSwizzleBytes), s.n0 + 64 * b, s.m0, s.g);
-    ptx::bulk_commit_group();
-    if (wait_read) ptx::bulk_wait_group_read<0>();
-  }
-  if (wait_read) ptx::named_bar_sync(1, 256);
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(out_full);
 }
 
 // Resource budget (deliberate): 384 threads x 144 registers = 55296 of the SM's 65536 registers (the producer warpgroup
@@ -451,16 +455,26 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   auto smem_b = [&](int s) { return smem_base + s * C::STAGE_BYTES + C::A_BYTES; };
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
-  // 128 x 256: the aux operand has landed in the output tile / the TMA store has finished reading the output tile
+  // 128 x 256: the aux operand has landed in the output tile / the store warp has finished reading the output tile / the
+  // consumers have handed the output tile to the store warp / a tile's side inputs have landed in slot 0 or 1
   const uint32_t aux_full = bar_base + 128u;
   const uint32_t out_empty = bar_base + 136u;
+  const uint32_t out_full = bar_base + 144u;
+  auto side_full = [&](uint32_t slot) { return bar_base + 152u + 8u * slot; };
   const uint32_t epi_base = bar_base + C::BAR_BYTES;
   float* epi_ptr = reinterpret_cast<float*>(smem_raw + (epi_base - ptx::smem_u32(smem_raw)));
   uint8_t* out_tile = smem_raw + (out_base - ptx::smem_u32(smem_raw));
-  float* colsum_rows = epi_ptr;   // 128 x 256: two rows of BN floats (EPI_BYTES is 0)
-  // The 128 x 256 epilogue reads the aux operand of RELU_BWD / ADD / ACT_BWD from the output tile; the producer loads
+  // 128 x 256 (EPI_BYTES is 0): eight rows of BN bias-gradient partial sums, then the two side-input slots
+  float* colsum_part = epi_ptr;
+  const uint32_t side_base = epi_base + C::COLSUM_BYTES;
+  // The 128 x 256 epilogue reads the aux operand of RELU_BWD / ADD / ACT_BWD from the output tile; the store warp loads
   // it there with TMA while the main loop runs.
   const bool aux_tma = C::WIDE && (args.epilogue == EPI_RELU_BWD || args.epilogue == EPI_ADD || args.epilogue == EPI_ACT_BWD);
+  // ... and the bias and column scales from the tile's side-input slot, which the store warp fills
+  const bool side_bias = C::WIDE && args.bias != nullptr && !aux_tma && args.epilogue != EPI_NONE;
+  const bool side_in = side_bias || (C::WIDE && args.scale_b != nullptr);
+  // BIAS_GELU / BIAS_SILU with a pre-activation output: every tile goes through the output tile twice (d2, then d)
+  const bool pre_act = C::WIDE && args.d2 != nullptr && (args.epilogue == EPI_BIAS_GELU || args.epilogue == EPI_BIAS_SILU);
 
   if (warp == 0 && ptx::elect_one()) {
     ptx::prefetch_tensormap(&tmA);
@@ -468,6 +482,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (args.dual) ptx::prefetch_tensormap(&tmB2);
     if (C::WIDE) ptx::prefetch_tensormap(&tmD);
     if (aux_tma) ptx::prefetch_tensormap(&tmAux);
+    if (pre_act) ptx::prefetch_tensormap(&tmD2);
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < stages; ++s) {
@@ -476,10 +491,10 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
     ptx::mbar_init(aux_full, 1);
     ptx::mbar_init(out_empty, 1);
+    ptx::mbar_init(out_full, 8);         // one arrival per consumer warp
+    ptx::mbar_init(side_full(0), 1);
+    ptx::mbar_init(side_full(1), 1);
     ptx::fence_mbar_init();
-  }
-  if constexpr (C::WIDE) {
-    for (int i = threadIdx.x; i < 2 * BN; i += kThreads) colsum_rows[i] = 0.0f;
   }
   __syncthreads();
 
@@ -494,10 +509,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   // 32-column gate / up / gradient segments do not fit the consumers' 232 registers.
   const bool dual = !C::WIDE && args.dual != 0;
   const int tile_n = dual ? BN / 2 : BN;   // output columns per tile
-  // 128 x 256: in the main loop of tile i, once K block kb_out_free has been issued, the thread that stored tile i - 1
-  // waits until that store has read the output tile and releases the tile (out_empty); the producer then loads tile i's
-  // aux operand into it.  Late enough that the store has normally drained, early enough to hide the aux load.
-  const int kb_out_free = min(2, num_kb - 1);
 
   if (warp < 4) {
     ptx::setmaxnreg_dec<40>();
@@ -505,7 +516,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       // =============================== TMA producer ===============================
       int s = 0;
       uint32_t ph = 0;
-      uint32_t it = 0;   // tiles processed
       int seen_group = -1;
       unsigned long long seen_mask = 0ull;
       for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
@@ -574,18 +584,113 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
           __syncwarp();
           if (++s == stages) { s = 0; ph ^= 1u; }
-          if (aux_tma && kb == kb_out_free) {
-            ptx::mbar_wait_quiet(out_empty, (it & 1u) ^ 1u);   // tile it - 1's store has read the output tile
-            if (ptx::elect_one()) {
-              ptx::mbar_expect_tx(aux_full, C::OUT_TILE_BYTES);
-              for (int b = 0; b < BN / 64; ++b)
-                ptx::tma_load_3d(out_base + b * C::OUT_BOX_BYTES, &tmAux, aux_full, n0 + 64 * b, m0, tc.g);
+        }
+      }
+    } else if (C::WIDE && warp == 1) {
+      // =============================== store warp (128 x 256) ===============================
+      // Walks the consumers' tile sequence one tile behind them.  Each time the consumers hand over the output tile
+      // (out_full), lane 0 TMA-stores it; the whole warp meanwhile adds up the bias-gradient partial rows; once the store
+      // has read the tile, it is released to the consumers: with the next tile's aux operand (aux_full) for the aux
+      // epilogues, by out_empty otherwise.  A tile's side inputs are copied into slot it % 2 when the consumers have handed
+      // over tile it - 1, which they could only do after they had read slot it % 2 for tile it - 2.
+      const int side_es = args.bias_is_fp32 ? 4 : 2;
+      uint32_t it = 0;     // tiles seen
+      uint32_t outs = 0;   // output tiles handed over so far (two per tile with pre_act)
+      TileCoord prev{};
+      int prev_m_valid = 0;
+      // Stores the tile the consumers hand over next, through `map`; then releases it (with `next`'s aux operand when
+      // has_next).
+      auto drain = [&](const CUtensorMap* map, const TileCoord& tc, int m_valid, bool colsum, bool has_next, TileCoord next) {
+        const int m0 = tc.m_blk * C::BM, n0 = tc.n_blk * BN;
+        const bool straddle = m0 + C::BM > m_valid && m_valid < args.M;   // the consumers copied it out row-guarded
+        ptx::mbar_wait_quiet(out_full, outs & 1u);
+        if (!straddle && lane == 0) {
+          for (int b = 0; b < BN / 64; ++b)
+            if (n0 + 64 * b < args.N) ptx::tma_store_3d(map, out_base + b * C::OUT_BOX_BYTES, n0 + 64 * b, m0, tc.g);
+          ptx::bulk_commit_group();
+        }
+        if (colsum) {
+          // the eight consumer warps' rows, added in warp order: lane l owns columns 4 l.. and 128 + 4 l..
+#pragma unroll 1
+          for (int h = 0; h < 2; ++h) {
+            const int c = 128 * h + 4 * lane;
+            float4 v = *reinterpret_cast<const float4*>(colsum_part + c);
+#pragma unroll
+            for (int w = 1; w < 8; ++w) {
+              const float4 p = *reinterpret_cast<const float4*>(colsum_part + w * BN + c);
+              v.x += p.x; v.y += p.y; v.z += p.z; v.w += p.w;
             }
-            __syncwarp();
+            const int n = n0 + c;
+            if (n < args.N) {   // N is a multiple of 8: all four columns are in range
+              float* cs = args.colsum + static_cast<long long>(tc.g / args.b_group_div) * args.colsum_group_stride + n;
+              if ((reinterpret_cast<uintptr_t>(cs) & 15) == 0) {
+                ptx::red_add_v4_f32(cs, v.x, v.y, v.z, v.w);
+              } else {
+                atomicAdd(cs, v.x); atomicAdd(cs + 1, v.y); atomicAdd(cs + 2, v.z); atomicAdd(cs + 3, v.w);
+              }
+            }
           }
         }
+        __syncwarp();   // every lane has read the partial rows
+        if (lane == 0) {
+          ptx::bulk_wait_group_read<0>();   // the store has read the output tile
+          if (has_next) {
+            ptx::mbar_expect_tx(aux_full, C::OUT_TILE_BYTES);
+            for (int b = 0; b < BN / 64; ++b)
+              ptx::tma_load_3d(out_base + b * C::OUT_BOX_BYTES, &tmAux, aux_full, next.n_blk * BN + 64 * b,
+                               next.m_blk * C::BM, next.g);
+          } else if (!aux_tma) {
+            ptx::mbar_arrive(out_empty);
+          }
+        }
+        __syncwarp();
+        ++outs;
+      };
+      for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
+        TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
+        tc.g = rotate_group(tc.g, args.group_rot, args.group_mod);
+        int m_valid = args.M;
+        if (args.row_counts != nullptr) {
+          m_valid = min(args.M, args.row_counts[tc.g]);
+          if (tc.m_blk * C::BM >= m_valid) continue;
+        }
+        if (it > 0 && pre_act) drain(&tmD2, prev, prev_m_valid, false, false, prev);
+        if (side_in) {
+          // tile it's bias / column scales -> slot it % 2 (the consumers have finished tile it - 2 once out_full of
+          // tile it - 1 has completed; with pre_act its first hand-over is enough)
+          if (it > 0 && !pre_act) ptx::mbar_wait_quiet(out_full, outs & 1u);
+          const int n0 = tc.n_blk * BN;
+          const int gb = tc.g / args.b_group_div;
+          const int cols = min(BN, args.N - n0);
+          const uint32_t slot = side_base + (it & 1u) * C::SIDE_SLOT_BYTES;
+          // (16-byte aligned: see gemm_sm90_launch)
+          const uint8_t* bsrc = reinterpret_cast<const uint8_t*>(args.bias) +
+                                (static_cast<long long>(gb) * args.bias_group_stride + n0) * side_es;
+          const float* ssrc = args.scale_b + static_cast<long long>(gb) * args.scale_b_group_stride + n0;
+          if (lane == 0) {
+            const uint32_t bar = side_full(it & 1u);
+            ptx::mbar_expect_tx(bar, (side_bias ? cols * side_es : 0) + (args.scale_b != nullptr ? cols * 4 : 0));
+            if (side_bias) ptx::bulk_load(slot, bsrc, cols * side_es, bar);
+            if (args.scale_b != nullptr) ptx::bulk_load(slot + C::SIDE_BIAS_BYTES, ssrc, cols * 4, bar);
+          }
+          __syncwarp();
+        }
+        if (it > 0) drain(&tmD, prev, prev_m_valid, args.colsum != nullptr, aux_tma, tc);
+        else if (aux_tma && lane == 0) {   // the output tile is free: tile 0's aux operand
+          ptx::mbar_expect_tx(aux_full, C::OUT_TILE_BYTES);
+          for (int b = 0; b < BN / 64; ++b)
+            ptx::tma_load_3d(out_base + b * C::OUT_BOX_BYTES, &tmAux, aux_full, tc.n_blk * BN + 64 * b, tc.m_blk * C::BM, tc.g);
+        }
+        __syncwarp();
+        prev = tc;
+        prev_m_valid = m_valid;
         ++it;
       }
+      if (it > 0) {
+        if (pre_act) drain(&tmD2, prev, prev_m_valid, false, false, prev);
+        drain(&tmD, prev, prev_m_valid, args.colsum != nullptr, false, prev);
+      }
+      if (lane == 0) ptx::bulk_wait_group<0>();   // the last tile's store has completed
     }
   } else {
     ptx::setmaxnreg_inc<C::CONSUMER_REGS>();
@@ -626,7 +731,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // 128 x 256 epilogue geometry (see wide_main): this thread's words of the output tile are at row0 + out_tile_off(j)
     // and 8 rows further down.
     const int ct = threadIdx.x - 128;       // consumer thread 0..255
-    const bool out_writer = ct == 0;        // issues the output tile's TMA stores and releases the tile (out_empty)
     const int r0 = cw * 16 + (lane >> 2);
     const int swz = lane >> 2;              // = r0 % 8
     uint8_t* row0 = out_tile + r0 * kSwizzleBytes + (lane & 3) * 4;
@@ -635,7 +739,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     : args.epilogue == EPI_RELU_BWD ? WM_RELU_BWD
                     : args.epilogue == EPI_ACT_BWD ? (args.act == ACT_GELU ? WM_GELU_BWD : args.act == ACT_SILU ? WM_SILU_BWD : WM_RELU_BWD)
                     : WM_BIAS;
-    uint32_t it = 0;   // tiles processed
+    uint32_t it = 0;     // tiles processed
+    uint32_t outs = 0;   // 128 x 256: output tiles handed to the store warp
 
     for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
       TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
@@ -667,13 +772,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           else ptx::wgmma_m64n128<DT, A_MN, B_MN>(acc, ad, bd, (kb | k) != 0);
         }
         ptx::wgmma_commit();
-        if constexpr (C::WIDE) {
-          if (out_writer && it > 0 && kb == kb_out_free) {
-            ptx::bulk_wait_group_read<0>();
-            ptx::mbar_arrive(out_empty);
-          }
-          __syncwarp();
-        }
         if (kb > 0) {
           ptx::wgmma_wait<1>();                                   // the group that read the previous stage has retired
           if (wg_leader) ptx::mbar_arrive(empty_bar(prev_s));
@@ -687,69 +785,55 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if constexpr (C::WIDE) {
         // ------------------------- 128 x 256 epilogue -------------------------
         const int m0 = tc.m_blk * C::BM, n0 = tc.n_blk * BN;
-        const int gb = tc.g / args.b_group_div;
         const bool ok0 = m0 + r0 < m_valid, ok1 = m0 + r0 + 8 < m_valid;
-        const int n_lane = n0 + 2 * (lane & 3);
+        const int n_lane = 2 * (lane & 3);   // column in the tile
+        const int n_lim = args.N - n0;
         // a row block that straddles the group's row count (at most one per group) must not write past the count,
         // which the output tensor map cannot express: it is copied out with row-guarded stores instead
         const bool straddle = m0 + C::BM > m_valid && m_valid < args.M;
+        // this tile's bias / column scales have landed in its side-input slot
+        const uint8_t* side = reinterpret_cast<const uint8_t*>(colsum_part + 8 * BN) + (it & 1u) * C::SIDE_SLOT_BYTES;
+        if (side_in) ptx::mbar_wait_quiet(side_full(it & 1u), (it >> 1) & 1u);
         if (args.scale_a != nullptr || args.scale_b != nullptr) {
           const float* sa = args.scale_a != nullptr ? args.scale_a + static_cast<long long>(tc.g) * args.scale_a_group_stride + m0 + r0 : nullptr;
           const float sa0 = (sa != nullptr && ok0) ? sa[0] : 1.0f;
           const float sa1 = (sa != nullptr && ok1) ? sa[8] : 1.0f;
-          const float* sb = args.scale_b != nullptr ? args.scale_b + static_cast<long long>(gb) * args.scale_b_group_stride : nullptr;
-          wide_scale(acc, sa0, sa1, sb, n_lane, args.N);
+          const float* sb = args.scale_b != nullptr ? reinterpret_cast<const float*>(side + C::SIDE_BIAS_BYTES) : nullptr;
+          wide_scale(acc, sa0, sa1, sb, n_lane, n_lim);
         }
-        const uint8_t* bias_g = nullptr;
-        if (args.bias != nullptr)
-          bias_g = reinterpret_cast<const uint8_t*>(args.bias) +
-                   static_cast<long long>(gb) * args.bias_group_stride * (args.bias_is_fp32 ? 4 : 2);
-        const uint32_t out_free_parity = (it & 1u) ^ 1u;   // out_empty phase it - 1: tile it - 1's store has read the tile
-
-        const OutTileStore st{out_tile, out_base, m0, n0, m_valid, args.N, tc.g, args.d_group_stride, args.ldd, straddle, ct,
-                              out_writer};
+        // the output tile is free again: the store warp has read tile it - 1 (two hand-overs per tile with pre_act)
+        auto wait_out_free = [&]() { ptx::mbar_wait_quiet(out_empty, (outs & 1u) ^ 1u); };
+        auto hand_over = [&](uint8_t* dst) {
+          hand_over_tile(out_tile, straddle, m0, n0, m_valid, args.N, tc.g, args.d_group_stride, args.ldd, dst, ct, lane, out_full);
+          ++outs;
+        };
 
         if (wmain == WM_BIAS) {
-          if (bias_g != nullptr)
-            wide_main<WM_BIAS>(acc, row0, swz, bias_g, args.bias_is_fp32 != 0, args.bias_is_bf16 != 0, n_lane, args.N, out_bf16, 1.0f);
-          if (args.d2 != nullptr && (args.epilogue == EPI_BIAS_GELU || args.epilogue == EPI_BIAS_SILU)) {
+          if (side_bias)
+            wide_main<WM_BIAS>(acc, row0, swz, side, args.bias_is_fp32 != 0, args.bias_is_bf16 != 0, n_lane, n_lim, out_bf16, 1.0f);
+          if (pre_act) {
             // training: the backward pass needs the pre-activation (ReLU gets by with the sign of its output)
-            ptx::mbar_wait_quiet(out_empty, out_free_parity);
+            wait_out_free();
             wide_stage(acc, row0, swz, out_bf16);
-            flush_out_tile(st, &tmD2, reinterpret_cast<uint8_t*>(args.d2), true);
+            hand_over(reinterpret_cast<uint8_t*>(args.d2));
           }
           if (args.epilogue == EPI_BIAS_RELU) wide_act<ACT_RELU>(acc);
           else if (args.epilogue == EPI_BIAS_GELU) wide_act<ACT_GELU>(acc);
           else if (args.epilogue == EPI_BIAS_SILU) wide_act<ACT_SILU>(acc);
         } else if (wmain == WM_NONE) {
-          if (args.alpha != 1.0f) wide_main<WM_NONE>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, args.alpha);
+          if (args.alpha != 1.0f) wide_main<WM_NONE>(acc, row0, swz, nullptr, false, false, n_lane, n_lim, out_bf16, args.alpha);
         } else {
           ptx::mbar_wait_quiet(aux_full, it & 1u);   // this tile's aux operand is in the output tile
-          if (wmain == WM_RELU_BWD) wide_main<WM_RELU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
-          else if (wmain == WM_ADD) wide_main<WM_ADD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
-          else if (wmain == WM_GELU_BWD) wide_main<WM_GELU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
-          else wide_main<WM_SILU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, args.N, out_bf16, 1.0f);
+          if (wmain == WM_RELU_BWD) wide_main<WM_RELU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, n_lim, out_bf16, 1.0f);
+          else if (wmain == WM_ADD) wide_main<WM_ADD>(acc, row0, swz, nullptr, false, false, n_lane, n_lim, out_bf16, 1.0f);
+          else if (wmain == WM_GELU_BWD) wide_main<WM_GELU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, n_lim, out_bf16, 1.0f);
+          else wide_main<WM_SILU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, n_lim, out_bf16, 1.0f);
         }
-        if (!aux_tma) ptx::mbar_wait_quiet(out_empty, out_free_parity);
+        if (!aux_tma) wait_out_free();
         wide_stage(acc, row0, swz, out_bf16);     // aux epilogues: each word overwrites the aux word it was computed from
-        float* colrow = colsum_rows + (it & 1u) * BN;
-        if (args.colsum != nullptr) wide_colsum(acc, ok0, ok1, lane, colrow);
-        flush_out_tile(st, &tmD, reinterpret_cast<uint8_t*>(args.d), false);
-        if (args.colsum != nullptr && ct < BN / 4) {
-          // one 4-column add per thread and tile: 64 global reductions instead of one per column and 16-row slice
-          float4* src = reinterpret_cast<float4*>(colrow) + ct;
-          const float4 v = *src;
-          *src = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-          const int n = n0 + 4 * ct;
-          if (n < args.N) {   // N is a multiple of 8: all four columns are in range
-            float* cs = args.colsum + static_cast<long long>(gb) * args.colsum_group_stride + n;
-            if ((reinterpret_cast<uintptr_t>(cs) & 15) == 0) {
-              ptx::red_add_v4_f32(cs, v.x, v.y, v.z, v.w);
-            } else {
-              atomicAdd(cs, v.x); atomicAdd(cs + 1, v.y); atomicAdd(cs + 2, v.z); atomicAdd(cs + 3, v.w);
-            }
-          }
-        }
+        // the partial rows are free: the store warp read them before it released the output tile
+        if (args.colsum != nullptr) wide_colsum(acc, ok0, ok1, lane, colsum_part + cw * BN);
+        hand_over(reinterpret_cast<uint8_t*>(args.d));
         ++it;
         continue;
       }
@@ -984,9 +1068,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-    if constexpr (C::WIDE) {
-      if (out_writer) ptx::bulk_wait_group<0>();   // the last tile's store has completed
-    }
   }
 }
 
@@ -1143,8 +1224,13 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
   // completion signals are built around the 128 x 128 configuration) or pins that configuration with block_n == 128.
   // The GLU epilogues (see gemm_sm90_kernel) and fp32 outputs (the 128 x 256 output tile is 16-bit) always take the
   // 128 x 128 configuration.
+  // The 128 x 256 store warp bulk-copies each tile's bias and column scales into shared memory, which needs 16-byte
+  // aligned rows; scale_b rows are only required to be 8-byte aligned, and such rows take the 128 x 128 configuration too.
+  const bool side_aligned =
+      ((reinterpret_cast<uintptr_t>(p.bias) | static_cast<uintptr_t>(p.bias_group_stride * 2)) & 15) == 0 &&
+      ((reinterpret_cast<uintptr_t>(p.scale_b) | static_cast<uintptr_t>(p.scale_b_group_stride * 4)) & 15) == 0;
   const bool wide = p.block_n != 128 && p.wait_flags == nullptr && p.signal_ptr_table == nullptr && p.d_ptr_table == nullptr &&
-                    p.epilogue != EPI_GLU && p.epilogue != EPI_GLU_BWD && p.out_dtype != DT_FP32;
+                    p.epilogue != EPI_GLU && p.epilogue != EPI_GLU_BWD && p.out_dtype != DT_FP32 && side_aligned;
   constexpr int bm = 128;
   const int bn = wide ? 256 : 128;
   GemmArgs a{};

@@ -221,6 +221,13 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const void* tmap,
       "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// Plain (non-tensor) bulk copy global -> this CTA's smem, completing on this CTA's mbarrier: `bytes` a multiple of 16,
+// both addresses 16-byte aligned.
+__device__ __forceinline__ void bulk_load(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_dst),
+               "l"(gsrc), "r"(bytes), "r"(bar)
+               : "memory");
+}
 // Ask the L2 to fetch `bytes` (multiple of 16) starting at a 16-byte aligned global address.
 __device__ __forceinline__ void prefetch_l2_bulk(const void* gptr, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gptr), "r"(bytes) : "memory");
