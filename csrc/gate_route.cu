@@ -414,6 +414,18 @@ int sm_count() {
 
 int gate_route_tiles(int S) { return (S + kTileTokens - 1) / kTileTokens; }
 
+// Dynamic shared memory above the default 48 KB needs an opt-in per kernel (both launches grow with k * E: at E = 512
+// and k = 32 the histograms take 68 KB and 133 KB).
+static cudaError_t allow_dynamic_smem(const void* fn, size_t bytes) {
+  if (bytes <= 48 * 1024) return cudaSuccess;
+  int dev = 0, optin = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (e != cudaSuccess) return e;
+  if (bytes > static_cast<size_t>(optin)) return cudaErrorInvalidValue;
+  return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+}
+
 template <typename T>
 static cudaError_t gate_route_forward_t(const void* logits, float* scores, int* idx, float* top, float* gates,
                                         float* me_partial, int* hist, int* loc, int* counts, int* slot_src,
@@ -423,11 +435,16 @@ static cudaError_t gate_route_forward_t(const void* logits, float* scores, int* 
   const long long slot_n = slot_src != nullptr ? static_cast<long long>(E) * C : 0;
   const size_t smem1 = sizeof(int) * static_cast<size_t>(k) * E + sizeof(float) * E;
   const size_t smem2 = sizeof(int) * (2 * static_cast<size_t>(k) * E + E);
-  if (smem1 > 48 * 1024 || smem2 > 48 * 1024) return cudaErrorInvalidValue;
+  cudaError_t err = allow_dynamic_smem(reinterpret_cast<const void*>(route_finish_kernel<T>), smem2);
+  if (err != cudaSuccess) return err;
 #define TB_GR(VPTv)                                                                                                   \
-  gate_route_kernel<T, VPTv><<<ntiles, kGateThreads, smem1, stream>>>(static_cast<const T*>(logits), scores, idx, top, \
-                                                                      gates, me_partial, hist, slot_src, slot_n, S, E, \
-                                                                      k, normalize ? 1 : 0, eps)
+  do {                                                                                                                \
+    if ((err = allow_dynamic_smem(reinterpret_cast<const void*>(gate_route_kernel<T, VPTv>), smem1)) != cudaSuccess)  \
+      return err;                                                                                                     \
+    gate_route_kernel<T, VPTv><<<ntiles, kGateThreads, smem1, stream>>>(static_cast<const T*>(logits), scores, idx,   \
+                                                                        top, gates, me_partial, hist, slot_src,       \
+                                                                        slot_n, S, E, k, normalize ? 1 : 0, eps);     \
+  } while (0)
   if (E <= 32) TB_GR(1);
   else if (E <= 64) TB_GR(2);
   else if (E <= 128) TB_GR(4);
