@@ -16,6 +16,11 @@ experts (experts that received at least one token), the weight bytes those exper
 time (`active_weight_GBps`: the weight bandwidth the dropless path needs, whatever the path actually read).  The expert
 module alone is timed the same way on the dispatch buffer of one call (`experts_median_ms`,
 `experts_active_weight_GBps`), and the output is compared with the padded path (`rel_err_vs_padded`).
+
+`--fp8` builds fp8 experts (`fp8=True`: e4m3 weight copies with one fp32 scale per row; in dropless decoding the skinny
+kernels `skinny_ffn_fp8_kernel` / `skinny_glu_ffn_fp8_kernel` stream those copies, x stays 16 bit).  With it,
+`active_weight_bytes` and both `*_GBps` count the bytes that path needs - the e4m3 copies, their fp32 scales and any
+biases - not the bytes of the 16-bit master parameters.  `rel_err_vs_padded` then compares with the padded fp8 path.
 """
 import argparse
 import json
@@ -34,9 +39,11 @@ ap.add_argument('--dim', type=int, default=2048)
 ap.add_argument('--hidden', type=int, default=0, help='hidden size per expert (default: --dim)')
 ap.add_argument('--dtype', default='float32')
 ap.add_argument('--iters', type=int, default=50)
+ap.add_argument('--fp8', action='store_true', help='fp8 experts (e4m3 weights with per-row scales); 16-bit --dtype only')
 ap.add_argument('--graph', action='store_true', help='ours only: replay the forward as one CUDA graph (tutel_b200.utils.graph)')
 args = ap.parse_args()
 hidden = args.hidden or args.dim
+assert not args.fp8 or (args.impl == 'ours' and args.dtype in ('bfloat16', 'float16')), '--fp8: ours, with a 16-bit --dtype'
 if args.impl == 'reference':
     sys.path.insert(0, os.path.join(ROOT, 'baseline', '_ref'))
     from tutel import moe, system
@@ -53,6 +60,8 @@ torch.manual_seed(0)
 experts = {'type': args.expert_type, 'num_experts_per_device': args.experts, 'hidden_size_per_expert': hidden}
 if args.expert_type == 'ffn':
     experts['activation_fn'] = lambda x: F.relu(x)
+if args.fp8:
+    experts['fp8'] = True
 with torch.device(dev):        # initialise the (multi-GB) weights on the GPU
     layer = moe.moe_layer(gate_type={'type': 'top', 'k': args.top_k, 'capacity_factor': 0.0}, model_dim=args.dim,
                           experts=experts, seeds=(1, 1, 1)).eval()
@@ -90,11 +99,27 @@ with torch.no_grad():
     hook.remove()
     _, expert_times = timed(lambda: layer.experts(bufs[-1], layer), args.iters)
     padded = layer(x)
-bytes_per_expert = sum(p.numel() * p.element_size() for p in layer.experts.parameters()) // args.experts
+
+
+def expert_bytes():
+    """Weight bytes one expert's forward reads: the parameters, or with --fp8 the e4m3 copies (1 byte per weight), one
+    fp32 scale per quantised row (ops/gemm.py: fp8_weight) and the 16-bit biases."""
+    e = layer.experts
+    if not args.fp8:
+        return sum(p.numel() * p.element_size() for p in e.parameters()) // args.experts
+    M, H, N = args.dim, hidden, args.dim
+    if args.expert_type == 'ffn':          # Q1 [H, M] + s1 [H], Q2^T [N, H] + s2 [N], biases
+        biases = sum(p.numel() * p.element_size() for p in (e.batched_fc1_bias, e.batched_fc2_bias) if p is not None)
+        return H * M + N * H + 4 * (H + N) + biases // args.experts
+    return 2 * H * M + N * H + 4 * (2 * H + N)   # Q1^T, Q2^T [H, M] + s1, s2 [H], Q3^T [N, H] + s3 [N]
+
+
+bytes_per_expert = expert_bytes()
 median, expert_median = times[len(times) // 2], expert_times[len(expert_times) // 2]
-print(json.dumps({'impl': args.impl, 'config': 'dropless cf=0 top-%d E=%d tokens=%d dim=%d hidden=%d %s %s megablocks_size=%d%s' % (
+config = 'dropless cf=0 top-%d E=%d tokens=%d dim=%d hidden=%d %s %s megablocks_size=%d%s%s' % (
     args.top_k, args.experts, args.tokens, args.dim, hidden, args.expert_type, args.dtype, args.megablocks_size,
-    ' cuda-graph' if args.graph and args.impl == 'ours' else ''), 'median_ms': median, 'min_ms': times[0], 'max_ms': times[-1],
+    ' fp8' if args.fp8 else '', ' cuda-graph' if args.graph and args.impl == 'ours' else '')
+print(json.dumps({'impl': args.impl, 'config': config, 'median_ms': median, 'min_ms': times[0], 'max_ms': times[-1],
     'experts_median_ms': expert_median, 'active_experts': active, 'active_weight_bytes': active * bytes_per_expert,
     'active_weight_GBps': active * bytes_per_expert / (median * 1e-3) / 1e9,
     'experts_active_weight_GBps': active * bytes_per_expert / (expert_median * 1e-3) / 1e9,

@@ -629,6 +629,78 @@ at::Tensor skinny_glu_ffn(const at::Tensor& x, const at::Tensor& w1, const at::T
   return y;
 }
 
+// Checks shared by the weight-only fp8 skinny kernels.
+void check_fp8_x(const at::Tensor& x, const char* fn) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 3 && x.is_contiguous(), fn, ": x must be a contiguous 3-d CUDA tensor");
+  TORCH_CHECK(x.scalar_type() == at::kHalf || x.scalar_type() == at::kBFloat16, fn, ": x must be float16 or bfloat16");
+}
+
+void check_fp8_weight(const at::Tensor& q, const at::Tensor& s, int64_t G, int64_t rows, int64_t cols, const char* fn,
+                      const char* name) {
+  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kFloat8_e4m3fn && q.is_contiguous(), fn, ": ", name,
+              " must be a contiguous float8_e4m3fn CUDA tensor");
+  TORCH_CHECK(q.dim() == 3 && q.size(0) == G && q.size(1) == rows && q.size(2) == cols, fn, ": ", name, " must be [", G, ", ",
+              rows, ", ", cols, "], got ", q.sizes());
+  TORCH_CHECK(s.is_cuda() && s.scalar_type() == at::kFloat && s.is_contiguous() && s.numel() == G * rows, fn, ": the scales of ",
+              name, " must be contiguous float32 with ", G * rows, " elements");
+}
+
+const int* opt_counts(const c10::optional<at::Tensor>& counts, int64_t G) {
+  if (!counts.has_value() || !counts->defined()) return nullptr;
+  TORCH_CHECK(counts->is_cuda() && counts->scalar_type() == at::kInt && counts->numel() >= G);
+  return counts->data_ptr<int>();
+}
+
+// x [G, R, K] (fp16 / bf16), q1 [G, H, K] + s1 [G, H], q2t [G, N, H] + s2 [G, N] (e4m3 + fp32), biases [G, H] / [G, N] in
+// x's dtype or None, counts int [G] or None -> fp32 [G, R, N]
+at::Tensor skinny_ffn_fp8(const at::Tensor& x, const at::Tensor& q1, const at::Tensor& s1, const c10::optional<at::Tensor>& b1,
+                          const at::Tensor& q2t, const at::Tensor& s2, const c10::optional<at::Tensor>& b2,
+                          const c10::optional<at::Tensor>& counts, int64_t act) {
+  check_fp8_x(x, "skinny_ffn_fp8");
+  const int64_t G = x.size(0), R = x.size(1), K = x.size(2), H = q1.dim() == 3 ? q1.size(1) : -1;
+  const int64_t N = q2t.dim() == 3 ? q2t.size(1) : -1;
+  check_fp8_weight(q1, s1, G, H, K, "skinny_ffn_fp8", "q1");
+  check_fp8_weight(q2t, s2, G, N, H, "skinny_ffn_fp8", "q2t");
+  TORCH_CHECK(act >= 1 && act <= 3, "skinny_ffn_fp8: act must be 1 (relu), 2 (gelu) or 3 (silu)");
+  const c10::cuda::CUDAGuard guard(x.device());
+  auto opt_ptr = [&](const c10::optional<at::Tensor>& t, int64_t n) -> const void* {
+    if (!t.has_value() || !t->defined()) return nullptr;
+    TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == x.scalar_type() && t->numel() == n,
+                "skinny_ffn_fp8: biases must be contiguous, in x's dtype, with G * H / G * N elements");
+    return t->data_ptr();
+  };
+  const void* pb1 = opt_ptr(b1, G * H);
+  const void* pb2 = opt_ptr(b2, G * N);
+  at::Tensor y = at::zeros({G, R, N}, x.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::skinny_grouped_ffn_fp8(x.data_ptr(), q1.data_ptr(), s1.data_ptr<float>(), pb1, q2t.data_ptr(),
+                                           s2.data_ptr<float>(), pb2, y.data_ptr<float>(), opt_counts(counts, G),
+                                           static_cast<int>(G), static_cast<int>(R), static_cast<int>(K), static_cast<int>(H),
+                                           static_cast<int>(N), static_cast<int>(act), elem_type_of(x), cur_stream()));
+  return y;
+}
+
+// x [G, R, M] (fp16 / bf16), q1t / q2t [G, H, M] + s1 / s2 [G, H], q3t [G, N, H] + s3 [G, N], counts int [G] or None
+// -> fp32 [G, R, N]
+at::Tensor skinny_glu_ffn_fp8(const at::Tensor& x, const at::Tensor& q1t, const at::Tensor& s1, const at::Tensor& q2t,
+                              const at::Tensor& s2, const at::Tensor& q3t, const at::Tensor& s3,
+                              const c10::optional<at::Tensor>& counts, int64_t act) {
+  check_fp8_x(x, "skinny_glu_ffn_fp8");
+  const int64_t G = x.size(0), R = x.size(1), M = x.size(2), H = q1t.dim() == 3 ? q1t.size(1) : -1;
+  const int64_t N = q3t.dim() == 3 ? q3t.size(1) : -1;
+  check_fp8_weight(q1t, s1, G, H, M, "skinny_glu_ffn_fp8", "q1t");
+  check_fp8_weight(q2t, s2, G, H, M, "skinny_glu_ffn_fp8", "q2t");
+  check_fp8_weight(q3t, s3, G, N, H, "skinny_glu_ffn_fp8", "q3t");
+  TORCH_CHECK(act >= 1 && act <= 3, "skinny_glu_ffn_fp8: act must be 1 (relu), 2 (gelu) or 3 (silu)");
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor y = at::zeros({G, R, N}, x.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::skinny_grouped_glu_ffn_fp8(x.data_ptr(), q1t.data_ptr(), s1.data_ptr<float>(), q2t.data_ptr(),
+                                               s2.data_ptr<float>(), q3t.data_ptr(), s3.data_ptr<float>(), y.data_ptr<float>(),
+                                               opt_counts(counts, G), static_cast<int>(G), static_cast<int>(R),
+                                               static_cast<int>(M), static_cast<int>(H), static_cast<int>(N),
+                                               static_cast<int>(act), elem_type_of(x), cur_stream()));
+  return y;
+}
+
 }  // namespace
 
 void register_symm_bindings(pybind11::module& m);  // symm_heap.cpp / p2p bindings
@@ -654,6 +726,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("skinny_gemm", &skinny_gemm);
   m.def("skinny_ffn", &skinny_ffn);
   m.def("skinny_glu_ffn", &skinny_glu_ffn);
+  m.def("skinny_ffn_fp8", &skinny_ffn_fp8);
+  m.def("skinny_glu_ffn_fp8", &skinny_glu_ffn_fp8);
   m.def("quantize_rows", &quantize_rows);
   m.def("dequant_rows", &dequant_rows);
   m.def("quantize_transpose", &quantize_transpose);

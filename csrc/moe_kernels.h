@@ -118,4 +118,20 @@ cudaError_t skinny_grouped_ffn(const void* x, const void* w1, const void* b1, co
 cudaError_t skinny_grouped_glu_ffn(const void* x, const void* w1, const void* w2, const void* w3, float* y, const int* counts,
                                    int G, int rows_cap, int M, int H, int N, int act, int elem_type, cudaStream_t stream);
 
+// Weight-only fp8 (W8A16) versions of the two kernels above, on the e4m3 copies the fp8 wgmma forward caches
+// (ops/gemm.py: fp8_weight); x is fp16 / bf16 and is not quantised, accumulation is fp32, scales multiply finished dot
+// products.  Same launch contract: y fp32 [G, rows_cap, N] ZERO-INITIALISED, rows r < min(counts[g], rows_cap) only.
+//   skinny_grouped_ffn_fp8:     y[g, r] += act(s1[g] * (x[g, r] @ Q1[g]^T) + b1[g]) @ (s2[g] * Q2t[g])^T + b2[g]
+//       Q1 [G, H, K] e4m3, s1 fp32 [G, H];  Q2t [G, N, H] e4m3, s2 fp32 [G, N];  biases [G, H] / [G, N] in x's dtype or null.
+//   skinny_grouped_glu_ffn_fp8: y[g, r] += (act(s1[g] * (x @ Q1t[g]^T)) * (s2[g] * (x @ Q2t[g]^T))) @ (s3[g] * Q3t[g])^T
+//       Q1t / Q2t [G, H, M] e4m3, s1 / s2 fp32 [G, H];  Q3t [G, N, H] e4m3, s3 fp32 [G, N].
+// cudaErrorInvalidValue for a 32-bit x, unaligned x / e4m3 pointers, K (M), H or N not a multiple of 16, or staged rows of
+// x beyond the 200 KB of shared memory of the 16-bit kernels.  act: 1 relu, 2 gelu, 3 silu.
+cudaError_t skinny_grouped_ffn_fp8(const void* x, const void* q1, const float* s1, const void* b1, const void* q2t,
+                                   const float* s2, const void* b2, float* y, const int* counts, int G, int rows_cap, int K,
+                                   int H, int N, int act, int elem_type, cudaStream_t stream);
+cudaError_t skinny_grouped_glu_ffn_fp8(const void* x, const void* q1t, const float* s1, const void* q2t, const float* s2,
+                                       const void* q3t, const float* s3, float* y, const int* counts, int G, int rows_cap,
+                                       int M, int H, int N, int act, int elem_type, cudaStream_t stream);
+
 }  // namespace tb

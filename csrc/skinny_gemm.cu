@@ -10,6 +10,7 @@
 // W is [G, N, K] ("nk", one warp per output column, lanes stride K) or [G, K, N] ("kn", lanes stride N).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 
 #include "moe_kernels.h"
 
@@ -476,6 +477,311 @@ cudaError_t launch_glu_ffn(const void* x, const void* w1, const void* w2, const 
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------
+// Weight-only fp8: the two expert kernels above with e4m3 weights and one fp32 scale per weight row (W8A16)
+// ------------------------------------------------------------------------------------------------
+// The operands are the cached copies the e4m3 wgmma forward reads (ops/gemm.py: fp8_weight), so prefill and decode share
+// one e4m3 copy per weight.  Both kernels have the same two layers:
+//   layer 1: rows of an [H, K] matrix (K contiguous), one hidden unit per warp, lanes stride K with 16-byte loads;
+//            h = act(s1[j] * dot + b1[j])  (FFN)  or  act(s1[j] * dot1) * (s2[j] * dot2)  (SwiGLU, both rows in one loop);
+//   layer 2: rows of an [N, H] matrix (H contiguous): the block's kHS8-unit slice of output n's row is one 128-byte line,
+//            spread over 8 lanes and reduced with three shuffles; y[r, n] += s[n] * partial (+ bias[n]) with fp32 atomics.
+// x stays 16 bit on the way in (staged as fp32), accumulation is fp32 and each scale multiplies a finished dot product.
+constexpr int kHS8 = 128;       // hidden units per block: 128 e4m3 bytes per layer-2 row, the bytes of the 16-bit kHS slice
+
+// 16 e4m3 values (one 16-byte load) -> fp32 with the hardware unpack (F2FP.F16.E4M3.UNPACK, then f16 -> f32); e4m3 is
+// exact in f16.  Byte i of the load is element i.
+__device__ __forceinline__ void e4m3x16(const uint4 u, float* f) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+#pragma unroll
+    for (int p = 0; p < 2; ++p) {
+      const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w[i] >> (16 * p)), __NV_E4M3);
+      const float2 t = __half22float2(__half2(h));
+      f[4 * i + 2 * p] = t.x;
+      f[4 * i + 2 * p + 1] = t.y;
+    }
+  }
+}
+
+// Index of element k of a staged row of length K (K % 16 == 0) in the "chunk-split" layout: the four float4s of 16-element
+// chunk c lie K/16 float4s apart, so a lane that owns the 16 weights of chunk c reads its four float4s of x at
+// consecutive addresses across consecutive lanes (no bank conflicts), instead of 64 contiguous bytes per lane.
+__device__ __forceinline__ int split_index(int k, int K) { return ((((k & 15) >> 2) * (K >> 4) + (k >> 4)) << 2) + (k & 3); }
+
+template <typename T>
+__device__ __forceinline__ void stage_rows_split(float* __restrict__ xs, const T* __restrict__ xrow0, int nr, int K) {
+  __syncthreads();
+  for (int i = threadIdx.x * 8; i < nr * K; i += 256 * 8) {
+    float f[8];
+    WVec<T>::load(xrow0 + i, f);          // 8 elements of one row (K % 16 == 0): two float4s of one chunk
+    const int r = i / K, k = i - r * K;
+    float* row = xs + r * K;
+    *reinterpret_cast<float4*>(row + split_index(k, K)) = make_float4(f[0], f[1], f[2], f[3]);
+    *reinterpret_cast<float4*>(row + split_index(k + 4, K)) = make_float4(f[4], f[5], f[6], f[7]);
+  }
+  if (nr > 2)
+    for (int i = threadIdx.x + nr * K; i < kFfnRows * K; i += 256) xs[i] = 0.0f;
+  __syncthreads();
+}
+
+// Warp-wide dot products of ROWS staged rows of x with row q[0] (and q[1] when NMAT == 2) of K e4m3 weights; every lane
+// gets the full sums.  Four 16-byte loads per matrix in flight per lane; each weight is converted once for all rows.
+template <int ROWS, int NMAT>
+__device__ __forceinline__ void fp8_row_dots(const float* __restrict__ xs, const uint8_t* const (&q)[NMAT], int K,
+                                             float (&acc)[NMAT][ROWS]) {
+  const int lane = threadIdx.x & 31;
+  const int K16 = K >> 4;
+#pragma unroll
+  for (int m = 0; m < NMAT; ++m)
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) acc[m][r] = 0.0f;
+  for (int c = lane; c < K16; c += 32 * 4) {
+    uint4 raw[4][NMAT];
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+#pragma unroll
+      for (int m = 0; m < NMAT; ++m)
+        raw[u][m] = c + 32 * u < K16 ? __ldcs(reinterpret_cast<const uint4*>(q[m]) + c + 32 * u) : make_uint4(0, 0, 0, 0);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int cc = c + 32 * u;
+      if (cc < K16) {
+        float wv[NMAT][16];
+#pragma unroll
+        for (int m = 0; m < NMAT; ++m) e4m3x16(raw[u][m], wv[m]);
+#pragma unroll
+        for (int r = 0; r < ROWS; ++r) {
+          const float4* xr = reinterpret_cast<const float4*>(xs + r * K) + cc;
+#pragma unroll
+          for (int p = 0; p < 4; ++p) {
+            const float4 xv = xr[p * K16];
+#pragma unroll
+            for (int m = 0; m < NMAT; ++m) {
+              acc[m][r] = fmaf(xv.x, wv[m][4 * p], acc[m][r]);
+              acc[m][r] = fmaf(xv.y, wv[m][4 * p + 1], acc[m][r]);
+              acc[m][r] = fmaf(xv.z, wv[m][4 * p + 2], acc[m][r]);
+              acc[m][r] = fmaf(xv.w, wv[m][4 * p + 3], acc[m][r]);
+            }
+          }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int m = 0; m < NMAT; ++m)
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc[m][r] += __shfl_xor_sync(0xffffffffu, acc[m][r], o);
+}
+
+// Layer 2 of a pass (shared by both kernels): yrow0[r, n] += s[n] * sum_{j < hs} h[r, j] * q[n, j] (+ bias[n]) for r < nr.
+// q points at the slice's first column of the [N, H] matrix; hsm holds h [ROWS][kHS8] in the chunk-split layout.  Lane
+// (sub, c) of a warp takes hidden units [16c, 16c + 16) of output sub (4 outputs per warp and load, each a whole line); its
+// 16 h values per row stay in registers for the whole pass.  After the 8-lane reduction lane c adds row c.
+template <typename T, int ROWS>
+__device__ __forceinline__ void fp8_layer2(const float* __restrict__ hsm, const uint8_t* __restrict__ q,
+                                           const float* __restrict__ s, const T* __restrict__ bias,
+                                           float* __restrict__ yrow0, int nr, int hs, int H, int N) {
+  constexpr int U = ROWS <= 2 ? 8 : 4;          // loads in flight per lane
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int c = lane & 7, sub = lane >> 3;
+  const bool live = c * 16 < hs;                // hs % 16 == 0: a chunk is wholly inside the slice or wholly outside
+  float hv[ROWS][16];
+#pragma unroll
+  for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      const float4 t = live ? reinterpret_cast<const float4*>(hsm + r * kHS8)[p * (kHS8 / 16) + c] : make_float4(0.f, 0.f, 0.f, 0.f);
+      hv[r][4 * p] = t.x; hv[r][4 * p + 1] = t.y; hv[r][4 * p + 2] = t.z; hv[r][4 * p + 3] = t.w;
+    }
+  for (int nb = warp * 4; nb < N; nb += 32 * U) {   // warp-uniform bound: all lanes reach the shuffles
+    uint4 raw[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int n = nb + sub + 32 * u;
+      raw[u] = live && n < N ? __ldcs(reinterpret_cast<const uint4*>(q + static_cast<long long>(n) * H) + c) : make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      float wv[16];
+      e4m3x16(raw[u], wv);
+      float acc[ROWS];
+#pragma unroll
+      for (int r = 0; r < ROWS; ++r) {
+        acc[r] = 0.0f;
+#pragma unroll
+        for (int e = 0; e < 16; ++e) acc[r] = fmaf(hv[r][e], wv[e], acc[r]);
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) acc[r] += __shfl_xor_sync(0xffffffffu, acc[r], o);
+      }
+      const int n = nb + sub + 32 * u;
+      if (c < nr && n < N) {
+        float v = acc[0];
+#pragma unroll
+        for (int r = 1; r < ROWS; ++r) if (c == r) v = acc[r];
+        v *= s[n];
+        if (bias != nullptr) v += ldf<T>(bias + n);
+        atomicAdd(yrow0 + static_cast<long long>(c) * N + n, v);
+      }
+    }
+  }
+}
+
+template <typename T, int ROWS>
+__device__ __forceinline__ void ffn_fp8_pass(const float* __restrict__ xs, float* __restrict__ hsm, const uint8_t* __restrict__ q1g,
+                                             const float* __restrict__ s1g, const T* __restrict__ b1g,
+                                             const uint8_t* __restrict__ q2g, const float* __restrict__ s2g,
+                                             const T* __restrict__ b2g, float* __restrict__ yrow0, int nr, int K, int hs,
+                                             int H, int N, int act) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int j = warp; j < hs; j += 8) {
+    const uint8_t* const rows[1] = {q1g + static_cast<long long>(j) * K};
+    float acc[1][ROWS];
+    fp8_row_dots<ROWS, 1>(xs, rows, K, acc);
+    if (lane < ROWS) {
+      float v = acc[0][0];
+#pragma unroll
+      for (int r = 1; r < ROWS; ++r) if (lane == r) v = acc[0][r];
+      const float b = b1g != nullptr ? ldf<T>(b1g + j) : 0.0f;
+      hsm[lane * kHS8 + split_index(j, kHS8)] = ffn_act(fmaf(s1g[j], v, b), act);
+    }
+  }
+  __syncthreads();
+  fp8_layer2<T, ROWS>(hsm, q2g, s2g, b2g, yrow0, nr, hs, H, N);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256, 2)
+skinny_ffn_fp8_kernel(const T* __restrict__ x, const uint8_t* __restrict__ q1, const float* __restrict__ s1,
+                      const T* __restrict__ b1, const uint8_t* __restrict__ q2t, const float* __restrict__ s2,
+                      const T* __restrict__ b2, float* __restrict__ y, const int* __restrict__ counts, int rows_cap, int K,
+                      int H, int N, int act) {
+  extern __shared__ __align__(16) float sm8[];  // x rows [kFfnRows][K] | hidden slice [kFfnRows][kHS8], both chunk-split
+  const int g = blockIdx.y;
+  const int count = counts != nullptr ? min(counts[g], rows_cap) : rows_cap;
+  if (count <= 0) return;
+  const int h0 = blockIdx.x * kHS8;
+  const int hs = min(kHS8, H - h0);
+  float* xs = sm8;
+  float* hsm = sm8 + kFfnRows * K;
+  const T* xg = x + static_cast<long long>(g) * rows_cap * K;
+  const uint8_t* q1g = q1 + (static_cast<long long>(g) * H + h0) * K;
+  const float* s1g = s1 + static_cast<long long>(g) * H + h0;
+  const T* b1g = b1 != nullptr ? b1 + static_cast<long long>(g) * H + h0 : nullptr;
+  const uint8_t* q2g = q2t + static_cast<long long>(g) * N * H + h0;
+  const float* s2g = s2 + static_cast<long long>(g) * N;
+  const T* b2g = b2 != nullptr && blockIdx.x == 0 ? b2 + static_cast<long long>(g) * N : nullptr;
+  float* yg = y + static_cast<long long>(g) * rows_cap * N;
+
+  for (int r0 = 0; r0 < count; r0 += kFfnRows) {
+    const int nr = min(kFfnRows, count - r0);
+    stage_rows_split<T>(xs, xg + static_cast<long long>(r0) * K, nr, K);
+    float* yrow0 = yg + static_cast<long long>(r0) * N;
+    if (nr == 1) ffn_fp8_pass<T, 1>(xs, hsm, q1g, s1g, b1g, q2g, s2g, b2g, yrow0, nr, K, hs, H, N, act);
+    else if (nr == 2) ffn_fp8_pass<T, 2>(xs, hsm, q1g, s1g, b1g, q2g, s2g, b2g, yrow0, nr, K, hs, H, N, act);
+    else ffn_fp8_pass<T, kFfnRows>(xs, hsm, q1g, s1g, b1g, q2g, s2g, b2g, yrow0, nr, K, hs, H, N, act);
+  }
+}
+
+template <typename T, int ROWS>
+__device__ __forceinline__ void glu_fp8_pass(const float* __restrict__ xs, float* __restrict__ hsm, const uint8_t* __restrict__ q1g,
+                                             const float* __restrict__ s1g, const uint8_t* __restrict__ q2g,
+                                             const float* __restrict__ s2g, const uint8_t* __restrict__ q3g,
+                                             const float* __restrict__ s3g, float* __restrict__ yrow0, int nr, int M, int hs,
+                                             int H, int N, int act) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int j = warp; j < hs; j += 8) {
+    const uint8_t* const rows[2] = {q1g + static_cast<long long>(j) * M, q2g + static_cast<long long>(j) * M};
+    float acc[2][ROWS];
+    fp8_row_dots<ROWS, 2>(xs, rows, M, acc);
+    if (lane < ROWS) {
+      float gv = acc[0][0], uv = acc[1][0];
+#pragma unroll
+      for (int r = 1; r < ROWS; ++r)
+        if (lane == r) { gv = acc[0][r]; uv = acc[1][r]; }
+      hsm[lane * kHS8 + split_index(j, kHS8)] = ffn_act(s1g[j] * gv, act) * (s2g[j] * uv);
+    }
+  }
+  __syncthreads();
+  fp8_layer2<T, ROWS>(hsm, q3g, s3g, nullptr, yrow0, nr, hs, H, N);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256, 2)
+skinny_glu_ffn_fp8_kernel(const T* __restrict__ x, const uint8_t* __restrict__ q1t, const float* __restrict__ s1,
+                          const uint8_t* __restrict__ q2t, const float* __restrict__ s2, const uint8_t* __restrict__ q3t,
+                          const float* __restrict__ s3, float* __restrict__ y, const int* __restrict__ counts, int rows_cap,
+                          int M, int H, int N, int act) {
+  extern __shared__ __align__(16) float sm8[];  // x rows [kFfnRows][M] | hidden slice [kFfnRows][kHS8], both chunk-split
+  const int g = blockIdx.y;
+  const int count = counts != nullptr ? min(counts[g], rows_cap) : rows_cap;
+  if (count <= 0) return;
+  const int h0 = blockIdx.x * kHS8;
+  const int hs = min(kHS8, H - h0);
+  float* xs = sm8;
+  float* hsm = sm8 + kFfnRows * M;
+  const T* xg = x + static_cast<long long>(g) * rows_cap * M;
+  const uint8_t* q1g = q1t + (static_cast<long long>(g) * H + h0) * M;
+  const uint8_t* q2g = q2t + (static_cast<long long>(g) * H + h0) * M;
+  const float* s1g = s1 + static_cast<long long>(g) * H + h0;
+  const float* s2g = s2 + static_cast<long long>(g) * H + h0;
+  const uint8_t* q3g = q3t + static_cast<long long>(g) * N * H + h0;
+  const float* s3g = s3 + static_cast<long long>(g) * N;
+  float* yg = y + static_cast<long long>(g) * rows_cap * N;
+
+  for (int r0 = 0; r0 < count; r0 += kFfnRows) {
+    const int nr = min(kFfnRows, count - r0);
+    stage_rows_split<T>(xs, xg + static_cast<long long>(r0) * M, nr, M);
+    float* yrow0 = yg + static_cast<long long>(r0) * N;
+    if (nr == 1) glu_fp8_pass<T, 1>(xs, hsm, q1g, s1g, q2g, s2g, q3g, s3g, yrow0, nr, M, hs, H, N, act);
+    else if (nr == 2) glu_fp8_pass<T, 2>(xs, hsm, q1g, s1g, q2g, s2g, q3g, s3g, yrow0, nr, M, hs, H, N, act);
+    else glu_fp8_pass<T, kFfnRows>(xs, hsm, q1g, s1g, q2g, s2g, q3g, s3g, yrow0, nr, M, hs, H, N, act);
+  }
+}
+
+// Dynamic shared memory of both fp8 kernels: the staged x rows and the hidden slice (K % 16 == 0 keeps both 16-byte aligned).
+size_t fp8_smem_bytes(int K) { return sizeof(float) * (static_cast<size_t>(kFfnRows) * K + kFfnRows * kHS8); }
+
+template <typename Kern>
+cudaError_t fp8_opt_in(Kern* kern, size_t smem) {
+  if (smem > kFfnSmemLimit) return cudaErrorInvalidValue;
+  if (smem > 48 * 1024) return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t launch_ffn_fp8(const void* x, const void* q1, const float* s1, const void* b1, const void* q2t, const float* s2,
+                           const void* b2, float* y, const int* counts, int G, int rows_cap, int K, int H, int N, int act,
+                           cudaStream_t stream) {
+  const size_t smem = fp8_smem_bytes(K);
+  auto* kern = skinny_ffn_fp8_kernel<T>;
+  cudaError_t e = fp8_opt_in(kern, smem);
+  if (e != cudaSuccess) return e;
+  dim3 grid((H + kHS8 - 1) / kHS8, G);
+  kern<<<grid, 256, smem, stream>>>(static_cast<const T*>(x), static_cast<const uint8_t*>(q1), s1, static_cast<const T*>(b1),
+                                    static_cast<const uint8_t*>(q2t), s2, static_cast<const T*>(b2), y, counts, rows_cap, K,
+                                    H, N, act);
+  return cudaGetLastError();
+}
+
+template <typename T>
+cudaError_t launch_glu_ffn_fp8(const void* x, const void* q1t, const float* s1, const void* q2t, const float* s2,
+                               const void* q3t, const float* s3, float* y, const int* counts, int G, int rows_cap, int M,
+                               int H, int N, int act, cudaStream_t stream) {
+  const size_t smem = fp8_smem_bytes(M);
+  auto* kern = skinny_glu_ffn_fp8_kernel<T>;
+  cudaError_t e = fp8_opt_in(kern, smem);
+  if (e != cudaSuccess) return e;
+  dim3 grid((H + kHS8 - 1) / kHS8, G);
+  kern<<<grid, 256, smem, stream>>>(static_cast<const T*>(x), static_cast<const uint8_t*>(q1t), s1,
+                                    static_cast<const uint8_t*>(q2t), s2, static_cast<const uint8_t*>(q3t), s3, y, counts,
+                                    rows_cap, M, H, N, act);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 cudaError_t skinny_grouped_gemm(const void* x, const void* w, const void* bias, void* y, const int* counts, int G,
@@ -510,6 +816,34 @@ cudaError_t skinny_grouped_glu_ffn(const void* x, const void* w1, const void* w2
     case ET_F32: return launch_glu_ffn<float>(x, w1, w2, w3, y, counts, G, rows_cap, M, H, N, act, stream);
     case ET_F16: return launch_glu_ffn<__half>(x, w1, w2, w3, y, counts, G, rows_cap, M, H, N, act, stream);
     case ET_BF16: return launch_glu_ffn<__nv_bfloat16>(x, w1, w2, w3, y, counts, G, rows_cap, M, H, N, act, stream);
+  }
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t skinny_grouped_ffn_fp8(const void* x, const void* q1, const float* s1, const void* b1, const void* q2t,
+                                   const float* s2, const void* b2, float* y, const int* counts, int G, int rows_cap, int K,
+                                   int H, int N, int act, int elem_type, cudaStream_t stream) {
+  if (G <= 0 || rows_cap <= 0 || K <= 0 || H <= 0 || N <= 0) return cudaSuccess;
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(q1) | reinterpret_cast<uintptr_t>(q2t)) & 15) return cudaErrorInvalidValue;
+  if (K % 16 || H % 16 || N % 16) return cudaErrorInvalidValue;
+  switch (elem_type) {
+    case ET_F16: return launch_ffn_fp8<__half>(x, q1, s1, b1, q2t, s2, b2, y, counts, G, rows_cap, K, H, N, act, stream);
+    case ET_BF16: return launch_ffn_fp8<__nv_bfloat16>(x, q1, s1, b1, q2t, s2, b2, y, counts, G, rows_cap, K, H, N, act, stream);
+  }
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t skinny_grouped_glu_ffn_fp8(const void* x, const void* q1t, const float* s1, const void* q2t, const float* s2,
+                                       const void* q3t, const float* s3, float* y, const int* counts, int G, int rows_cap,
+                                       int M, int H, int N, int act, int elem_type, cudaStream_t stream) {
+  if (G <= 0 || rows_cap <= 0 || M <= 0 || H <= 0 || N <= 0) return cudaSuccess;
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(q1t) | reinterpret_cast<uintptr_t>(q2t) |
+       reinterpret_cast<uintptr_t>(q3t)) & 15) return cudaErrorInvalidValue;
+  if (M % 16 || H % 16 || N % 16) return cudaErrorInvalidValue;
+  switch (elem_type) {
+    case ET_F16: return launch_glu_ffn_fp8<__half>(x, q1t, s1, q2t, s2, q3t, s3, y, counts, G, rows_cap, M, H, N, act, stream);
+    case ET_BF16:
+      return launch_glu_ffn_fp8<__nv_bfloat16>(x, q1t, s1, q2t, s2, q3t, s3, y, counts, G, rows_cap, M, H, N, act, stream);
   }
   return cudaErrorInvalidValue;
 }

@@ -20,7 +20,12 @@ class LlamaFFNNetwork(torch.nn.Module):
                  activation_fn=torch.nn.functional.silu, fp8=None):
         super().__init__()
         import os
-        self.fp8 = bool(int(os.environ.get('TUTEL_B200_FP8', '0'))) if fp8 is None else bool(fp8)
+        # fp8=True / 'row' (or TUTEL_B200_FP8=1 / true / row): e4m3 weights with per-row scales on every path, as in `ffn`.
+        # OCP MX ('mx') has no SwiGLU kernel.
+        mode = str(os.environ.get('TUTEL_B200_FP8', '0') if fp8 is None else fp8).lower()
+        assert mode in ('0', '1', 'true', 'false', 'none', 'row'), \
+            'llama_ffn: fp8 must be a bool or "row" (got %r); "mx" has no SwiGLU path' % (mode,)
+        self.fp8 = mode in ('1', 'true', 'row')
         self.sharded_count = sharded_count
         self.full_shapes = {
             'W_fc1': torch.Size([num_experts_per_device, model_dim, hidden_size_per_expert]),
@@ -60,6 +65,9 @@ class LlamaFFNNetwork(torch.nn.Module):
         if row_counts is not None and G.can_use_skinny_glu_ffn(x, w1, w2, w3, kind) and (
                 not G.can_use_wgmma(x, w1) or x.size(1) * getattr(ctx, 'top_k', 1) <= G.SKINNY_PASS_ROWS * x.size(0)):
             # dropless decoder inference: a few tokens per expert -> ONE launch streams the active experts' weights once
+            # (with fp8: the cached e4m3 copies the wgmma fp8 forward uses, half the bytes)
+            if self.fp8 and G.can_use_skinny_glu_ffn_fp8(x, w1, w2, w3, kind):
+                return G.skinny_glu_ffn_fp8(x, w1, w2, w3, row_counts, kind)
             return G.skinny_glu_ffn(x, w1, w2, w3, row_counts, kind)
         if kind in G.ACT_CODES and G.can_use_wgmma(x, w1) and w3.size(-1) % 8 == 0:
             # gate/up GEMMs + activation + multiply in one dual-B wgmma launch; backward without elementwise passes

@@ -431,6 +431,43 @@ def fused_relu_ffn_fp8(x, w1, b1, w2, b2, row_counts=None):
     return FusedReluFFNFp8.apply(x, w1, b1, w2, b2, row_counts)
 
 
+# Weight-only fp8 skinny kernels (csrc/skinny_gemm.cu): they read the same cached e4m3 copies as the wgmma fp8 forward,
+# x stays 16 bit.  Staged x rows + the 128-unit hidden slice in fp32, within the 16-bit kernels' 100 KB (2 blocks / SM).
+def _fp8_skinny_dims(x, *dims) -> bool:
+    return x.dtype in (torch.float16, torch.bfloat16) and all(d % 16 == 0 for d in dims) and 16 * x.size(2) + 2048 <= 100 * 1024
+
+
+def can_use_skinny_ffn_fp8(x: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, act_kind) -> bool:
+    """``skinny_ffn`` with the e4m3 copies of W1 ('nk') and W2 ('kn') (csrc/skinny_gemm.cu: skinny_ffn_fp8_kernel)."""
+    return can_use_skinny_ffn(x, w1, w2, act_kind) and _fp8_skinny_dims(x, x.size(2), w1.size(1), w2.size(2))
+
+
+def skinny_ffn_fp8(x, w1, b1, w2, b2, row_counts, act_kind):
+    """y[g, r] = act(x[g, r] @ Q1[g]^T + b1[g]) @ Q2[g] + b2[g] for r < row_counts[g] (other rows zero), where Q1 / Q2 are
+    the cached per-row-scaled e4m3 copies of the 16-bit master weights ``w1 [G, H, M]`` / ``w2 [G, H, N]``."""
+    q1, s1 = fp8_weight(w1, 'nk')            # [G, H, M], [G, H]
+    q2t, s2 = fp8_weight(w2, 'kn')           # [G, N, H], [G, N]
+    backend.count_launch(2)                  # zero-fill of the fp32 accumulator + the kernel
+    b1 = None if b1 is None else b1.reshape(w1.size(0), -1).to(x.dtype).contiguous()
+    b2 = None if b2 is None else b2.reshape(w2.size(0), -1).to(x.dtype).contiguous()
+    y = backend.require_ext().skinny_ffn_fp8(x.contiguous(), q1, s1, b1, q2t, s2, b2, row_counts, _SKINNY_ACTS[act_kind])
+    return y.to(x.dtype)
+
+
+def can_use_skinny_glu_ffn_fp8(x: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch.Tensor, act_kind) -> bool:
+    """``skinny_glu_ffn`` with the e4m3 copies of W1, W2, W3 (all 'kn') (csrc/skinny_gemm.cu: skinny_glu_ffn_fp8_kernel)."""
+    return can_use_skinny_glu_ffn(x, w1, w2, w3, act_kind) and _fp8_skinny_dims(x, x.size(2), w1.size(2), w3.size(2))
+
+
+def skinny_glu_ffn_fp8(x, w1, w2, w3, row_counts, act_kind):
+    """y[g, r] = (act(x[g, r] @ Q1[g]) * (x[g, r] @ Q2[g])) @ Q3[g] for r < row_counts[g] (other rows zero), where Q1..Q3
+    are the cached per-row-scaled e4m3 copies of ``w1, w2 [G, M, H]`` and ``w3 [G, H, N]`` that ``fused_glu_ffn`` uses."""
+    (q1, s1), (q2, s2), (q3, s3) = fp8_weight(w1, 'kn'), fp8_weight(w2, 'kn'), fp8_weight(w3, 'kn')
+    backend.count_launch(2)                  # zero-fill of the fp32 accumulator + the kernel
+    y = backend.require_ext().skinny_glu_ffn_fp8(x.contiguous(), q1, s1, q2, s2, q3, s3, row_counts, _SKINNY_ACTS[act_kind])
+    return y.to(x.dtype)
+
+
 def _glu_extra(kw):
     return (int(kw.get('b_group_div', 1)), int(kw.get('cta_group', 0)), int(kw.get('wait_flags', 0)),
             int(kw.get('wait_rows_per_flag', 0)), int(kw.get('wait_flags_per_group', 0)), int(kw.get('wait_target', 0)),
