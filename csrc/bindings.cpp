@@ -344,6 +344,90 @@ at::Tensor gate_route_backward(const at::Tensor& scores, const at::Tensor& idx, 
   return out;
 }
 
+// Sigmoid scoring with a selection bias and group-limited choice: same outputs as gate_route_forward (top = unbiased
+// scores, ce = fp32 all-choice counts); `expert_load` fp32 [E] (optional) accumulates the all-choice counts.
+std::vector<at::Tensor> sigmoid_gate_route_forward(const at::Tensor& logits, const at::Tensor& bias, int64_t k, int64_t C,
+                                                   bool normalize, double eps, int64_t n_group, int64_t topk_group,
+                                                   double scale, const c10::optional<at::Tensor>& expert_load) {
+  TORCH_CHECK(logits.is_cuda() && logits.dim() == 2 && logits.is_contiguous(), "sigmoid_gate_route_forward: contiguous CUDA [S, E] logits expected");
+  const c10::cuda::CUDAGuard guard(logits.device());
+  const int S = static_cast<int>(logits.size(0)), E = static_cast<int>(logits.size(1));
+  TORCH_CHECK(E <= 512 && k >= 1 && k <= 32 && k <= E, "sigmoid_gate_route_forward: needs E <= 512 and 1 <= k <= min(32, E)");
+  TORCH_CHECK(n_group >= 1 && n_group <= 32 && E % n_group == 0 && topk_group >= 1 && topk_group <= n_group &&
+              k <= topk_group * (E / n_group),
+              "sigmoid_gate_route_forward: needs n_group <= 32 dividing E, 1 <= topk_group <= n_group and k <= topk_group * E / n_group");
+  TORCH_CHECK(bias.is_cuda() && bias.device() == logits.device() && bias.scalar_type() == at::kFloat && bias.is_contiguous() && bias.numel() == E,
+              "sigmoid_gate_route_forward: fp32 [E] bias on the logits' device expected");
+  float* load_p = nullptr;
+  if (expert_load.has_value() && expert_load->defined()) {
+    TORCH_CHECK(expert_load->is_cuda() && expert_load->device() == logits.device() && expert_load->scalar_type() == at::kFloat &&
+                expert_load->is_contiguous() && expert_load->numel() == E,
+                "sigmoid_gate_route_forward: fp32 [E] expert_load on the logits' device expected");
+    load_p = expert_load->data_ptr<float>();
+  }
+  const int tiles = tb::gate_route_tiles(S);
+  auto f32 = logits.options().dtype(at::kFloat);
+  auto i32 = logits.options().dtype(at::kInt);
+  at::Tensor scores = at::empty({S, E}, f32);
+  at::Tensor idx = at::empty({k, S}, i32), loc = at::empty({k, S}, i32), counts = at::empty({E}, i32);
+  at::Tensor top = at::empty({k, S}, f32), gates = at::empty({k, S}, f32), ce = at::empty({E}, f32);
+  at::Tensor l_aux = at::empty({}, logits.options());
+  at::Tensor me = at::empty({tiles, E}, f32);
+  at::Tensor hist = at::empty({tiles, k, E}, i32);
+  at::Tensor slot;
+  if (C > 0) slot = at::empty({E * C}, i32);
+  TB_CHECK_CUDA(tb::sigmoid_gate_route_forward(
+      logits.data_ptr(), bias.data_ptr<float>(), scores.data_ptr<float>(), idx.data_ptr<int>(), top.data_ptr<float>(),
+      gates.data_ptr<float>(), me.data_ptr<float>(), hist.data_ptr<int>(), loc.data_ptr<int>(), counts.data_ptr<int>(),
+      C > 0 ? slot.data_ptr<int>() : nullptr, ce.data_ptr<float>(), l_aux.data_ptr(), load_p, S, E, static_cast<int>(k),
+      static_cast<int>(C), normalize, static_cast<float>(eps), static_cast<int>(n_group), static_cast<int>(topk_group),
+      static_cast<float>(scale), elem_type_of(logits), cur_stream()));
+  std::vector<at::Tensor> out{scores, idx, top, gates, loc, counts, ce, l_aux};
+  if (C > 0) out.push_back(slot);
+  return out;
+}
+
+// -> d logits [S, E] in `like`'s dtype, as gate_route_backward with the sigmoid closed form; ce = all-choice counts
+at::Tensor sigmoid_gate_route_backward(const at::Tensor& scores, const at::Tensor& idx, const at::Tensor& top,
+                                       const c10::optional<at::Tensor>& dgates, const c10::optional<at::Tensor>& ce,
+                                       const c10::optional<at::Tensor>& dl, const at::Tensor& like, bool normalize,
+                                       double eps, double scale) {
+  TORCH_CHECK(scores.is_cuda() && scores.scalar_type() == at::kFloat && scores.dim() == 2 && scores.is_contiguous());
+  const int S = static_cast<int>(scores.size(0)), E = static_cast<int>(scores.size(1));
+  const int k = static_cast<int>(idx.size(0));
+  TORCH_CHECK(idx.scalar_type() == at::kInt && idx.is_contiguous() && idx.size(1) == S);
+  TORCH_CHECK(top.scalar_type() == at::kFloat && top.is_contiguous() && top.sizes() == idx.sizes());
+  const float* dg_p = nullptr;
+  const float* ce_p = nullptr;
+  const void* dl_p = nullptr;
+  if (dgates.has_value() && dgates->defined()) {
+    TORCH_CHECK(dgates->scalar_type() == at::kFloat && dgates->is_contiguous() && dgates->sizes() == idx.sizes());
+    dg_p = dgates->data_ptr<float>();
+  }
+  if (ce.has_value() && ce->defined() && dl.has_value() && dl->defined()) {
+    TORCH_CHECK(ce->is_cuda() && ce->scalar_type() == at::kFloat && ce->is_contiguous() && ce->numel() == E);
+    TORCH_CHECK(dl->is_cuda() && dl->scalar_type() == like.scalar_type() && dl->numel() == 1);
+    ce_p = ce->data_ptr<float>();
+    dl_p = dl->data_ptr();
+  }
+  const c10::cuda::CUDAGuard guard(scores.device());
+  at::Tensor out = at::empty({S, E}, like.options());
+  TB_CHECK_CUDA(tb::sigmoid_gate_route_backward(scores.data_ptr<float>(), idx.data_ptr<int>(), top.data_ptr<float>(), dg_p,
+                                                ce_p, dl_p, out.data_ptr(), S, E, k, normalize, static_cast<float>(eps),
+                                                static_cast<float>(scale), elem_type_of(like), cur_stream()));
+  return out;
+}
+
+// in place: bias[e] += gamma * sign(mean(load) - load[e]); load = 0      - one launch
+void expert_bias_update(at::Tensor& bias, at::Tensor& load, double gamma) {
+  TORCH_CHECK(bias.is_cuda() && bias.scalar_type() == at::kFloat && bias.is_contiguous(), "expert_bias_update: fp32 CUDA bias expected");
+  TORCH_CHECK(load.device() == bias.device() && load.scalar_type() == at::kFloat && load.is_contiguous() &&
+              load.numel() == bias.numel(), "expert_bias_update: fp32 load of the bias' shape and device expected");
+  const c10::cuda::CUDAGuard guard(bias.device());
+  TB_CHECK_CUDA(tb::expert_bias_update(bias.data_ptr<float>(), load.data_ptr<float>(), static_cast<int>(bias.numel()),
+                                       static_cast<float>(gamma), cur_stream()));
+}
+
 // x [G, T, N] (last dim contiguous) -> [G, N] column sums in x's dtype (fp32 accumulation)
 at::Tensor grouped_colsum(const at::Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 3 && x.stride(2) == 1, "grouped_colsum: CUDA [G, T, N] tensor expected");
@@ -721,6 +805,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gate_grad", &gate_grad);
   m.def("gate_route_forward", &gate_route_forward);
   m.def("gate_route_backward", &gate_route_backward);
+  m.def("sigmoid_gate_route_forward", &sigmoid_gate_route_forward);
+  m.def("sigmoid_gate_route_backward", &sigmoid_gate_route_backward);
+  m.def("expert_bias_update", &expert_bias_update);
   m.def("grouped_colsum", &grouped_colsum);
   m.def("cumsum_sub_one", &cumsum_sub_one);
   m.def("skinny_gemm", &skinny_gemm);

@@ -12,6 +12,12 @@
 //                        slot -> (token, choice) map; block 0 also emits the per-expert counts and the auxiliary loss.
 //
 // Backward of the whole gate is ONE kernel (closed form through normalisation, top-k selection and softmax).
+//
+// Both gate kernels and route_finish_kernel also have a sigmoid instantiation (SIGMOID = true, DeepSeek-V3 routing):
+// scores sigmoid(z), selection on score + per-expert bias, optionally limited to the best `topk_group` of `n_group`
+// expert groups, gates from the unbiased scores times `routed_scaling_factor`, and the balance loss
+// E / (k S^2) sum_e n_e sum_s s_se / T_s on all-choice counts n_e.  expert_bias_update_kernel applies the
+// auxiliary-loss-free balancing step to the bias.
 // Also here: grouped column sums (bias gradients at copy bandwidth) and the public `fast_cumsum_sub_one` scan.
 #include "moe_kernels.h"
 
@@ -36,22 +42,79 @@ template <> __device__ __forceinline__ void stf<float>(float* p, float v) { *p =
 template <> __device__ __forceinline__ void stf<__half>(__half* p, float v) { *p = __float2half_rn(v); }
 template <> __device__ __forceinline__ void stf<__nv_bfloat16>(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
+// Parameters of the sigmoid instantiations (ignored by the softmax ones).
+struct SigmoidArgs {
+  const float* bias;     // [E] selection bias (e_score_correction_bias)
+  float* load;           // [E] += all-choice counts of this call, or null
+  int n_group;           // expert groups; 1 = no group limit
+  int topk_group;        // groups a token may choose from
+  float scale;           // routed_scaling_factor
+};
+
+// Group-limited selection, one warp per token: the score of group g (experts [g*E/n_group, (g+1)*E/n_group)) is the
+// sum of its top min(2, E/n_group) keys, lane g computes it from the warp's key row in shared memory; the best
+// `topk_group` groups are picked by iterative arg-max (ties -> lower group id; NaN / -inf keys and group scores never
+// win against the -inf sentinel).  Returns the lane's experts outside the kept groups as a bit mask over i
+// (bit i: expert lane + 32 i), ready to be OR-ed into the top-k loop's `taken` mask.
+template <int VPT>
+__device__ __forceinline__ unsigned excluded_by_groups(const float* sm_key, int E, int n_group, int topk_group,
+                                                       int lane) {
+  const int gsz = E / n_group;
+  float gs = -INFINITY;
+  if (lane < n_group) {
+    float b1 = -INFINITY, b2 = -INFINITY;
+#pragma unroll 1                    // (unrolled, the group loops push the 16-value instantiations into spills)
+    for (int e = lane * gsz; e < (lane + 1) * gsz; ++e) {
+      const float key = sm_key[e];
+      if (key > b1) { b2 = b1; b1 = key; }
+      else if (key > b2) b2 = key;
+    }
+    gs = gsz > 1 ? b1 + b2 : b1;
+  }
+  unsigned kept = 0;
+#pragma unroll 1
+  for (int t = 0; t < topk_group; ++t) {
+    float best = ((kept >> lane) & 1u) ? -INFINITY : gs;
+    int best_g = best > -INFINITY ? lane : 0x7fffffff;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const int og = __shfl_xor_sync(0xffffffffu, best_g, o);
+      if (ob > best || (ob == best && og < best_g)) { best = ob; best_g = og; }
+    }
+    if (best_g >= 32) break;
+    kept |= 1u << best_g;
+  }
+  unsigned excluded = 0;
+#pragma unroll
+  for (int i = 0; i < VPT; ++i) {
+    const int e = lane + 32 * i;
+    if (e < E && !((kept >> (e / gsz)) & 1u)) excluded |= 1u << i;
+  }
+  return excluded;
+}
+
 // ------------------------------------------------------------------------------------------------
 // launch 1: softmax + top-k + normalised gates + per-tile histograms / importance sums (+ slot map pre-fill)
 // ------------------------------------------------------------------------------------------------
-template <typename T, int VPT>
+template <typename T, int VPT, bool SIGMOID>
 __global__ void __launch_bounds__(kGateThreads)
 gate_route_kernel(const T* __restrict__ logits, float* __restrict__ scores, int* __restrict__ idx,
                   float* __restrict__ top, float* __restrict__ gates, float* __restrict__ me_partial,
                   int* __restrict__ hist, int* __restrict__ slot_src, long long slot_n, int S, int E, int k,
-                  int normalize, float eps) {
-  extern __shared__ int sm_dyn[];                 // [k * E] histogram, then [E] floats of importance sums
+                  int normalize, float eps, SigmoidArgs sg) {
+  // [k * E] histogram, then [E] floats of importance sums; sigmoid: then [E] bias and a [32][E] key row per warp
+  extern __shared__ int sm_dyn[];
   int* sm_hist = sm_dyn;
   float* sm_me = reinterpret_cast<float*>(sm_dyn + k * E);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  float* sm_bias = sm_me + E;
+  float* sm_s = sm_bias + E + warp * E;
   for (int i = threadIdx.x; i < k * E; i += kGateThreads) sm_hist[i] = 0;
   for (int i = threadIdx.x; i < E; i += kGateThreads) sm_me[i] = 0.0f;
+  if constexpr (SIGMOID)
+    for (int i = threadIdx.x; i < E; i += kGateThreads) sm_bias[i] = sg.bias[i];
   for (long long i = static_cast<long long>(blockIdx.x) * kGateThreads + threadIdx.x; i < slot_n;
        i += static_cast<long long>(gridDim.x) * kGateThreads)
     slot_src[i] = -1;
@@ -64,44 +127,75 @@ gate_route_kernel(const T* __restrict__ logits, float* __restrict__ scores, int*
   const long long s_end = min(s_begin + kTileTokens, static_cast<long long>(S));
   for (long long s = s_begin + warp; s < s_end; s += kGateThreads / 32) {
     float v[VPT];
-    float mx = -INFINITY;
+    if constexpr (!SIGMOID) {
+      float mx = -INFINITY;
 #pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-      const int e = lane + 32 * i;
-      v[i] = e < E ? ldf<T>(logits + s * E + e) : -INFINITY;
-      mx = fmaxf(mx, v[i]);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    float sum = 0.0f;
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-      v[i] = (lane + 32 * i < E) ? expf(v[i] - mx) : 0.0f;
-      sum += v[i];
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float inv = 1.0f / sum;
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-      const int e = lane + 32 * i;
-      v[i] *= inv;
-      if (e < E) {
-        scores[s * E + e] = v[i];
-        me[i] += v[i];
+      for (int i = 0; i < VPT; ++i) {
+        const int e = lane + 32 * i;
+        v[i] = e < E ? ldf<T>(logits + s * E + e) : -INFINITY;
+        mx = fmaxf(mx, v[i]);
       }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      float sum = 0.0f;
+#pragma unroll
+      for (int i = 0; i < VPT; ++i) {
+        v[i] = (lane + 32 * i < E) ? expf(v[i] - mx) : 0.0f;
+        sum += v[i];
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      const float inv = 1.0f / sum;
+#pragma unroll
+      for (int i = 0; i < VPT; ++i) {
+        const int e = lane + 32 * i;
+        v[i] *= inv;
+        if (e < E) {
+          scores[s * E + e] = v[i];
+          me[i] += v[i];
+        }
+      }
+    } else {
+      // v = sigmoid(z); me += v / T_s; the selection keys v + bias go to the warp's shared row (read by the group
+      // scores and the top-k loop: at 16 values per lane, registers for both v and me would spill)
+      float tsum = 0.0f;
+#pragma unroll
+      for (int i = 0; i < VPT; ++i) {
+        const int e = lane + 32 * i;
+        v[i] = 0.0f;
+        if (e < E) {
+          v[i] = 1.0f / (1.0f + expf(-ldf<T>(logits + s * E + e)));
+          scores[s * E + e] = v[i];
+        }
+        tsum += v[i];
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) tsum += __shfl_xor_sync(0xffffffffu, tsum, o);
+      const float inv = 1.0f / tsum;
+#pragma unroll
+      for (int i = 0; i < VPT; ++i) {
+        const int e = lane + 32 * i;
+        if (e < E) {
+          me[i] += v[i] * inv;
+          sm_s[e] = v[i] + sm_bias[e];
+        }
+      }
+      __syncwarp();
     }
     // iterative arg-max (ties -> lower expert id); lane j keeps the j-th choice
     unsigned taken = 0;
+    if constexpr (SIGMOID)
+      if (sg.n_group > 1) taken = excluded_by_groups<VPT>(sm_s, E, sg.n_group, sg.topk_group, lane);
     float mine = 0.0f;
     int mine_e = -1;
     for (int j = 0; j < k; ++j) {
-      float best = -1.0f;
+      float best = SIGMOID ? -INFINITY : -1.0f;     // sigmoid keys can be negative (the bias can be)
       int best_e = 0x7fffffff;
 #pragma unroll
       for (int i = 0; i < VPT; ++i) {
         const int e = lane + 32 * i;
-        if (e < E && !((taken >> i) & 1u) && (v[i] > best)) { best = v[i]; best_e = e; }
+        const float key = SIGMOID ? (e < E ? sm_s[e] : 0.0f) : v[i];
+        if (e < E && !((taken >> i) & 1u) && (key > best)) { best = key; best_e = e; }
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
@@ -115,15 +209,18 @@ gate_route_kernel(const T* __restrict__ logits, float* __restrict__ scores, int*
       }
       if (lane == j) { mine = best; mine_e = best_e; }
     }
+    if constexpr (SIGMOID) mine = (lane < k && mine_e >= 0 && mine_e < E) ? scores[s * E + mine_e] : 0.0f;   // unbiased
     float denom = (lane < k) ? mine : 0.0f;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) denom += __shfl_xor_sync(0xffffffffu, denom, o);
     if (lane < k) {
-      const float g = (normalize != 0 && k > 1) ? mine / fmaxf(denom, eps) : mine;
+      float g = (normalize != 0 && k > 1) ? mine / fmaxf(denom, eps) : mine;
+      if constexpr (SIGMOID) g *= sg.scale;
       idx[static_cast<long long>(lane) * S + s] = mine_e;
       top[static_cast<long long>(lane) * S + s] = mine;
       gates[static_cast<long long>(lane) * S + s] = g;
     }
+    if constexpr (SIGMOID) __syncwarp();          // the next token overwrites this warp's score row
   }
 #pragma unroll
   for (int i = 0; i < VPT; ++i)
@@ -136,11 +233,13 @@ gate_route_kernel(const T* __restrict__ logits, float* __restrict__ scores, int*
 // ------------------------------------------------------------------------------------------------
 // launch 2: queue offsets from the tile histograms, in-tile ranking, locations, slot map, counts, loss
 // ------------------------------------------------------------------------------------------------
-template <typename T>
+// Sigmoid mode: the loss, ce_out and `load` use the all-choice counts n_e, me_partial holds sums of s_se / T_s.
+template <typename T, bool SIGMOID>
 __global__ void __launch_bounds__(kTileTokens)
 route_finish_kernel(const int* __restrict__ idx, const int* __restrict__ hist, const float* __restrict__ me_partial,
                     int* __restrict__ loc, int* __restrict__ counts, int* __restrict__ slot_src,
-                    float* __restrict__ ce_out, T* __restrict__ l_aux, int S, int E, int k, int C, int ntiles) {
+                    float* __restrict__ ce_out, T* __restrict__ l_aux, int S, int E, int k, int C, int ntiles,
+                    float* __restrict__ load) {
   extern __shared__ int sm_dyn[];        // total[k*E] | base[k*E] | cnt[E]
   int* sm_total = sm_dyn;
   int* sm_base = sm_dyn + k * E;
@@ -176,8 +275,10 @@ route_finish_kernel(const int* __restrict__ idx, const int* __restrict__ hist, c
       int c = 0;
       for (int j = 0; j < k; ++j) c += sm_total[j * E + e];
       counts[e] = c;
-      const float ce = static_cast<float>(sm_total[e]);
+      const float ce = static_cast<float>(SIGMOID ? c : sm_total[e]);
       if (ce_out != nullptr) ce_out[e] = ce;
+      if constexpr (SIGMOID)
+        if (load != nullptr) load[e] += ce;
       float me = 0.0f;
       for (int t = 0; t < ntiles; ++t) me += me_partial[static_cast<long long>(t) * E + e];
       part += me * ce;
@@ -189,7 +290,8 @@ route_finish_kernel(const int* __restrict__ idx, const int* __restrict__ hist, c
     if (threadIdx.x == 0 && l_aux != nullptr) {
       float tot = 0.0f;
       for (int w = 0; w < kTileTokens / 32; ++w) tot += sm_red[w];
-      stf<T>(l_aux, tot * static_cast<float>(E) / (static_cast<float>(S) * static_cast<float>(S)));
+      const float ss = static_cast<float>(S) * static_cast<float>(S);
+      stf<T>(l_aux, tot * static_cast<float>(E) / (SIGMOID ? static_cast<float>(k) * ss : ss));
     }
   }
   // (3) stable rank of every token inside its tile, choice by choice
@@ -232,23 +334,47 @@ route_finish_kernel(const int* __restrict__ idx, const int* __restrict__ hist, c
 //   dr_j = dg_j / Dc - [D > eps] * (sum_i dg_i r_i) / Dc^2
 //   dp_e = dl * ce_e * E / S^2 + sum_j [idx_j == e] dr_j        (l_aux = E/S^2 * sum_e me_e ce_e; ce is constant)
 //   dlogit_e = p_e * (dp_e - sum_e' dp_e' p_e')
+// Sigmoid (p = sigmoid scores, ce = all-choice counts n, T = sum_e p_e, l_aux = E/(k S^2) sum_e n_e sum_s p_se / T_s):
+//   dr_j scaled by routed_scaling_factor
+//   dp_e = dl E / (k S^2 T) * (n_e - sum_e' n_e' p_e' / T) + sum_j [idx_j == e] dr_j
+//   dlogit_e = p_e (1 - p_e) dp_e
 // ------------------------------------------------------------------------------------------------
-template <typename T, int VPT>
+template <typename T, int VPT, bool SIGMOID>
 __global__ void __launch_bounds__(256)
 gate_route_bwd_kernel(const float* __restrict__ scores, const int* __restrict__ idx, const float* __restrict__ top,
                       const float* __restrict__ dgates, const float* __restrict__ ce, const T* __restrict__ dl,
-                      T* __restrict__ dlogits, int S, int E, int k, int normalize, float eps) {
+                      T* __restrict__ dlogits, int S, int E, int k, int normalize, float eps, float scale) {
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const float ss = static_cast<float>(S) * static_cast<float>(S);
   const float aux_scale = (dl != nullptr ? ldf<T>(dl) : 0.0f) * static_cast<float>(E) /
-                          (static_cast<float>(S) * static_cast<float>(S));
+                          (SIGMOID ? static_cast<float>(k) * ss : ss);
   for (long long s = static_cast<long long>(blockIdx.x) * 8 + warp; s < S; s += static_cast<long long>(gridDim.x) * 8) {
     float p[VPT], dp[VPT];
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
       const int e = lane + 32 * i;
       p[i] = e < E ? scores[s * E + e] : 0.0f;
-      dp[i] = (e < E && ce != nullptr) ? aux_scale * ce[e] : 0.0f;
+      if constexpr (SIGMOID) dp[i] = (e < E && ce != nullptr) ? ce[e] : 0.0f;
+      else dp[i] = (e < E && ce != nullptr) ? aux_scale * ce[e] : 0.0f;
+    }
+    if constexpr (SIGMOID) {
+      if (ce != nullptr) {
+        float t = 0.0f, nd = 0.0f;
+#pragma unroll
+        for (int i = 0; i < VPT; ++i) {
+          t += p[i];
+          nd += dp[i] * p[i];
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          t += __shfl_xor_sync(0xffffffffu, t, o);
+          nd += __shfl_xor_sync(0xffffffffu, nd, o);
+        }
+        const float c = aux_scale / t, m = nd / t;
+#pragma unroll
+        for (int i = 0; i < VPT; ++i) dp[i] = c * (dp[i] - m);
+      }
     }
     // lane j owns choice j
     const float r = lane < k ? top[static_cast<long long>(lane) * S + s] : 0.0f;
@@ -265,6 +391,7 @@ gate_route_bwd_kernel(const float* __restrict__ scores, const int* __restrict__ 
       const float Dc = fmaxf(D, eps);
       dr = dg / Dc - (D > eps ? dot / (Dc * Dc) : 0.0f);
     }
+    if constexpr (SIGMOID) dr *= scale;
     for (int j = 0; j < k; ++j) {
       const int e = __shfl_sync(0xffffffffu, my_e, j);
       const float d = __shfl_sync(0xffffffffu, dr, j);
@@ -273,6 +400,14 @@ gate_route_bwd_kernel(const float* __restrict__ scores, const int* __restrict__ 
         for (int i = 0; i < VPT; ++i)
           if (i == (e >> 5)) dp[i] += d;
       }
+    }
+    if constexpr (SIGMOID) {
+#pragma unroll
+      for (int i = 0; i < VPT; ++i) {
+        const int e = lane + 32 * i;
+        if (e < E) stf<T>(dlogits + s * E + e, p[i] * (1.0f - p[i]) * dp[i]);
+      }
+      continue;
     }
     float acc = 0.0f;
 #pragma unroll
@@ -284,6 +419,29 @@ gate_route_bwd_kernel(const float* __restrict__ scores, const int* __restrict__ 
       const int e = lane + 32 * i;
       if (e < E) stf<T>(dlogits + s * E + e, p[i] * (dp[i] - acc));
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// auxiliary-loss-free balancing: bias_e += gamma * sign(mean(load) - load_e), then load = 0.  One block; the loads are
+// integer-valued, so their fp32 sum is exact (below 2^24) and the result does not depend on the summation order.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(1024)
+expert_bias_update_kernel(float* __restrict__ bias, float* __restrict__ load, int E, float gamma) {
+  __shared__ float sm_red[32];
+  float part = 0.0f;
+  for (int e = threadIdx.x; e < E; e += 1024) part += load[e];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  if ((threadIdx.x & 31) == 0) sm_red[threadIdx.x >> 5] = part;
+  __syncthreads();
+  float tot = 0.0f;
+  for (int w = 0; w < 32; ++w) tot += sm_red[w];
+  const float mean = tot / static_cast<float>(E);
+  for (int e = threadIdx.x; e < E; e += 1024) {
+    const float d = mean - load[e];
+    bias[e] = bias[e] + gamma * static_cast<float>((d > 0.0f) - (d < 0.0f));
+    load[e] = 0.0f;
   }
 }
 
@@ -426,24 +584,25 @@ static cudaError_t allow_dynamic_smem(const void* fn, size_t bytes) {
   return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
 }
 
-template <typename T>
+template <typename T, bool SIGMOID>
 static cudaError_t gate_route_forward_t(const void* logits, float* scores, int* idx, float* top, float* gates,
                                         float* me_partial, int* hist, int* loc, int* counts, int* slot_src,
                                         float* ce_out, void* l_aux, int S, int E, int k, int C, bool normalize, float eps,
-                                        cudaStream_t stream) {
+                                        const SigmoidArgs& sg, cudaStream_t stream) {
   const int ntiles = gate_route_tiles(S);
   const long long slot_n = slot_src != nullptr ? static_cast<long long>(E) * C : 0;
-  const size_t smem1 = sizeof(int) * static_cast<size_t>(k) * E + sizeof(float) * E;
+  const size_t smem1 = sizeof(int) * static_cast<size_t>(k) * E + sizeof(float) * E +
+                       (SIGMOID ? sizeof(float) * E * (1 + kGateThreads / 32) : 0);
   const size_t smem2 = sizeof(int) * (2 * static_cast<size_t>(k) * E + E);
-  cudaError_t err = allow_dynamic_smem(reinterpret_cast<const void*>(route_finish_kernel<T>), smem2);
+  cudaError_t err = allow_dynamic_smem(reinterpret_cast<const void*>(route_finish_kernel<T, SIGMOID>), smem2);
   if (err != cudaSuccess) return err;
 #define TB_GR(VPTv)                                                                                                   \
   do {                                                                                                                \
-    if ((err = allow_dynamic_smem(reinterpret_cast<const void*>(gate_route_kernel<T, VPTv>), smem1)) != cudaSuccess)  \
-      return err;                                                                                                     \
-    gate_route_kernel<T, VPTv><<<ntiles, kGateThreads, smem1, stream>>>(static_cast<const T*>(logits), scores, idx,   \
-                                                                        top, gates, me_partial, hist, slot_src,       \
-                                                                        slot_n, S, E, k, normalize ? 1 : 0, eps);     \
+    const void* fn = reinterpret_cast<const void*>(gate_route_kernel<T, VPTv, SIGMOID>);                              \
+    if ((err = allow_dynamic_smem(fn, smem1)) != cudaSuccess) return err;                                             \
+    gate_route_kernel<T, VPTv, SIGMOID><<<ntiles, kGateThreads, smem1, stream>>>(                                     \
+        static_cast<const T*>(logits), scores, idx, top, gates, me_partial, hist, slot_src, slot_n, S, E, k,          \
+        normalize ? 1 : 0, eps, sg);                                                                                  \
   } while (0)
   if (E <= 32) TB_GR(1);
   else if (E <= 64) TB_GR(2);
@@ -452,8 +611,9 @@ static cudaError_t gate_route_forward_t(const void* logits, float* scores, int* 
   else if (E <= 512) TB_GR(16);
   else return cudaErrorInvalidValue;
 #undef TB_GR
-  route_finish_kernel<T><<<ntiles, kTileTokens, smem2, stream>>>(idx, hist, me_partial, loc, counts, slot_src, ce_out,
-                                                                 static_cast<T*>(l_aux), S, E, k, C, ntiles);
+  route_finish_kernel<T, SIGMOID><<<ntiles, kTileTokens, smem2, stream>>>(idx, hist, me_partial, loc, counts, slot_src,
+                                                                          ce_out, static_cast<T*>(l_aux), S, E, k, C,
+                                                                          ntiles, sg.load);
   return cudaGetLastError();
 }
 
@@ -461,23 +621,44 @@ cudaError_t gate_route_forward(const void* logits, float* scores, int* idx, floa
                                int* hist, int* loc, int* counts, int* slot_src, float* ce_out, void* l_aux, int S, int E,
                                int k, int C, bool normalize, float eps, int elem_type, cudaStream_t stream) {
   if (S <= 0 || k > 32 || k <= 0) return cudaErrorInvalidValue;
+  const SigmoidArgs sg{nullptr, nullptr, 1, 1, 1.0f};
   switch (elem_type) {
-    case ET_F32: return gate_route_forward_t<float>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, stream);
-    case ET_F16: return gate_route_forward_t<__half>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, stream);
-    case ET_BF16: return gate_route_forward_t<__nv_bfloat16>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, stream);
+    case ET_F32: return gate_route_forward_t<float, false>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, sg, stream);
+    case ET_F16: return gate_route_forward_t<__half, false>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, sg, stream);
+    case ET_BF16: return gate_route_forward_t<__nv_bfloat16, false>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, sg, stream);
   }
   return cudaErrorInvalidValue;
 }
 
-template <typename T>
+cudaError_t sigmoid_gate_route_forward(const void* logits, const float* bias, float* scores, int* idx, float* top,
+                                       float* gates, float* me_partial, int* hist, int* loc, int* counts, int* slot_src,
+                                       float* ce_out, void* l_aux, float* load, int S, int E, int k, int C,
+                                       bool normalize, float eps, int n_group, int topk_group, float scale,
+                                       int elem_type, cudaStream_t stream) {
+  if (S <= 0 || k > 32 || k <= 0 || bias == nullptr) return cudaErrorInvalidValue;
+  if (n_group < 1 || n_group > 32 || E % n_group != 0 || topk_group < 1 || topk_group > n_group ||
+      k > topk_group * (E / n_group))
+    return cudaErrorInvalidValue;
+  const SigmoidArgs sg{bias, load, n_group, topk_group, scale};
+  switch (elem_type) {
+    case ET_F32: return gate_route_forward_t<float, true>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, sg, stream);
+    case ET_F16: return gate_route_forward_t<__half, true>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, sg, stream);
+    case ET_BF16: return gate_route_forward_t<__nv_bfloat16, true>(logits, scores, idx, top, gates, me_partial, hist, loc, counts, slot_src, ce_out, l_aux, S, E, k, C, normalize, eps, sg, stream);
+  }
+  return cudaErrorInvalidValue;
+}
+
+template <typename T, bool SIGMOID>
 static cudaError_t gate_route_backward_t(const float* scores, const int* idx, const float* top, const float* dgates,
                                          const float* ce, const void* dl, void* dlogits, int S, int E, int k,
-                                         bool normalize, float eps, cudaStream_t stream) {
+                                         bool normalize, float eps, float scale, cudaStream_t stream) {
   const long long want = (static_cast<long long>(S) + 7) / 8;
   const int grid = static_cast<int>(want < 4LL * sm_count() ? want : 4LL * sm_count());
-#define TB_GRB(VPTv)                                                                                          \
-  gate_route_bwd_kernel<T, VPTv><<<grid, 256, 0, stream>>>(scores, idx, top, dgates, ce, static_cast<const T*>(dl), \
-                                                           static_cast<T*>(dlogits), S, E, k, normalize ? 1 : 0, eps)
+#define TB_GRB(VPTv)                                                                                             \
+  gate_route_bwd_kernel<T, VPTv, SIGMOID><<<grid, 256, 0, stream>>>(scores, idx, top, dgates, ce,                \
+                                                                    static_cast<const T*>(dl),                 \
+                                                                    static_cast<T*>(dlogits), S, E, k,          \
+                                                                    normalize ? 1 : 0, eps, scale)
   if (E <= 32) TB_GRB(1);
   else if (E <= 64) TB_GRB(2);
   else if (E <= 128) TB_GRB(4);
@@ -494,11 +675,30 @@ cudaError_t gate_route_backward(const float* scores, const int* idx, const float
   if (S <= 0) return cudaSuccess;
   if (k > 32) return cudaErrorInvalidValue;
   switch (elem_type) {
-    case ET_F32: return gate_route_backward_t<float>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, stream);
-    case ET_F16: return gate_route_backward_t<__half>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, stream);
-    case ET_BF16: return gate_route_backward_t<__nv_bfloat16>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, stream);
+    case ET_F32: return gate_route_backward_t<float, false>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, 1.0f, stream);
+    case ET_F16: return gate_route_backward_t<__half, false>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, 1.0f, stream);
+    case ET_BF16: return gate_route_backward_t<__nv_bfloat16, false>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, 1.0f, stream);
   }
   return cudaErrorInvalidValue;
+}
+
+cudaError_t sigmoid_gate_route_backward(const float* scores, const int* idx, const float* top, const float* dgates,
+                                        const float* ce, const void* dl, void* dlogits, int S, int E, int k,
+                                        bool normalize, float eps, float scale, int elem_type, cudaStream_t stream) {
+  if (S <= 0) return cudaSuccess;
+  if (k > 32) return cudaErrorInvalidValue;
+  switch (elem_type) {
+    case ET_F32: return gate_route_backward_t<float, true>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, scale, stream);
+    case ET_F16: return gate_route_backward_t<__half, true>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, scale, stream);
+    case ET_BF16: return gate_route_backward_t<__nv_bfloat16, true>(scores, idx, top, dgates, ce, dl, dlogits, S, E, k, normalize, eps, scale, stream);
+  }
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t expert_bias_update(float* bias, float* load, int E, float gamma, cudaStream_t stream) {
+  if (E <= 0) return cudaSuccess;
+  expert_bias_update_kernel<<<1, 1024, 0, stream>>>(bias, load, E, gamma);
+  return cudaGetLastError();
 }
 
 int colsum_row_splits(int G, int rows, int N, int elem_bytes) {

@@ -65,6 +65,20 @@ cudaError_t gate_route_forward(const void* logits, float* scores, int* idx, floa
 cudaError_t gate_route_backward(const float* scores, const int* idx, const float* top, const float* dgates,
                                 const float* ce, const void* dl, void* dlogits, int S, int E, int k, bool normalize,
                                 float eps, int elem_type, cudaStream_t stream);
+// Sigmoid scoring (DeepSeek-V3 routing), same outputs and workspaces as gate_route_forward: scores = sigmoid(logits),
+// ids chosen on scores + bias[E] (fp32) among the best `topk_group` of `n_group` expert groups (n_group <= 32),
+// top = the unbiased scores, gates = scale * normalised top, ce = fp32 all-choice counts, l_aux the balance loss
+// E / (k S^2) sum_e n_e sum_s s_se / T_s.  `load` (fp32 [E], may be null) accumulates the all-choice counts.
+cudaError_t sigmoid_gate_route_forward(const void* logits, const float* bias, float* scores, int* idx, float* top,
+                                       float* gates, float* me_partial, int* hist, int* loc, int* counts, int* slot_src,
+                                       float* ce_out, void* l_aux, float* load, int S, int E, int k, int C,
+                                       bool normalize, float eps, int n_group, int topk_group, float scale,
+                                       int elem_type, cudaStream_t stream);
+cudaError_t sigmoid_gate_route_backward(const float* scores, const int* idx, const float* top, const float* dgates,
+                                        const float* ce, const void* dl, void* dlogits, int S, int E, int k,
+                                        bool normalize, float eps, float scale, int elem_type, cudaStream_t stream);
+// bias[e] += gamma * sign(mean(load) - load[e]); load = 0.  One launch, fp32 [E] both.
+cudaError_t expert_bias_update(float* bias, float* load, int E, float gamma, cudaStream_t stream);
 
 // out[g, n] = sum_r x[g, r, n]  (bias gradients).  splits = colsum_row_splits(..): 1 -> results are written to `out`
 // (dtype of x); > 1 -> partial sums are atomically added to the zero-initialised fp32 buffer `acc` [G, N].

@@ -26,7 +26,8 @@ from torch import Tensor
 from torch.nn import ModuleList
 
 from ..ops.dispatch import fast_decode, fast_encode
-from ..ops.gating import fused_gate_mode, fused_gate_route_available, fused_topk_gate
+from ..ops.gating import (fused_gate_mode, fused_gate_route_available, fused_topk_gate, sigmoid_gate_route_available,
+                          sigmoid_topk_gate)
 from ..ops.routing import extract_critical, fused_extract_critical, get_dispatch_count
 from ..parallel import communicate as C
 from ..parallel.overlap import a2a_ffn_overlap_forward
@@ -186,6 +187,12 @@ class MOELayer(torch.nn.Module):
                 torch.manual_seed(seeds[0] + gi)
             gates.append(self._build_gate(spec))
         self.gates = ModuleList(gates)
+        for gate in self.gates:
+            if getattr(gate, 'scoring_func', 'softmax') == 'sigmoid':
+                if not self.is_gshard_loss:
+                    raise ValueError('is_gshard_loss=False is not supported with a sigmoid gate: the load-importance '
+                                     'loss is defined on softmax scores')
+                gate.balance_group = self.group
 
         if seeds is not None and len(seeds) > 2 and seeds[2] is not None:
             torch.manual_seed(seeds[2])
@@ -259,6 +266,9 @@ class MOELayer(torch.nn.Module):
         alignment = (self.sharded_count * a2a_ffn_overlap_degree + mega - 1) // mega * mega
         if alignment > 256:
             alignment = (alignment + 127) // 128 * 128
+        if getattr(gctx, 'scoring_func', 'softmax') == 'sigmoid':
+            return self._route_sigmoid(x, logits, logits_w_noise, gctx, top_k, capacity_factor, alignment,
+                                       megablocks_size, inequivalent_tokens)
         fused_gate, gate_mode = None, fused_gate_mode()
         k_eff = min(top_k, self.num_global_experts)
         cuda_fused = (self.is_gshard_loss and gate_mode != 'off' and not self.batch_prioritized_routing and
@@ -267,13 +277,7 @@ class MOELayer(torch.nn.Module):
             if cuda_fused:
                 # CUDA: gate + routing in two launches, gate backward in one (ops/gating.py, csrc/gate_route.cu)
                 cf = capacity_factor or gctx.capacity_factor
-                bound = 0
-                if cf <= 0 and megablocks_size > 0 and self.world_size == 1 and not inequivalent_tokens:
-                    # single-GPU dropless inference: a worst-case row bound replaces the host read-back of the capacity
-                    S = int(logits_w_noise.size(0))
-                    budget = int(os.environ.get('TUTEL_B200_DROPLESS_BOUND_MB', 512)) << 20
-                    if S * self.num_global_experts * self.model_dim * x.element_size() <= budget:
-                        bound = S
+                bound = self._dropless_bound(logits_w_noise, x, cf, megablocks_size, inequivalent_tokens)
                 crit, l_aux = fused_extract_critical(logits_w_noise, top_k, cf, self.normalize_gate, alignment, self.group,
                                                      inequivalent_tokens, rows_bound=bound)
                 if getattr(crit, 'skip_padding', False) and not getattr(self.experts, 'rows_independent', False):
@@ -297,6 +301,55 @@ class MOELayer(torch.nn.Module):
                                        normalize_gate=self.normalize_gate, group=self.group, alignment=alignment,
                                        inequivalent_tokens=inequivalent_tokens, _fused=fused_gate)
         return logits.dtype, crit, l_aux
+
+    def _dropless_bound(self, logits, x, cf, megablocks_size, inequivalent_tokens):
+        """Single-GPU dropless inference: a worst-case row bound replaces the host read-back of the capacity."""
+        if cf <= 0 and megablocks_size > 0 and self.world_size == 1 and not inequivalent_tokens:
+            S = int(logits.size(0))
+            budget = int(os.environ.get('TUTEL_B200_DROPLESS_BOUND_MB', 512)) << 20
+            if S * self.num_global_experts * self.model_dim * x.element_size() <= budget:
+                return S
+        return 0
+
+    def _route_sigmoid(self, x, logits, logits_w_noise, gctx, top_k, capacity_factor, alignment, megablocks_size,
+                       inequivalent_tokens):
+        """Sigmoid scoring with the gate's selection bias and group limit (ops/gating.py).  Training forwards with
+        gradients add their all-choice counts to the gate's ``expert_load`` for the next bias update."""
+        k_eff = min(top_k, self.num_global_experts)
+        gctx.check_top_k(k_eff)
+        accumulate = gctx.balancing and gctx.training and torch.is_grad_enabled()
+        load = gctx.expert_load if accumulate else None
+        args = dict(bias=gctx.e_score_correction_bias, n_group=gctx.n_group, topk_group=gctx.topk_group,
+                    scale=gctx.routed_scaling_factor)
+        cf = capacity_factor or gctx.capacity_factor
+        if (fused_gate_mode() != 'off' and not self.batch_prioritized_routing and
+                sigmoid_gate_route_available(logits_w_noise, k_eff, gctx.n_group)):
+            # CUDA: gate + routing in two launches (the loads are added inside the second), backward in one
+            bound = self._dropless_bound(logits_w_noise, x, cf, megablocks_size, inequivalent_tokens)
+            crit, l_aux = fused_extract_critical(logits_w_noise, top_k, cf, self.normalize_gate, alignment, self.group,
+                                                 inequivalent_tokens, rows_bound=bound,
+                                                 sigmoid=dict(args, expert_load=load))
+            if getattr(crit, 'skip_padding', False) and not getattr(self.experts, 'rows_independent', False):
+                crit.skip_padding = False
+        else:
+            idx, gates, l_aux, counts, top1 = sigmoid_topk_gate(logits_w_noise, k=k_eff, normalize=self.normalize_gate,
+                                                                **args)
+            if load is not None:
+                load.add_(counts)
+            crit, _ = extract_critical(logits_w_noise, top_k=top_k, loss_fn=None, capacity_factor=cf,
+                                       batch_prioritized_routing=self.batch_prioritized_routing,
+                                       normalize_gate=self.normalize_gate, group=self.group, alignment=alignment,
+                                       inequivalent_tokens=inequivalent_tokens, _fused=(idx, gates, l_aux, top1))
+        if accumulate:
+            gctx.note_training_forward()
+        return logits.dtype, crit, l_aux
+
+    def update_expert_bias(self):
+        """Apply the pending auxiliary-loss-free bias update of every sigmoid gate of this layer.  An optimizer-step
+        post-hook does this after every ``torch.optim`` step; call it in loops that update parameters otherwise."""
+        for gate in self.gates:
+            if getattr(gate, 'scoring_func', 'softmax') == 'sigmoid':
+                gate.update_bias()
 
     def forward(self, input: Tensor, gate_index=0, capacity_factor=None, top_k=None, a2a_ffn_overlap_degree=None,
                 reserve_dims=1, inequivalent_tokens=False, adaptive_r=None, megablocks_size=0):

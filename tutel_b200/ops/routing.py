@@ -137,11 +137,15 @@ def _capacity(num_samples, num_global_experts, top_k, top_k_original, capacity_f
 
 
 def fused_extract_critical(logits: torch.Tensor, top_k: int, capacity_factor: float = 1.0, normalize_gate: bool = True,
-                           alignment: int = 1, group=None, inequivalent_tokens: bool = False, rows_bound: int = 0):
+                           alignment: int = 1, group=None, inequivalent_tokens: bool = False, rows_bound: int = 0,
+                           sigmoid: Optional[dict] = None):
     """CUDA fast path of :func:`extract_critical` for GShard-loss top-k gates: softmax, top-k, gate normalisation, the
     auxiliary loss, queue locations, counts and the inverse slot map come out of TWO kernel launches
-    (:func:`tutel_b200.ops.gating.fused_gate_route`); with a positive capacity factor nothing touches the host."""
-    from .gating import fused_gate_route
+    (:func:`tutel_b200.ops.gating.fused_gate_route`); with a positive capacity factor nothing touches the host.
+
+    ``sigmoid``: sigmoid scoring instead (:func:`tutel_b200.ops.gating.sigmoid_gate_route`), a dict with ``bias``,
+    ``n_group``, ``topk_group``, ``scale`` and ``expert_load`` (or None)."""
+    from .gating import fused_gate_route, sigmoid_gate_route
     E = int(logits.size(1))
     top_k_original, top_k = top_k, min(top_k, E)
     num_samples = _num_samples(int(logits.size(0)), logits.device, group, inequivalent_tokens)
@@ -153,7 +157,11 @@ def fused_extract_critical(logits: torch.Tensor, top_k: int, capacity_factor: fl
         static_cap = rows_bound if capacity_factor == 0 else min(rows_bound, top_k * int(-capacity_factor * ((num_samples + E - 1) // E)))
         static_cap = (static_cap + alignment - 1) // alignment * alignment
         capacity_factor = 1.0          # (only selects the "capacity is already known" branch below)
-    idx, loc, gates, l_aux, counts, _top1, slot = fused_gate_route(logits, top_k, normalize_gate, static_cap)
+    if sigmoid is None:
+        idx, loc, gates, l_aux, counts, _top1, slot = fused_gate_route(logits, top_k, normalize_gate, static_cap)
+    else:
+        idx, loc, gates, l_aux, counts, _top1, slot = sigmoid_gate_route(logits, k=top_k, normalize=normalize_gate,
+                                                                         capacity=static_cap, **sigmoid)
     capacity = static_cap if capacity_factor > 0 else \
         _capacity(num_samples, E, top_k, top_k_original, capacity_factor, counts, group, alignment)
     crit = CriticalData(E, idx, loc, gates, capacity, counts)
