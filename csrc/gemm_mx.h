@@ -8,7 +8,8 @@ namespace tb {
 // Scale factors (UE8M0, one per 32 consecutive K elements of a row) are stored in the tile order the tensor core
 // reads them from shared memory:   sf[g][kb][rt][ (r % 32) * 16 + ((r % 128) / 32) * 4 + (k % 128) / 32 ]
 // with kb = k / 128, rt = r / 128 - one 512-byte atom per 128 rows x 128 K elements, so a CTA stages the scales of a
-// whole operand tile with a single bulk copy.  Rows are padded to a multiple of 128 (pad scales are 0 = 2^-127).
+// whole operand tile with a single bulk copy.  Rows are padded to a multiple of 128 with byte 0.  A block with a non-zero
+// element has a byte in [1, 253] (e in [-126, 126]); byte 0 (a block that is all zero or NaN, a pad row) decodes to a scale of 0.
 inline long long mx_sf_bytes(int groups, long long rows, long long k) {
   return static_cast<long long>(groups) * (k / 128) * ((rows + 127) / 128) * 512;
 }
@@ -43,6 +44,7 @@ struct MxGemmProblem {
   int max_ctas = 0;              // 0: one CTA per SM
 };
 
+// sa * sb is formed in fp32, so ea + eb (byte_a + byte_b - 254) must stay in fp32's normal exponent range [-126, 127].
 cudaError_t mx_gemm_launch(const MxGemmProblem& p, cudaStream_t stream, const char** why = nullptr);
 
 }  // namespace tb

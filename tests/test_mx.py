@@ -16,7 +16,7 @@ def test_scale_layout_round_trip_and_atom_offsets():
     RT = 2
     off = ((g * (K // 128) + k // 128) * RT + r // 128) * 512 + (r % 32) * 16 + ((r % 128) // 32) * 4 + (k % 128) // 32
     assert int(sf[off]) == int(e[g, r, k // 32]) + 127
-    # padded rows carry byte 0 (2^-127)
+    # padded rows carry byte 0, which decodes to a scale of 0
     r = 250
     off = ((0 * (K // 128) + 0) * RT + r // 128) * 512 + (r % 32) * 16 + ((r % 128) // 32) * 4
     assert int(sf[off]) == 0

@@ -8,9 +8,10 @@ csrc/gemm_sm90.cu, this module is the finer-grained alternative for GEMMs whose 
 Everything here also has a pure PyTorch definition (``*_reference``) that runs on CPU: the tests compare the kernels
 against it, and it documents the number format:
 
-* block exponent   ``e = ceil(log2(amax / 448))`` clamped to [-127, 126]
-* elements         ``q = e4m3_rn(x * 2**-e)``
-* scale byte       ``e + 127``
+* block exponent   ``e = ceil(log2(amax / 448))`` clamped to [-126, 126] for a block with a non-zero element, where
+  ``amax`` is the largest magnitude that is not NaN; ``e = -127`` (scale byte 0) for a block whose ``amax`` is 0
+* elements         ``q = e4m3_rn_satfinite(x * 2**-e)`` (+-inf saturate to +-448, NaN stays NaN)
+* scale byte       ``e + 127``; byte 0 decodes to a scale of 0, not 2**-127 (the GEMM kernel and :func:`mx_dequantize`)
 * scale storage    ``sf[g][k // 128][r // 128][(r % 32) * 16 + ((r % 128) // 32) * 4 + (k % 128) // 32]`` - 512-byte
   atoms in the order the tensor core reads them from tensor memory (rows padded to a multiple of 128 with byte 0).
 """
@@ -33,8 +34,12 @@ def _check_k(K: int):
 
 def block_exponents_reference(x: torch.Tensor) -> torch.Tensor:
     """Shared exponents [.., K / 32] (int32) of the 32-element blocks along the last dim."""
-    amax = x.float().abs().reshape(*x.shape[:-1], x.shape[-1] // BLOCK, BLOCK).amax(-1)
-    # ceil(log2(v)) from the float representation: exponent field (+1 when the mantissa is non-zero), as the kernel does
+    a = x.float().abs()
+    # NaN takes no part in the maximum (the kernels' fmaxf): the block's other elements keep their scale
+    a = torch.where(torch.isnan(a), torch.zeros_like(a), a)
+    amax = a.reshape(*x.shape[:-1], x.shape[-1] // BLOCK, BLOCK).amax(-1)
+    # ceil(log2(v)) from the float representation: exponent field (+1 when the mantissa is non-zero), as the kernel does.
+    # Below 448 * 2^-126, v is an fp32 subnormal and this gives -126; only amax == 0 gives -127.
     v = (amax * (1.0 / E4M3_MAX)).contiguous()
     bits = v.view(torch.int32)
     e = ((bits >> 23) & 0xFF) - 127 + ((bits & 0x7FFFFF) != 0).to(torch.int32)
@@ -73,10 +78,12 @@ def mx_quantize_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
 
 
 def mx_dequantize(q: torch.Tensor, sf: torch.Tensor) -> torch.Tensor:
-    """fp32 values of an MX operand (pure PyTorch)."""
+    """fp32 values of an MX operand (pure PyTorch).  Scale byte 0 (e = -127, only all-zero blocks and padded rows) is
+    a scale of 0, as in the GEMM kernel."""
     G, R, K = q.shape
     e = unpack_scales(sf, G, R, K)
-    return (q.float().view(G, R, K // BLOCK, BLOCK) * torch.exp2(e.float()).unsqueeze(-1)).view(G, R, K)
+    s = torch.where(e == -127, torch.zeros_like(e, dtype=torch.float32), torch.exp2(e.float()))
+    return (q.float().view(G, R, K // BLOCK, BLOCK) * s.unsqueeze(-1)).view(G, R, K)
 
 
 def mx_quantize(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
