@@ -44,16 +44,37 @@ int elem_type_of(const at::Tensor& t) {
 
 cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
+// Optional packed-layout launch modes of the grouped GEMM (see GemmProblem): b_group_map int [G] (B group of each
+// A group), k_offsets int [G + 1] (ragged K: a [1, K, M] / b [1, K, N], d [G, M, N]).
+void set_packed_modes(tb::GemmProblem& p, const at::Tensor& a, const at::Tensor& b, const at::Tensor& d,
+                      const c10::optional<at::Tensor>& b_group_map, const c10::optional<at::Tensor>& k_offsets) {
+  if (b_group_map.has_value() && b_group_map->defined()) {
+    TORCH_CHECK(b_group_map->is_cuda() && b_group_map->scalar_type() == at::kInt && b_group_map->is_contiguous() &&
+                    b_group_map->numel() >= p.G, "tutel_b200.gemm: b_group_map must be a contiguous int32 [G]");
+    p.b_group_map = b_group_map->data_ptr<int>();
+    p.b_groups = static_cast<int>(b.size(0));
+  }
+  if (k_offsets.has_value() && k_offsets->defined()) {
+    TORCH_CHECK(k_offsets->is_cuda() && k_offsets->scalar_type() == at::kInt && k_offsets->is_contiguous() &&
+                    k_offsets->numel() == d.size(0) + 1 && a.size(0) == 1 && b.size(0) == 1,
+                "tutel_b200.gemm: k_offsets must be a contiguous int32 [G + 1] with a [1, K, M], b [1, K, N] and d [G, M, N]");
+    p.k_offsets = k_offsets->data_ptr<int>();
+    p.G = static_cast<int>(d.size(0));
+  }
+}
+
 // a: [G, M, K] (a_mn=false) or [G, K, M] (a_mn=true); b: [Gb, N, K] (b_mn=false) or [Gb, K, N] (b_mn=true);
 // d: [G, M, N].  Innermost dims contiguous.  Pointer-table / flag arguments are raw device addresses (0 = off).
-void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn, bool b_mn, int64_t epilogue,
+// b_group_map / k_offsets: see set_packed_modes.
+void gemm_ex_packed(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn, bool b_mn, int64_t epilogue,
              const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
              const c10::optional<at::Tensor>& row_counts, double alpha, int64_t b_group_div, int64_t cta_group,
              int64_t block_n, int64_t d_ptr_table, int64_t signal_ptr_table, int64_t wait_flags,
              int64_t wait_rows_per_flag, int64_t wait_flags_per_group, int64_t wait_target, int64_t max_ctas,
              int64_t group_rot, int64_t group_mod, const c10::optional<at::Tensor>& scale_a,
              const c10::optional<at::Tensor>& scale_b, const c10::optional<at::Tensor>& colsum,
-             const c10::optional<at::Tensor>& d2, int64_t act) {
+             const c10::optional<at::Tensor>& d2, int64_t act, const c10::optional<at::Tensor>& b_group_map,
+             const c10::optional<at::Tensor>& k_offsets) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && d.is_cuda(), "tutel_b200.gemm: CUDA tensors required");
   TORCH_CHECK(a.dim() == 3 && b.dim() == 3 && d.dim() == 3, "tutel_b200.gemm: expected 3-D operands");
   TORCH_CHECK(a.stride(2) == 1 && b.stride(2) == 1 && d.stride(2) == 1, "tutel_b200.gemm: innermost dim must be contiguous");
@@ -65,9 +86,11 @@ void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn,
   p.K = static_cast<int>(a_mn ? a.size(1) : a.size(2));
   p.N = static_cast<int>(b_mn ? b.size(2) : b.size(1));
   TORCH_CHECK((b_mn ? b.size(1) : b.size(2)) == p.K, "tutel_b200.gemm: K mismatch");
+  set_packed_modes(p, a, b, d, b_group_map, k_offsets);
   TORCH_CHECK(d.size(0) == p.G && d.size(1) == p.M && d.size(2) == p.N, "tutel_b200.gemm: output shape mismatch");
   p.b_group_div = static_cast<int>(b_group_div > 0 ? b_group_div : 1);
-  TORCH_CHECK(b.size(0) * p.b_group_div >= p.G, "tutel_b200.gemm: not enough B groups");
+  TORCH_CHECK(p.b_group_map != nullptr || p.k_offsets != nullptr || b.size(0) * p.b_group_div >= p.G,
+              "tutel_b200.gemm: not enough B groups");
   p.a = a.data_ptr(); p.lda = a.stride(1); p.a_group_stride = a.stride(0); p.a_mn_major = a_mn;
   p.b = b.data_ptr(); p.ldb = b.stride(1); p.b_group_stride = b.stride(0); p.b_mn_major = b_mn;
   p.in_dtype = gemm_dtype_of(a);
@@ -76,8 +99,9 @@ void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn,
   TORCH_CHECK(p.out_dtype <= tb::DT_FP32, "tutel_b200.gemm: output must be bf16/fp16/fp32");
   p.epilogue = static_cast<int>(epilogue);
   p.alpha = static_cast<float>(alpha);
-  // groups of B (and rows of bias / scale_b / colsum) the kernel indexes: g / b_group_div for g < G
-  const int64_t gb = (p.G + p.b_group_div - 1) / p.b_group_div;
+  // groups of B (and rows of bias / scale_b / colsum) the kernel indexes: g / b_group_div for g < G (block-mapped B:
+  // the map's values, which are below b.size(0); ragged K: g)
+  const int64_t gb = p.b_group_map != nullptr ? b.size(0) : p.k_offsets != nullptr ? p.G : (p.G + p.b_group_div - 1) / p.b_group_div;
   // The epilogues read bias 16 bytes at a time (128 x 128) and scale_b 8 bytes at a time (128 x 256), from the row of
   // each B group: the base and the row stride must keep that alignment.
   auto aligned_rows = [](const at::Tensor& t, int64_t bytes) {
@@ -142,6 +166,19 @@ void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn,
   const char* why = nullptr;
   cudaError_t e = tb::gemm_sm90_launch(p, cur_stream(), &why);
   TORCH_CHECK(e == cudaSuccess, "tutel_b200.gemm launch failed: ", why ? why : cudaGetErrorString(e));
+}
+
+void gemm_ex(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn, bool b_mn, int64_t epilogue,
+             const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
+             const c10::optional<at::Tensor>& row_counts, double alpha, int64_t b_group_div, int64_t cta_group,
+             int64_t block_n, int64_t d_ptr_table, int64_t signal_ptr_table, int64_t wait_flags,
+             int64_t wait_rows_per_flag, int64_t wait_flags_per_group, int64_t wait_target, int64_t max_ctas,
+             int64_t group_rot, int64_t group_mod, const c10::optional<at::Tensor>& scale_a,
+             const c10::optional<at::Tensor>& scale_b, const c10::optional<at::Tensor>& colsum,
+             const c10::optional<at::Tensor>& d2, int64_t act) {
+  gemm_ex_packed(a, b, d, a_mn, b_mn, epilogue, bias, aux, row_counts, alpha, b_group_div, cta_group, block_n, d_ptr_table,
+                 signal_ptr_table, wait_flags, wait_rows_per_flag, wait_flags_per_group, wait_target, max_ctas, group_rot,
+                 group_mod, scale_a, scale_b, colsum, d2, act, c10::nullopt, c10::nullopt);
 }
 
 void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& d, bool a_mn, bool b_mn, int64_t epilogue,
@@ -252,14 +289,29 @@ std::vector<at::Tensor> encode_rows_fp8(const at::Tensor& x, const c10::optional
   return out;
 }
 
-// buf [E*C, M]; gates float [k, S] or None; idx/loc int [k, S]; returns [S, M]
-at::Tensor decode_rows(const at::Tensor& buf, const c10::optional<at::Tensor>& gates, const at::Tensor& idx,
-                       const at::Tensor& loc, int64_t E, int64_t C, int64_t wait_flags, int64_t wait_target) {
+// Expert-packed buffers: seg_off int [E + 1] (or at least [E]) of the packed layout; the buffer is [R, M] and C is
+// ignored (every location of a routed choice lies inside its expert's segment).
+const int* packed_seg_off(const c10::optional<at::Tensor>& seg_off, int64_t E) {
+  if (!seg_off.has_value() || !seg_off->defined()) return nullptr;
+  TORCH_CHECK(seg_off->is_cuda() && seg_off->scalar_type() == at::kInt && seg_off->is_contiguous() && seg_off->numel() >= E,
+              "tutel_b200: seg_off must be a contiguous int32 [E + 1]");
+  return seg_off->data_ptr<int>();
+}
+
+// buf [E*C, M] (seg_off: [R, M]); gates float [k, S] or None; idx/loc int [k, S]; returns [S, M]
+at::Tensor decode_rows_packed(const at::Tensor& buf, const c10::optional<at::Tensor>& gates, const at::Tensor& idx,
+                              const at::Tensor& loc, int64_t E, int64_t C, int64_t wait_flags, int64_t wait_target,
+                              const c10::optional<at::Tensor>& seg_off) {
   TORCH_CHECK(buf.is_cuda() && buf.is_contiguous() && idx.is_cuda() && loc.is_cuda());
   TORCH_CHECK(idx.scalar_type() == at::kInt && loc.scalar_type() == at::kInt && idx.is_contiguous() && loc.is_contiguous());
   const c10::cuda::CUDAGuard guard(buf.device());
   const int k = static_cast<int>(idx.size(0)), S = static_cast<int>(idx.size(1));
-  const int M = static_cast<int>(buf.numel() / (E * C));
+  const int* so = packed_seg_off(seg_off, E);
+  if (so != nullptr) {
+    TORCH_CHECK(buf.dim() == 2, "decode_rows: a packed buffer is [R, M]");
+    C = buf.size(0);
+  }
+  const int M = static_cast<int>(buf.numel() / (so != nullptr ? C : E * C));
   const void* g = nullptr;
   if (gates.has_value() && gates->defined()) {
     TORCH_CHECK(gates->is_cuda() && gates->scalar_type() == at::kFloat && gates->is_contiguous());
@@ -268,22 +320,57 @@ at::Tensor decode_rows(const at::Tensor& buf, const c10::optional<at::Tensor>& g
   at::Tensor out = at::empty({S, M}, buf.options());
   TB_CHECK_CUDA(tb::decode_rows(buf.data_ptr(), g, idx.data_ptr<int>(), loc.data_ptr<int>(), out.data_ptr(),
                                 reinterpret_cast<const uint32_t*>(wait_flags), static_cast<uint32_t>(wait_target), S,
-                                static_cast<int>(E), k, static_cast<int>(C), M, elem_type_of(buf), cur_stream()));
+                                static_cast<int>(E), k, static_cast<int>(C), M, elem_type_of(buf), cur_stream(), so));
   return out;
 }
 
-// a [S, M], buf [E*C, M] -> float [k, S]
-at::Tensor gate_grad(const at::Tensor& a, const at::Tensor& buf, const at::Tensor& idx, const at::Tensor& loc,
-                     int64_t E, int64_t C) {
+at::Tensor decode_rows(const at::Tensor& buf, const c10::optional<at::Tensor>& gates, const at::Tensor& idx,
+                       const at::Tensor& loc, int64_t E, int64_t C, int64_t wait_flags, int64_t wait_target) {
+  return decode_rows_packed(buf, gates, idx, loc, E, C, wait_flags, wait_target, c10::nullopt);
+}
+
+// a [S, M], buf [E*C, M] (seg_off: [R, M]) -> float [k, S]
+at::Tensor gate_grad_packed(const at::Tensor& a, const at::Tensor& buf, const at::Tensor& idx, const at::Tensor& loc,
+                            int64_t E, int64_t C, const c10::optional<at::Tensor>& seg_off) {
   TORCH_CHECK(a.is_cuda() && a.is_contiguous() && buf.is_cuda() && buf.is_contiguous());
   TORCH_CHECK(a.scalar_type() == buf.scalar_type());
   const c10::cuda::CUDAGuard guard(a.device());
   const int k = static_cast<int>(idx.size(0)), S = static_cast<int>(idx.size(1));
+  const int* so = packed_seg_off(seg_off, E);
+  if (so != nullptr) {
+    TORCH_CHECK(buf.dim() == 2 && buf.size(1) == a.size(1), "gate_grad: a packed buffer is [R, M]");
+    C = buf.size(0);
+  }
   at::Tensor out = at::empty({k, S}, a.options().dtype(at::kFloat));
   TB_CHECK_CUDA(tb::gate_grad(a.data_ptr(), buf.data_ptr(), idx.data_ptr<int>(), loc.data_ptr<int>(), out.data_ptr(),
                               S, static_cast<int>(E), k, static_cast<int>(C), static_cast<int>(a.size(1)),
-                              elem_type_of(a), cur_stream()));
+                              elem_type_of(a), cur_stream(), so));
   return out;
+}
+
+at::Tensor gate_grad(const at::Tensor& a, const at::Tensor& buf, const at::Tensor& idx, const at::Tensor& loc,
+                     int64_t E, int64_t C) {
+  return gate_grad_packed(a, buf, idx, loc, E, C, c10::nullopt);
+}
+
+// Expert-packed layout (see tb::packed_layout): idx / loc int [k, S], counts int [E], R rows ->
+// [seg_off [E + 1], block_expert [R / 128], block_rows [R / 128], slot_src [R]]
+std::vector<at::Tensor> packed_layout(const at::Tensor& idx, const at::Tensor& loc, const at::Tensor& counts, int64_t R) {
+  TORCH_CHECK(idx.is_cuda() && loc.is_cuda() && counts.is_cuda() && idx.scalar_type() == at::kInt &&
+              loc.scalar_type() == at::kInt && counts.scalar_type() == at::kInt && idx.is_contiguous() &&
+              loc.is_contiguous() && counts.is_contiguous() && idx.dim() == 2 && loc.sizes() == idx.sizes(),
+              "packed_layout: contiguous int32 CUDA idx / loc [k, S] and counts [E] expected");
+  TORCH_CHECK(R > 0 && R % 128 == 0, "packed_layout: R must be a positive multiple of 128");
+  const c10::cuda::CUDAGuard guard(idx.device());
+  const int64_t E = counts.numel();
+  auto opts = idx.options();
+  at::Tensor seg_off = at::empty({E + 1}, opts), block_expert = at::empty({R / 128}, opts),
+             block_rows = at::empty({R / 128}, opts), slot = at::empty({R}, opts);
+  TB_CHECK_CUDA(tb::packed_layout(idx.data_ptr<int>(), loc.data_ptr<int>(), counts.data_ptr<int>(), seg_off.data_ptr<int>(),
+                                  block_expert.data_ptr<int>(), block_rows.data_ptr<int>(), slot.data_ptr<int>(),
+                                  static_cast<int>(idx.size(1)), static_cast<int>(E), static_cast<int>(idx.size(0)),
+                                  static_cast<int>(R), cur_stream()));
+  return {seg_off, block_expert, block_rows, slot};
 }
 
 // logits [S, E] (fp32 / fp16 / bf16) -> [scores fp32 [S,E], idx int [k,S], top fp32 [k,S], gates fp32 [k,S], loc int [k,S],
@@ -428,6 +515,24 @@ void expert_bias_update(at::Tensor& bias, at::Tensor& load, double gamma) {
                                        static_cast<float>(gamma), cur_stream()));
 }
 
+// Segmented column sums: x [R, N] (rows contiguous), offsets int [G + 1] -> [G, N], row g = sum of rows
+// [offsets[g], offsets[g + 1]) in x's dtype (fp32 accumulation; no host read of the offsets).
+at::Tensor grouped_colsum_offsets(const at::Tensor& x, const at::Tensor& offsets) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.stride(1) == 1, "grouped_colsum: CUDA [R, N] tensor expected with offsets");
+  TORCH_CHECK(offsets.is_cuda() && offsets.scalar_type() == at::kInt && offsets.is_contiguous() && offsets.numel() >= 2,
+              "grouped_colsum: offsets must be a contiguous int32 [G + 1]");
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int G = static_cast<int>(offsets.numel() - 1), R = static_cast<int>(x.size(0)), N = static_cast<int>(x.size(1));
+  // the offsets are not known here: split as if one segment held every row (blocks of shorter segments finish early)
+  const int splits = tb::colsum_row_splits(1, R, N, static_cast<int>(x.element_size()));
+  at::Tensor acc = at::zeros({G, N}, x.options().dtype(at::kFloat));
+  at::Tensor out = at::empty({G, N}, x.options());
+  TB_CHECK_CUDA(tb::grouped_colsum(x.data_ptr(), x.stride(0), 0, out.data_ptr(), acc.data_ptr<float>(), G, R, N,
+                                   splits > 1 ? splits : 2, elem_type_of(x), cur_stream(), offsets.data_ptr<int>()));
+  out.copy_(acc);
+  return out;
+}
+
 // x [G, T, N] (last dim contiguous) -> [G, N] column sums in x's dtype (fp32 accumulation)
 at::Tensor grouped_colsum(const at::Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 3 && x.stride(2) == 1, "grouped_colsum: CUDA [G, T, N] tensor expected");
@@ -565,13 +670,14 @@ at::Tensor mx_gemm(const at::Tensor& a, const at::Tensor& sfa, const at::Tensor&
 // cuBLAS GEMMs plus separate activation and multiply kernels).
 //   forward  (b2 given):  h = act(a*b) .* (a*b2)   [+ g = a*b -> d2, u = a*b2 -> d3 when given]   ONE launch
 //   backward (aux given): acc = a*b (= dh);  d = dh .* u .* act'(g),  d2 = dh .* act(g)   with g = aux, u = aux2
-void gemm_glu(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::Tensor>& b2, at::Tensor& d,
+void gemm_glu_packed(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::Tensor>& b2, at::Tensor& d,
               const c10::optional<at::Tensor>& d2, const c10::optional<at::Tensor>& d3,
               const c10::optional<at::Tensor>& aux, const c10::optional<at::Tensor>& aux2, bool b_mn, int64_t act,
               const c10::optional<at::Tensor>& scale_a, const c10::optional<at::Tensor>& scale_b,
               const c10::optional<at::Tensor>& scale_b2, const c10::optional<at::Tensor>& row_counts,
               int64_t b_group_div, int64_t cta_group, int64_t wait_flags, int64_t wait_rows_per_flag,
-              int64_t wait_flags_per_group, int64_t wait_target, int64_t group_rot, int64_t group_mod) {
+              int64_t wait_flags_per_group, int64_t wait_target, int64_t group_rot, int64_t group_mod,
+              const c10::optional<at::Tensor>& b_group_map) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && d.is_cuda() && a.dim() == 3 && b.dim() == 3 && d.dim() == 3);
   TORCH_CHECK(a.stride(2) == 1 && b.stride(2) == 1 && d.stride(2) == 1 && a.scalar_type() == b.scalar_type());
   const c10::cuda::CUDAGuard guard(a.device());
@@ -583,7 +689,9 @@ void gemm_glu(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::
   p.N = static_cast<int>(b_mn ? b.size(2) : b.size(1));
   TORCH_CHECK((b_mn ? b.size(1) : b.size(2)) == p.K, "tutel_b200.gemm_glu: K mismatch");
   p.b_group_div = static_cast<int>(b_group_div > 0 ? b_group_div : 1);
-  TORCH_CHECK(b.size(0) * p.b_group_div >= p.G && d.size(0) == p.G && d.size(1) == p.M && d.size(2) == p.N && d.element_size() == 2);
+  set_packed_modes(p, a, b, d, b_group_map, c10::nullopt);
+  TORCH_CHECK((p.b_group_map != nullptr || b.size(0) * p.b_group_div >= p.G) && d.size(0) == p.G && d.size(1) == p.M &&
+              d.size(2) == p.N && d.element_size() == 2);
   p.cta_group = static_cast<int>(cta_group);
   p.wait_flags = reinterpret_cast<const uint32_t*>(wait_flags);
   p.wait_rows_per_flag = static_cast<int>(wait_rows_per_flag);
@@ -637,6 +745,17 @@ void gemm_glu(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::
   const char* why = nullptr;
   cudaError_t e = tb::gemm_sm90_launch(p, cur_stream(), &why);
   TORCH_CHECK(e == cudaSuccess, "tutel_b200.gemm_glu launch failed: ", why ? why : cudaGetErrorString(e));
+}
+
+void gemm_glu(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::Tensor>& b2, at::Tensor& d,
+              const c10::optional<at::Tensor>& d2, const c10::optional<at::Tensor>& d3,
+              const c10::optional<at::Tensor>& aux, const c10::optional<at::Tensor>& aux2, bool b_mn, int64_t act,
+              const c10::optional<at::Tensor>& scale_a, const c10::optional<at::Tensor>& scale_b,
+              const c10::optional<at::Tensor>& scale_b2, const c10::optional<at::Tensor>& row_counts,
+              int64_t b_group_div, int64_t cta_group, int64_t wait_flags, int64_t wait_rows_per_flag,
+              int64_t wait_flags_per_group, int64_t wait_target, int64_t group_rot, int64_t group_mod) {
+  gemm_glu_packed(a, b, b2, d, d2, d3, aux, aux2, b_mn, act, scale_a, scale_b, scale_b2, row_counts, b_group_div, cta_group,
+                  wait_flags, wait_rows_per_flag, wait_flags_per_group, wait_target, group_rot, group_mod, c10::nullopt);
 }
 
 at::Tensor skinny_gemm(const at::Tensor& x, const at::Tensor& w, const c10::optional<at::Tensor>& bias,
@@ -796,19 +915,25 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
             "P2P collectives, NVRTC JIT";
   m.def("gemm", &gemm);
   m.def("gemm_ex", &gemm_ex);
+  m.def("gemm_ex", &gemm_ex_packed);   // + b_group_map, k_offsets
   m.def("gemm_glu", &gemm_glu);
+  m.def("gemm_glu", &gemm_glu_packed); // + b_group_map
   m.def("route_locations", &route_locations);
   m.def("build_slot_map", &build_slot_map);
   m.def("encode_rows", &encode_rows);
   m.def("encode_rows_fp8", &encode_rows_fp8);
   m.def("decode_rows", &decode_rows);
+  m.def("decode_rows", &decode_rows_packed);
   m.def("gate_grad", &gate_grad);
+  m.def("gate_grad", &gate_grad_packed);
+  m.def("packed_layout", &packed_layout);
   m.def("gate_route_forward", &gate_route_forward);
   m.def("gate_route_backward", &gate_route_backward);
   m.def("sigmoid_gate_route_forward", &sigmoid_gate_route_forward);
   m.def("sigmoid_gate_route_backward", &sigmoid_gate_route_backward);
   m.def("expert_bias_update", &expert_bias_update);
   m.def("grouped_colsum", &grouped_colsum);
+  m.def("grouped_colsum", &grouped_colsum_offsets);
   m.def("cumsum_sub_one", &cumsum_sub_one);
   m.def("skinny_gemm", &skinny_gemm);
   m.def("skinny_ffn", &skinny_ffn);

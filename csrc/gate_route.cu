@@ -480,23 +480,29 @@ template <> struct V16<__nv_bfloat16> {
 
 // block = 256 threads = 16 row-lanes x 16 column-lanes; a block owns a strip of 16 * V columns of one group and the rows
 // [split * rows_per_split, ...).  Each thread keeps 4 independent 16-byte loads in flight.
-template <typename T>
+template <typename T, bool OFFS>
 __global__ void __launch_bounds__(256)
 colsum_kernel(const T* __restrict__ x, long long ld, long long group_stride, T* __restrict__ out, float* __restrict__ acc_out,
-              int rows, int N, int rows_per_split) {
+              int rows, int N, int rows_per_split, const int* __restrict__ offsets) {
   constexpr int V = V16<T>::N;
   __shared__ float sm[16][16 * V + 1];
   const int cl = threadIdx.x & 15;
   const int rl = threadIdx.x >> 4;
   const int col = (blockIdx.x * 16 + cl) * V;
   const int g = blockIdx.z;
-  const int r_begin = blockIdx.y * rows_per_split;
-  const int r_end = min(rows, r_begin + rows_per_split);
+  int r_lo = 0, r_hi = rows;
+  if (OFFS) {   // segment g of one [rows, N] tensor, split evenly over the blocks of its strip
+    r_lo = offsets[g];
+    r_hi = min(rows, offsets[g + 1]);
+    rows_per_split = (max(r_hi - r_lo, 0) + static_cast<int>(gridDim.y) - 1) / static_cast<int>(gridDim.y);
+  }
+  const int r_begin = r_lo + blockIdx.y * rows_per_split;
+  const int r_end = min(r_hi, r_begin + rows_per_split);
   float a[V];
 #pragma unroll
   for (int i = 0; i < V; ++i) a[i] = 0.0f;
   if (col < N) {
-    const T* base = x + static_cast<long long>(g) * group_stride + col;
+    const T* base = x + (OFFS ? 0LL : static_cast<long long>(g) * group_stride) + col;
     int r = r_begin + rl;
     for (; r + 48 < r_end; r += 64) {
       uint4 u[4];
@@ -711,17 +717,22 @@ int colsum_row_splits(int G, int rows, int N, int elem_bytes) {
 
 template <typename T>
 static cudaError_t colsum_t(const void* x, long long ld, long long group_stride, void* out, float* acc, int G, int rows,
-                            int N, int splits, cudaStream_t stream) {
+                            int N, int splits, const int* offsets, cudaStream_t stream) {
   constexpr int V = V16<T>::N;
   const int strips = (N + 16 * V - 1) / (16 * V);
   const int rps = (rows + splits - 1) / splits;
   dim3 grid(strips, splits, G);
-  colsum_kernel<T><<<grid, 256, 0, stream>>>(static_cast<const T*>(x), ld, group_stride, static_cast<T*>(out), acc, rows, N, rps);
+  if (offsets != nullptr)
+    colsum_kernel<T, true><<<grid, 256, 0, stream>>>(static_cast<const T*>(x), ld, group_stride, static_cast<T*>(out), acc, rows,
+                                                     N, rps, offsets);
+  else
+    colsum_kernel<T, false><<<grid, 256, 0, stream>>>(static_cast<const T*>(x), ld, group_stride, static_cast<T*>(out), acc, rows,
+                                                      N, rps, offsets);
   return cudaGetLastError();
 }
 
 cudaError_t grouped_colsum(const void* x, long long ld, long long group_stride, void* out, float* acc, int G, int rows,
-                           int N, int splits, int elem_type, cudaStream_t stream) {
+                           int N, int splits, int elem_type, cudaStream_t stream, const int* offsets) {
   if (G <= 0 || rows <= 0 || N <= 0) return cudaSuccess;
   const int eb = elem_type == ET_F32 ? 4 : 2;
   if ((reinterpret_cast<uintptr_t>(x) & 15) || ((ld * eb) & 15) || ((group_stride * eb) & 15) || (N * eb) % 16)
@@ -729,9 +740,9 @@ cudaError_t grouped_colsum(const void* x, long long ld, long long group_stride, 
   if (splits > 1 && acc == nullptr) return cudaErrorInvalidValue;
   if (splits <= 1) acc = nullptr;
   switch (elem_type) {
-    case ET_F32: return colsum_t<float>(x, ld, group_stride, out, acc, G, rows, N, splits, stream);
-    case ET_F16: return colsum_t<__half>(x, ld, group_stride, out, acc, G, rows, N, splits, stream);
-    case ET_BF16: return colsum_t<__nv_bfloat16>(x, ld, group_stride, out, acc, G, rows, N, splits, stream);
+    case ET_F32: return colsum_t<float>(x, ld, group_stride, out, acc, G, rows, N, splits, offsets, stream);
+    case ET_F16: return colsum_t<__half>(x, ld, group_stride, out, acc, G, rows, N, splits, offsets, stream);
+    case ET_BF16: return colsum_t<__nv_bfloat16>(x, ld, group_stride, out, acc, G, rows, N, splits, offsets, stream);
   }
   return cudaErrorInvalidValue;
 }

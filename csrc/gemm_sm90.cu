@@ -82,6 +82,12 @@ struct GemmArgs {
   uint32_t wait_target;
   const unsigned long long* signal_ptr_table;
   int group_rot, group_mod;  // tile order visits group (g/mod)*mod + (g%mod + rot)%mod  (own-rank segment first)
+  // Block-mapped B (packed expert layout): group g is one M tile whose B group (and bias / scale_b / colsum row) is
+  // b_group_map[g]; rows of a tile past row_counts[g] are stored as zeros.  Tiles are banded across groups.
+  const int* b_group_map;
+  // Ragged K (weight gradients on the packed layout): A and B are single [K_total, *] tensors and group g reduces the
+  // K range [k_offsets[g], k_offsets[g + 1]) (multiples of the 64-element K block).
+  const int* k_offsets;
 };
 
 namespace {
@@ -169,6 +175,49 @@ __device__ __forceinline__ int rotate_group(int g, int rot, int mod) {
     return base + (rot + m - (g - base)) % m;
   }
   return g;
+}
+
+// The packed-layout launch modes (b_group_map, k_offsets) run in their own instantiations of the kernel (PK = true), so
+// that every other launch compiles to code with none of their per-tile loads and branches.
+//
+// Tile t of a launch: group-major bands of row blocks (rotated groups for the fused engine), or - block-mapped B - one
+// band sequence over all groups, which are single row blocks, so that a wave reuses B columns across neighbouring blocks.
+template <int kBand, bool PK>
+__device__ __forceinline__ TileCoord tile_of(long long t, const GemmArgs& args) {
+  TileCoord tc;
+  if (PK && args.b_group_map != nullptr) {
+    tc = decode_tile<kBand>(t, args.G, args.tiles_n);
+    tc.g = tc.m_blk;
+    tc.m_blk = 0;
+  } else {
+    tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
+    tc.g = rotate_group(tc.g, args.group_rot, args.group_mod);
+  }
+  return tc;
+}
+
+// B group of A group g, which is also the row of bias, scale_b and colsum.
+template <bool PK>
+__device__ __forceinline__ int b_group_of(int g, const GemmArgs& args) {
+  return (PK && args.b_group_map != nullptr) ? args.b_group_map[g] : g / args.b_group_div;
+}
+
+// 64-deep K blocks of group g and the first K element: uniform, or the group's range of k_offsets.
+template <bool PK>
+__device__ __forceinline__ int2 k_range_of(int g, int num_kb, int bk_elems, const GemmArgs& args) {
+  if (!PK || args.k_offsets == nullptr) return make_int2(num_kb, 0);
+  const int k0 = args.k_offsets[g];
+  const int len = args.k_offsets[g + 1] - k0;
+  return make_int2(len > 0 ? (len + bk_elems - 1) / bk_elems : 0, k0);
+}
+
+// Block-mapped B: rows at or past the count are stored as zeros (r0 / r0 + 8 of wide_main's fragment layout).
+__device__ __forceinline__ void wide_zero_rows(float (&acc)[128], bool ok0, bool ok1) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    if (!ok0) { acc[4 * j] = 0.0f; acc[4 * j + 1] = 0.0f; }
+    if (!ok1) { acc[4 * j + 2] = 0.0f; acc[4 * j + 3] = 0.0f; }
+  }
 }
 
 // Per-element epilogue formulas.  Both configurations call these, so that they produce the same bits per element.
@@ -433,7 +482,7 @@ __device__ __forceinline__ void hand_over_tile(const uint8_t* tile, bool straddl
 // shared memory) always fits next to a GEMM CTA.  That is what makes the dispatch+GEMM fusion deadlock-free: a GEMM
 // whose producer spins on arrival flags can never starve the kernel that publishes them, whichever gets the SMs first.
 // (This is the BN = 128 configuration; the BN = 256 one takes the whole SM and is never used by the fused engine.)
-template <int BN_, bool A_MN, bool B_MN, int DT>
+template <int BN_, bool A_MN, bool B_MN, int DT, bool PK>
 __global__ void __maxnreg__(Cfg<BN_>::MAXNREG)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmB2, const __grid_constant__ CUtensorMap tmD,
@@ -475,6 +524,9 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const bool side_in = side_bias || (C::WIDE && args.scale_b != nullptr);
   // BIAS_GELU / BIAS_SILU with a pre-activation output: every tile goes through the output tile twice (d2, then d)
   const bool pre_act = C::WIDE && args.d2 != nullptr && (args.epilogue == EPI_BIAS_GELU || args.epilogue == EPI_BIAS_SILU);
+  // block-mapped B: every row of a computed tile is stored, rows past the count as zeros
+  const bool zero_pad = PK && args.b_group_map != nullptr;
+  const bool ragged_k = PK && args.k_offsets != nullptr;
 
   if (warp == 0 && ptx::elect_one()) {
     ptx::prefetch_tensormap(&tmA);
@@ -519,12 +571,14 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       int seen_group = -1;
       unsigned long long seen_mask = 0ull;
       for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
-        TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
-        tc.g = rotate_group(tc.g, args.group_rot, args.group_mod);
+        const TileCoord tc = tile_of<kBand, PK>(t, args);
         if (args.row_counts != nullptr && tc.m_blk * C::BM >= args.row_counts[tc.g]) continue;
         const int m0 = tc.m_blk * C::BM;
         const int n0 = tc.n_blk * BN;   // (non-dual) first B column of this tile
-        const int gb = tc.g / args.b_group_div;
+        // ragged K: A and B are single tensors, walked from the group's first K row
+        const int2 kr = k_range_of<PK>(tc.g, num_kb, bk_elems, args);
+        const int ga = ragged_k ? 0 : tc.g;
+        const int gb = ragged_k ? 0 : b_group_of<PK>(tc.g, args);
         if (args.wait_flags != nullptr) {
           // Dispatch fusion: rows of this tile are pushed by peer GPUs; acquire their release flags - once per
           // (group, flag): consecutive tiles of a group share flags, so remember which ones were already seen.
@@ -545,20 +599,20 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             seen_mask |= need;
           }
         }
-        for (int kb = 0; kb < num_kb; ++kb) {
+        for (int kb = 0; kb < kr.x; ++kb) {
           ptx::mbar_wait_quiet(empty_bar(s), ph ^ 1u);
           if (ptx::elect_one()) {
             const uint32_t fb = full_bar(s);
             ptx::mbar_expect_tx(fb, C::STAGE_BYTES);
-            const int k0 = kb * bk_elems;
+            const int k0 = kr.y + kb * bk_elems;
             constexpr int chunk_elems = kSwizzleBytes / kEltBytes;    // MN-major: one 128-byte chunk of the MN axis ...
             constexpr int chunk_bytes = bk_elems * kSwizzleBytes;     // ... times the stage's K rows
             // ---- A ----
             if constexpr (!A_MN) {
-              ptx::tma_load_3d(smem_a(s), &tmA, fb, k0, m0, tc.g);
+              ptx::tma_load_3d(smem_a(s), &tmA, fb, k0, m0, ga);
             } else {
               for (int c = 0; c < C::BM / chunk_elems; ++c)
-                ptx::tma_load_3d(smem_a(s) + c * chunk_bytes, &tmA, fb, m0 + c * chunk_elems, k0, tc.g);
+                ptx::tma_load_3d(smem_a(s) + c * chunk_bytes, &tmA, fb, m0 + c * chunk_elems, k0, ga);
             }
             // ---- B ----
             if (!dual) {
@@ -602,7 +656,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       // has_next).
       auto drain = [&](const CUtensorMap* map, const TileCoord& tc, int m_valid, bool colsum, bool has_next, TileCoord next) {
         const int m0 = tc.m_blk * C::BM, n0 = tc.n_blk * BN;
-        const bool straddle = m0 + C::BM > m_valid && m_valid < args.M;   // the consumers copied it out row-guarded
+        const bool straddle = zero_pad ? false : m0 + C::BM > m_valid && m_valid < args.M;   // the consumers copied it out row-guarded
         ptx::mbar_wait_quiet(out_full, outs & 1u);
         if (!straddle && lane == 0) {
           for (int b = 0; b < BN / 64; ++b)
@@ -622,7 +676,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
             const int n = n0 + c;
             if (n < args.N) {   // N is a multiple of 8: all four columns are in range
-              float* cs = args.colsum + static_cast<long long>(tc.g / args.b_group_div) * args.colsum_group_stride + n;
+              float* cs = args.colsum + static_cast<long long>(b_group_of<PK>(tc.g, args)) * args.colsum_group_stride + n;
               if ((reinterpret_cast<uintptr_t>(cs) & 15) == 0) {
                 ptx::red_add_v4_f32(cs, v.x, v.y, v.z, v.w);
               } else {
@@ -647,8 +701,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         ++outs;
       };
       for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
-        TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
-        tc.g = rotate_group(tc.g, args.group_rot, args.group_mod);
+        const TileCoord tc = tile_of<kBand, PK>(t, args);
         int m_valid = args.M;
         if (args.row_counts != nullptr) {
           m_valid = min(args.M, args.row_counts[tc.g]);
@@ -660,7 +713,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           // tile it - 1 has completed; with pre_act its first hand-over is enough)
           if (it > 0 && !pre_act) ptx::mbar_wait_quiet(out_full, outs & 1u);
           const int n0 = tc.n_blk * BN;
-          const int gb = tc.g / args.b_group_div;
+          const int gb = b_group_of<PK>(tc.g, args);
           const int cols = min(BN, args.N - n0);
           const uint32_t slot = side_base + (it & 1u) * C::SIDE_SLOT_BYTES;
           // (16-byte aligned: see gemm_sm90_launch)
@@ -743,23 +796,25 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint32_t outs = 0;   // 128 x 256: output tiles handed to the store warp
 
     for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
-      TileCoord tc = decode_tile<kBand>(t, args.tiles_m, args.tiles_n);
-      tc.g = rotate_group(tc.g, args.group_rot, args.group_mod);
+      const TileCoord tc = tile_of<kBand, PK>(t, args);
       int m_valid = args.M;
       if (args.row_counts != nullptr) {
         m_valid = min(args.M, args.row_counts[tc.g]);
         if (tc.m_blk * C::BM >= m_valid) continue;
       }
+      const int tile_kb = ragged_k ? k_range_of<PK>(tc.g, num_kb, bk_elems, args).x : num_kb;
       // ------------------------------- main loop -------------------------------
       float acc[BN / 2];
-      if constexpr (C::WIDE) {
+      // (packed launches zero it too: an empty K range of a ragged-K tile runs no wgmma at all.  A definition that depends
+      // on the tile, or a wgmma wait on a divergent path, would make ptxas serialise every wgmma of the main loop.)
+      if (C::WIDE || PK) {
         // The first wgmma of a tile ignores the accumulator, but its register operands are read-write: without a fresh
         // definition the previous tile's 128 values would stay live through the whole epilogue.
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
       }
       int prev_s = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
+      for (int kb = 0; kb < tile_kb; ++kb) {
         ptx::mbar_wait_quiet(full_bar(s), ph);
         const uint32_t a_lo = a_lo0 + static_cast<uint32_t>(s) * (C::STAGE_BYTES >> 4);
         const uint32_t b_lo = b_lo0 + static_cast<uint32_t>(s) * (C::STAGE_BYTES >> 4);
@@ -780,17 +835,20 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (++s == stages) { s = 0; ph ^= 1u; }
       }
       ptx::wgmma_wait<0>();
-      if (wg_leader) ptx::mbar_arrive(empty_bar(prev_s));
+      // (ragged K: an empty K range leaves the zeroed accumulator and consumes no stage)
+      if (wg_leader && (!PK || tile_kb > 0)) ptx::mbar_arrive(empty_bar(prev_s));
 
       if constexpr (C::WIDE) {
         // ------------------------- 128 x 256 epilogue -------------------------
         const int m0 = tc.m_blk * C::BM, n0 = tc.n_blk * BN;
         const bool ok0 = m0 + r0 < m_valid, ok1 = m0 + r0 + 8 < m_valid;
+        // block-mapped B stores rows past the count as zeros (branch-free: see the accumulator's definition above)
+        const bool keep0 = !zero_pad || ok0, keep1 = !zero_pad || ok1;
         const int n_lane = 2 * (lane & 3);   // column in the tile
         const int n_lim = args.N - n0;
         // a row block that straddles the group's row count (at most one per group) must not write past the count,
         // which the output tensor map cannot express: it is copied out with row-guarded stores instead
-        const bool straddle = m0 + C::BM > m_valid && m_valid < args.M;
+        const bool straddle = zero_pad ? false : m0 + C::BM > m_valid && m_valid < args.M;
         // this tile's bias / column scales have landed in its side-input slot
         const uint8_t* side = reinterpret_cast<const uint8_t*>(colsum_part + 8 * BN) + (it & 1u) * C::SIDE_SLOT_BYTES;
         if (side_in) ptx::mbar_wait_quiet(side_full(it & 1u), (it >> 1) & 1u);
@@ -814,6 +872,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (pre_act) {
             // training: the backward pass needs the pre-activation (ReLU gets by with the sign of its output)
             wait_out_free();
+            if constexpr (PK) wide_zero_rows(acc, keep0, keep1);
             wide_stage(acc, row0, swz, out_bf16);
             hand_over(reinterpret_cast<uint8_t*>(args.d2));
           }
@@ -830,6 +889,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           else wide_main<WM_SILU_BWD>(acc, row0, swz, nullptr, false, false, n_lane, n_lim, out_bf16, 1.0f);
         }
         if (!aux_tma) wait_out_free();
+        if constexpr (PK) wide_zero_rows(acc, keep0, keep1);
         wide_stage(acc, row0, swz, out_bf16);     // aux epilogues: each word overwrites the aux word it was computed from
         // the partial rows are free: the store warp read them before it released the output tile
         if (args.colsum != nullptr) wide_colsum(acc, ok0, ok1, lane, colsum_part + cw * BN);
@@ -851,7 +911,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
       const int m = tc.m_blk * C::BM + cw * 16 + (lane & 15);
       const bool row_ok = m < m_valid;
-      const int gb = tc.g / args.b_group_div;
+      const int gb = b_group_of<PK>(tc.g, args);
       uint8_t* d_base = (args.d_ptr_table != nullptr)
                             ? reinterpret_cast<uint8_t*>(args.d_ptr_table[tc.g])
                             : reinterpret_cast<uint8_t*>(args.d) +
@@ -872,11 +932,16 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
       // One 32-column segment of this lane's row -> global memory (local or a peer's): 64 contiguous bytes in 16 bit.
       // ncols (a multiple of 8) may be <= 0 for segments past the last column: nothing is touched then.
+      // Block-mapped B stores rows past the count as zeros.
       auto store_seg = [&](uint8_t* row, int n, int ncols, const float* v) {
-        if (!row_ok) return;
+        if (!row_ok && !(zero_pad && m < args.M)) return;
         if (out16) {
           uint32_t w[16];
           pack32(v, w, out_bf16);
+          if (zero_pad && !row_ok) {
+#pragma unroll
+            for (int q = 0; q < 16; ++q) w[q] = 0u;
+          }
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             if (q * 8 < ncols) {
@@ -887,7 +952,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             if (q * 4 < ncols) {
-              float4 o = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
+              float4 o = (!zero_pad || row_ok) ? make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
               *reinterpret_cast<float4*>(row + (n + q * 4) * 4) = o;
             }
           }
@@ -1150,11 +1215,11 @@ bool make_tile_map(CUtensorMap* map, const void* base, int dtype, long long rows
   return true;
 }
 
-template <int BN, bool A_MN, bool B_MN, int DT>
+template <int BN, bool A_MN, bool B_MN, int DT, bool PK = false>
 cudaError_t launch_inst(const CUtensorMap& ta, const CUtensorMap& tb_, const CUtensorMap& tb2, const CUtensorMap& td,
                         const CUtensorMap& taux, const CUtensorMap& td2, const GemmArgs& args, int grid,
                         cudaStream_t stream) {
-  auto* kern = gemm_sm90_kernel<BN, A_MN, B_MN, DT>;
+  auto* kern = gemm_sm90_kernel<BN, A_MN, B_MN, DT, PK>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES);
@@ -1203,8 +1268,10 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
   }
   // A zero group stride (an expanded tensor) would be taken for "one group" by the tensor maps, so group g would start g
   // rows into the matrix instead of at it: such operands must be materialised by the caller.
-  const int groups_b = (p.G + (p.b_group_div > 0 ? p.b_group_div : 1) - 1) / (p.b_group_div > 0 ? p.b_group_div : 1);
-  if ((p.G > 1 && (p.a_group_stride == 0 || (p.d_ptr_table == nullptr && p.d_group_stride == 0) ||
+  // (block-mapped B: as many B groups as the map names, known to the caller only; ragged K: one A and one B group)
+  const int groups_b = p.k_offsets != nullptr ? 1 : p.b_group_map != nullptr ? p.b_groups :
+                       (p.G + (p.b_group_div > 0 ? p.b_group_div : 1) - 1) / (p.b_group_div > 0 ? p.b_group_div : 1);
+  if ((p.G > 1 && ((p.k_offsets == nullptr && p.a_group_stride == 0) || (p.d_ptr_table == nullptr && p.d_group_stride == 0) ||
                    (uses_aux && p.aux_group_stride == 0))) ||
       (groups_b > 1 && p.b_group_stride == 0)) {
     *why = "group strides of A, B, aux and the output must be nonzero when there is more than one group";
@@ -1219,6 +1286,17 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
   if (p.alpha != 1.0f && p.epilogue != EPI_NONE) { *why = "alpha is applied by EPI_NONE only"; return cudaErrorInvalidValue; }
   if (p.cta_group < 0 || p.cta_group > 2) { *why = "cta_group must be 0, 1 or 2"; return cudaErrorInvalidValue; }
   if (p.block_n != 0 && p.block_n != 128 && p.block_n != 256) { *why = "block_n must be 0, 128 or 256"; return cudaErrorInvalidValue; }
+  const bool fused_engine = p.wait_flags != nullptr || p.signal_ptr_table != nullptr || p.d_ptr_table != nullptr;
+  if (p.b_group_map != nullptr && (eb != 2 || p.k_offsets != nullptr || p.M > 128 || fused_engine || p.group_mod != 1)) {
+    *why = "b_group_map needs 16-bit operands and groups of at most 128 rows, and excludes k_offsets, group rotation and the "
+           "fused engine";
+    return cudaErrorInvalidValue;
+  }
+  if (p.k_offsets != nullptr && (eb != 2 || p.b_group_div != 1 || p.scale_a != nullptr || p.scale_b != nullptr ||
+                                 fused_engine || p.group_mod != 1)) {
+    *why = "k_offsets needs 16-bit operands and excludes b_group_div, scales, group rotation and the fused engine";
+    return cudaErrorInvalidValue;
+  }
 
   // 128 x 256 tiles unless the caller is the fused multi-GPU engine (flags, peer stores and per-128 x 128-tile
   // completion signals are built around the 128 x 128 configuration) or pins that configuration with block_n == 128.
@@ -1254,10 +1332,12 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
   a.wait_flags_per_group = p.wait_flags_per_group; a.wait_target = p.wait_target;
   a.signal_ptr_table = p.signal_ptr_table;
   a.group_rot = p.group_rot; a.group_mod = p.group_mod;
+  a.b_group_map = p.b_group_map; a.k_offsets = p.k_offsets;
 
   CUtensorMap ta, tb_;
-  const int gB = (p.G + a.b_group_div - 1) / a.b_group_div;
-  if (!make_operand_map(&ta, p.a, p.in_dtype, p.a_mn_major, p.M, p.K, p.lda, p.a_group_stride, p.G, bm, why))
+  const int gB = groups_b;
+  const int gA = p.k_offsets != nullptr ? 1 : p.G;
+  if (!make_operand_map(&ta, p.a, p.in_dtype, p.a_mn_major, p.M, p.K, p.lda, p.a_group_stride, gA, bm, why))
     return cudaErrorInvalidValue;
   const int b_box = dual ? bn / 2 : bn;
   if (!make_operand_map(&tb_, p.b, p.in_dtype, p.b_mn_major, p.N, p.K, p.ldb, p.b_group_stride, gB, b_box, why))
@@ -1289,15 +1369,19 @@ cudaError_t gemm_sm90_launch(const GemmProblem& p, cudaStream_t stream, const ch
     if (p.in_dtype == DT_E4M3) return launch_inst<128, false, false, DT_E4M3>(ta, tb_, tb2, td, taux, td2, a, grid, stream);
     return launch_inst<128, false, false, DT_E5M2>(ta, tb_, tb2, td, taux, td2, a, grid, stream);
   }
-#define TB_SWITCH_MAJOR(BNv, DTv)                                                                                  \
-  do {                                                                                                             \
-    if (!p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, false, false, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);   \
-    if (!p.a_mn_major && p.b_mn_major) return launch_inst<BNv, false, true, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);     \
-    if (p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, true, false, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);     \
-    return launch_inst<BNv, true, true, DTv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);                                        \
+#define TB_SWITCH_MAJOR(BNv, DTv, PKv)                                                                                         \
+  do {                                                                                                                         \
+    if (!p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, false, false, DTv, PKv>(ta, tb_, tb2, td, taux, td2, a, grid, stream); \
+    if (!p.a_mn_major && p.b_mn_major) return launch_inst<BNv, false, true, DTv, PKv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);   \
+    if (p.a_mn_major && !p.b_mn_major) return launch_inst<BNv, true, false, DTv, PKv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);   \
+    return launch_inst<BNv, true, true, DTv, PKv>(ta, tb_, tb2, td, taux, td2, a, grid, stream);                                      \
   } while (0)
-  if (p.in_dtype == DT_BF16) { if (wide) TB_SWITCH_MAJOR(256, DT_BF16); TB_SWITCH_MAJOR(128, DT_BF16); }
-  if (p.in_dtype == DT_FP16) { if (wide) TB_SWITCH_MAJOR(256, DT_FP16); TB_SWITCH_MAJOR(128, DT_FP16); }
+  if (p.b_group_map != nullptr || p.k_offsets != nullptr) {
+    if (p.in_dtype == DT_BF16) { if (wide) TB_SWITCH_MAJOR(256, DT_BF16, true); TB_SWITCH_MAJOR(128, DT_BF16, true); }
+    if (p.in_dtype == DT_FP16) { if (wide) TB_SWITCH_MAJOR(256, DT_FP16, true); TB_SWITCH_MAJOR(128, DT_FP16, true); }
+  }
+  if (p.in_dtype == DT_BF16) { if (wide) TB_SWITCH_MAJOR(256, DT_BF16, false); TB_SWITCH_MAJOR(128, DT_BF16, false); }
+  if (p.in_dtype == DT_FP16) { if (wide) TB_SWITCH_MAJOR(256, DT_FP16, false); TB_SWITCH_MAJOR(128, DT_FP16, false); }
 #undef TB_SWITCH_MAJOR
   *why = "unsupported operand dtype";
   return cudaErrorInvalidValue;

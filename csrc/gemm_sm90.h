@@ -91,6 +91,17 @@ struct GemmProblem {
   // rows it produced itself while the peers' rows are still in flight.
   int group_rot = 0, group_mod = 1;
 
+  // Optional block-mapped B (device int32[G]): the B group of A group g - and the row of bias, scale_b and colsum - is
+  // b_group_map[g] instead of g / b_group_div, for b_groups B groups (16-bit operands).  Groups are single M tiles (M <= 128), e.g. the
+  // 128-row blocks of an expert-packed token buffer; with row_counts, rows of a block at or past its count are STORED AS
+  // ZEROS (not left untouched), and blocks with a count of 0 are skipped.
+  const int* b_group_map = nullptr;
+  int b_groups = 1;
+  // Optional ragged K (device int32[G + 1], multiples of 64): A and B are single tensors with K = total rows, and group g
+  // reduces K rows [k_offsets[g], k_offsets[g + 1]) - the weight gradients of an expert-packed buffer.  An empty range
+  // stores a zero tile.  16-bit operands only.
+  const int* k_offsets = nullptr;
+
   // Tile shape.  The launcher runs 128 x 256 tiles, except for the fused multi-GPU engine (wait_flags, signal_ptr_table
   // or d_ptr_table set: its flags, peer stores and per-tile completion counts assume 128 x 128 tiles and a GEMM CTA
   // that leaves room for one dispatch block per SM), the GLU epilogues and fp32 outputs, which run 128 x 128 tiles.

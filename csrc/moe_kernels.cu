@@ -116,6 +116,67 @@ __global__ void slot_map_kernel(const int* __restrict__ idx, const int* __restri
 }
 
 // ------------------------------------------------------------------------------------------------
+// expert-packed layout: expert e's rows are [seg_off[e], seg_off[e] + counts[e]), segments start on 128-row blocks
+// ------------------------------------------------------------------------------------------------
+constexpr int kPackBlock = 128;
+
+// One block of 1024 threads: warp 0 scans the rounded counts 32 experts at a time, then every thread describes blocks.
+__global__ void __launch_bounds__(1024)
+packed_layout_kernel(const int* __restrict__ counts, int* __restrict__ seg_off, int* __restrict__ block_expert,
+                     int* __restrict__ block_rows, int E, int nblocks) {
+  extern __shared__ int sh_off[];   // [E + 1]
+  if (threadIdx.x < 32) {
+    int carry = 0;
+    for (int e0 = 0; e0 < E; e0 += 32) {
+      const int e = e0 + static_cast<int>(threadIdx.x);
+      const int c = e < E ? max(counts[e], 0) : 0;
+      const int v = (c + kPackBlock - 1) / kPackBlock * kPackBlock;
+      int incl = v;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (static_cast<int>(threadIdx.x) >= o) incl += t;
+      }
+      if (e < E) sh_off[e] = carry + incl - v;
+      carry += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    if (threadIdx.x == 0) sh_off[E] = carry;
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e <= E; e += blockDim.x) seg_off[e] = sh_off[e];
+  const int total = sh_off[E];
+  for (int b = threadIdx.x; b < nblocks; b += blockDim.x) {
+    const int r0 = b * kPackBlock;
+    int e = 0, rows = 0;
+    if (r0 < total) {
+      int lo = 0, hi = E - 1;       // the last e with sh_off[e] <= r0 (empty experts share their successor's offset)
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (sh_off[mid] <= r0) lo = mid; else hi = mid - 1;
+      }
+      e = lo;
+      rows = min(kPackBlock, sh_off[e] + max(counts[e], 0) - r0);
+    }
+    block_expert[b] = e;
+    block_rows[b] = rows;
+  }
+}
+
+__global__ void packed_slot_kernel(const int* __restrict__ idx, const int* __restrict__ loc, const int* __restrict__ seg_off,
+                                   int* __restrict__ slot_src, int S, int E, int k, int R) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(S) * k) return;
+  const int j = static_cast<int>(i / S);
+  const int s = static_cast<int>(i - static_cast<long long>(j) * S);
+  const int e = idx[i];
+  const int l = loc[i];
+  if (e >= 0 && e < E && l >= 0) {
+    const int r = seg_off[e] + l;
+    if (r < R) slot_src[r] = s * k + j;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // 16-byte vector helpers
 // ------------------------------------------------------------------------------------------------
 template <typename T>
@@ -299,11 +360,11 @@ encode_rows_kernel(const T* __restrict__ x, const float* __restrict__ gates, con
 // ------------------------------------------------------------------------------------------------
 constexpr int kMaxK = 16;
 
-template <typename T, bool VEC>
+template <typename T, bool VEC, bool SEG>
 __global__ void __launch_bounds__(256)
 decode_rows_kernel(const T* __restrict__ buf, const float* __restrict__ gates, const int* __restrict__ idx,
                    const int* __restrict__ loc, T* __restrict__ out, const uint32_t* __restrict__ wait_flags,
-                   uint32_t wait_target, int S, int E, int k, int C, int M) {
+                   uint32_t wait_target, int S, int E, int k, int C, int M, const int* __restrict__ seg_off) {
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   for (long long s = static_cast<long long>(blockIdx.x) * 8 + warp; s < S; s += static_cast<long long>(gridDim.x) * 8) {
@@ -318,7 +379,7 @@ decode_rows_kernel(const T* __restrict__ buf, const float* __restrict__ gates, c
           if (lane == 0) ptx::wait_flag_ge_sys(wait_flags + e, wait_target);
           __syncwarp();
         }
-        rows[nsel] = buf + (static_cast<long long>(e) * C + l) * M;
+        rows[nsel] = buf + ((SEG ? static_cast<long long>(seg_off[e]) : static_cast<long long>(e) * C) + l) * M;
         w[nsel] = gates != nullptr ? gates[static_cast<long long>(j) * S + s] : 1.0f;
         ++nsel;
       }
@@ -361,10 +422,11 @@ decode_rows_kernel(const T* __restrict__ buf, const float* __restrict__ gates, c
   }
 }
 
-template <typename T, bool VEC>
+template <typename T, bool VEC, bool SEG>
 __global__ void __launch_bounds__(256)
 gate_grad_kernel(const T* __restrict__ a, const T* __restrict__ buf, const int* __restrict__ idx,
-                 const int* __restrict__ loc, float* __restrict__ dgate, int S, int E, int k, int C, int M) {
+                 const int* __restrict__ loc, float* __restrict__ dgate, int S, int E, int k, int C, int M,
+                 const int* __restrict__ seg_off) {
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   for (long long s = static_cast<long long>(blockIdx.x) * 8 + warp; s < S; s += static_cast<long long>(gridDim.x) * 8) {
@@ -374,7 +436,7 @@ gate_grad_kernel(const T* __restrict__ a, const T* __restrict__ buf, const int* 
       const int l = loc[static_cast<long long>(j) * S + s];
       float acc = 0.0f;
       if (e >= 0 && e < E && l >= 0 && l < C) {
-        const T* brow = buf + (static_cast<long long>(e) * C + l) * M;
+        const T* brow = buf + ((SEG ? static_cast<long long>(seg_off[e]) : static_cast<long long>(e) * C) + l) * M;
         if constexpr (VEC) {
           const int nv = M / Vec<T>::N;
           for (int v = lane; v < nv; v += 32) {
@@ -656,6 +718,18 @@ cudaError_t route_locations(const int* idx, int* loc, int* counts, int* workspac
   return cudaGetLastError();
 }
 
+cudaError_t packed_layout(const int* idx, const int* loc, const int* counts, int* seg_off, int* block_expert,
+                          int* block_rows, int* slot_src, int S, int E, int k, int R, cudaStream_t stream) {
+  if (E <= 0 || R <= 0 || R % kPackBlock != 0) return cudaErrorInvalidValue;
+  const int nblocks = R / kPackBlock;
+  packed_layout_kernel<<<1, 1024, sizeof(int) * (E + 1), stream>>>(counts, seg_off, block_expert, block_rows, E, nblocks);
+  cudaError_t e = cudaMemsetAsync(slot_src, 0xFF, sizeof(int) * static_cast<size_t>(R), stream);
+  if (e != cudaSuccess) return e;
+  const long long n = static_cast<long long>(S) * k;
+  if (n > 0) packed_slot_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(idx, loc, seg_off, slot_src, S, E, k, R);
+  return cudaGetLastError();
+}
+
 cudaError_t build_slot_map(const int* idx, const int* loc, int* slot_src, int S, int E, int k, int C,
                            cudaStream_t stream) {
   cudaError_t e = cudaMemsetAsync(slot_src, 0xFF, sizeof(int) * static_cast<size_t>(E) * C, stream);
@@ -777,58 +851,58 @@ cudaError_t quantize_transpose_e4m3(const void* x, void* qT, float* scale, float
 template <typename T>
 static cudaError_t decode_rows_t(const void* buf, const void* gates, const int* idx, const int* loc, void* out,
                                  const uint32_t* wait_flags, uint32_t wait_target, int S, int E, int k, int C, int M,
-                                 cudaStream_t stream) {
+                                 const int* seg_off, cudaStream_t stream) {
   if (S <= 0 || M <= 0) return cudaSuccess;
   if (k > kMaxK) return cudaErrorInvalidValue;
   const long long want = (static_cast<long long>(S) + 7) / 8;
   const int grid = static_cast<int>(want < 8LL * num_sms() ? want : 8LL * num_sms());
   const bool vec = (M % Vec<T>::N == 0) && ((reinterpret_cast<uintptr_t>(buf) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
-  if (vec)
-    decode_rows_kernel<T, true><<<grid, 256, 0, stream>>>(static_cast<const T*>(buf), static_cast<const float*>(gates),
-                                                          idx, loc, static_cast<T*>(out), wait_flags, wait_target, S,
-                                                          E, k, C, M);
-  else
-    decode_rows_kernel<T, false><<<grid, 256, 0, stream>>>(static_cast<const T*>(buf), static_cast<const float*>(gates),
-                                                           idx, loc, static_cast<T*>(out), wait_flags, wait_target, S,
-                                                           E, k, C, M);
+  // (expert-packed buffers run their own instantiations: the padded ones keep their address arithmetic)
+#define TB_DEC(VECv, SEGv)                                                                                            \
+  decode_rows_kernel<T, VECv, SEGv><<<grid, 256, 0, stream>>>(static_cast<const T*>(buf), static_cast<const float*>(gates), \
+                                                              idx, loc, static_cast<T*>(out), wait_flags, wait_target, S,  \
+                                                              E, k, C, M, seg_off)
+  if (seg_off != nullptr) { if (vec) TB_DEC(true, true); else TB_DEC(false, true); }
+  else { if (vec) TB_DEC(true, false); else TB_DEC(false, false); }
+#undef TB_DEC
   return cudaGetLastError();
 }
 
 cudaError_t decode_rows(const void* buf, const void* gates, const int* idx, const int* loc, void* out,
                         const uint32_t* wait_flags, uint32_t wait_target, int S, int E, int k, int C, int M,
-                        int elem_type, cudaStream_t stream) {
+                        int elem_type, cudaStream_t stream, const int* seg_off) {
   switch (elem_type) {
-    case ET_F32: return decode_rows_t<float>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, stream);
-    case ET_F16: return decode_rows_t<__half>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, stream);
-    case ET_BF16: return decode_rows_t<__nv_bfloat16>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, stream);
+    case ET_F32: return decode_rows_t<float>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, stream);
+    case ET_F16: return decode_rows_t<__half>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, stream);
+    case ET_BF16: return decode_rows_t<__nv_bfloat16>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, stream);
   }
   return cudaErrorInvalidValue;
 }
 
 template <typename T>
 static cudaError_t gate_grad_t(const void* a, const void* buf, const int* idx, const int* loc, void* dgate, int S, int E,
-                               int k, int C, int M, cudaStream_t stream) {
+                               int k, int C, int M, const int* seg_off, cudaStream_t stream) {
   if (S <= 0) return cudaSuccess;
   const long long want = (static_cast<long long>(S) + 7) / 8;
   const int grid = static_cast<int>(want < 8LL * num_sms() ? want : 8LL * num_sms());
   const bool vec = (M % Vec<T>::N == 0) && ((reinterpret_cast<uintptr_t>(a) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(buf) & 15) == 0);
-  if (vec)
-    gate_grad_kernel<T, true><<<grid, 256, 0, stream>>>(static_cast<const T*>(a), static_cast<const T*>(buf), idx, loc,
-                                                        static_cast<float*>(dgate), S, E, k, C, M);
-  else
-    gate_grad_kernel<T, false><<<grid, 256, 0, stream>>>(static_cast<const T*>(a), static_cast<const T*>(buf), idx, loc,
-                                                         static_cast<float*>(dgate), S, E, k, C, M);
+#define TB_GG(VECv, SEGv)                                                                                             \
+  gate_grad_kernel<T, VECv, SEGv><<<grid, 256, 0, stream>>>(static_cast<const T*>(a), static_cast<const T*>(buf), idx, loc, \
+                                                            static_cast<float*>(dgate), S, E, k, C, M, seg_off)
+  if (seg_off != nullptr) { if (vec) TB_GG(true, true); else TB_GG(false, true); }
+  else { if (vec) TB_GG(true, false); else TB_GG(false, false); }
+#undef TB_GG
   return cudaGetLastError();
 }
 
 cudaError_t gate_grad(const void* a, const void* buf, const int* idx, const int* loc, void* dgate, int S, int E, int k,
-                      int C, int M, int elem_type, cudaStream_t stream) {
+                      int C, int M, int elem_type, cudaStream_t stream, const int* seg_off) {
   switch (elem_type) {
-    case ET_F32: return gate_grad_t<float>(a, buf, idx, loc, dgate, S, E, k, C, M, stream);
-    case ET_F16: return gate_grad_t<__half>(a, buf, idx, loc, dgate, S, E, k, C, M, stream);
-    case ET_BF16: return gate_grad_t<__nv_bfloat16>(a, buf, idx, loc, dgate, S, E, k, C, M, stream);
+    case ET_F32: return gate_grad_t<float>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, stream);
+    case ET_F16: return gate_grad_t<__half>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, stream);
+    case ET_BF16: return gate_grad_t<__nv_bfloat16>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, stream);
   }
   return cudaErrorInvalidValue;
 }

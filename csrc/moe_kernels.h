@@ -42,13 +42,21 @@ cudaError_t encode_rows_fp8(const void* x, const void* gates, const int* slot_sr
 // out[s, :] = sum_j w_j * buf[idx_j[s]*C + loc_j[s], :]  (choices with loc >= C or idx < 0 contribute 0).
 // wait_flags (optional): uint32[E] counters that must reach wait_target (acquire.sys) before expert e's rows
 // are read (combine fusion).
+// seg_off (optional, int[E]): expert-packed buffer, the row of (e, l) is seg_off[e] + l instead of e*C + l.
 cudaError_t decode_rows(const void* buf, const void* gates, const int* idx, const int* loc, void* out,
                         const uint32_t* wait_flags, uint32_t wait_target, int S, int E, int k, int C, int M,
-                        int elem_type, cudaStream_t stream);
+                        int elem_type, cudaStream_t stream, const int* seg_off = nullptr);
 
-// dgate[j*S + s] = dot(a[s, :], buf[slot_j(s), :])   (fp32 accumulate, 0 for dropped choices).
+// dgate[j*S + s] = dot(a[s, :], buf[slot_j(s), :])   (fp32 accumulate, 0 for dropped choices).  seg_off: as decode_rows.
 cudaError_t gate_grad(const void* a, const void* buf, const int* idx, const int* loc, void* dgate, int S, int E,
-                      int k, int C, int M, int elem_type, cudaStream_t stream);
+                      int k, int C, int M, int elem_type, cudaStream_t stream, const int* seg_off = nullptr);
+
+// Expert-packed layout of R rows (R % 128 == 0, R >= sum_e roundup128(counts[e])), from device counts[E] with no host
+// read: seg_off[E + 1] = exclusive scan of roundup128(counts), block_expert / block_rows [R / 128] = the expert and the
+// valid rows of each 128-row block (0 past seg_off[E]), slot_src[R] = token*k + j of row seg_off[e] + loc, -1 for
+// padding.  Three launches (layout, -1 fill, scatter).
+cudaError_t packed_layout(const int* idx, const int* loc, const int* counts, int* seg_off, int* block_expert,
+                          int* block_rows, int* slot_src, int S, int E, int k, int R, cudaStream_t stream);
 
 // ---- fused gating + routing (gate_route.cu) ---------------------------------------------------------------------
 // Two launches: logits [S,E] (fp32/fp16/bf16) -> softmax scores (fp32), top-k ids idx[k,S], raw top-k scores top[k,S],
@@ -83,8 +91,10 @@ cudaError_t expert_bias_update(float* bias, float* load, int E, float gamma, cud
 // out[g, n] = sum_r x[g, r, n]  (bias gradients).  splits = colsum_row_splits(..): 1 -> results are written to `out`
 // (dtype of x); > 1 -> partial sums are atomically added to the zero-initialised fp32 buffer `acc` [G, N].
 int colsum_row_splits(int G, int rows, int N, int elem_bytes);
+// offsets (optional, int[G + 1]): group g is rows [offsets[g], offsets[g + 1]) of x (group_stride unused), split over
+// `splits` blocks per column strip; `rows` only bounds the offsets.
 cudaError_t grouped_colsum(const void* x, long long ld, long long group_stride, void* out, float* acc, int G, int rows,
-                           int N, int splits, int elem_type, cudaStream_t stream);
+                           int N, int splits, int elem_type, cudaStream_t stream, const int* offsets = nullptr);
 
 // out[s, e] = (sum_{s' <= s} in[s', e]) - 1   (`tutel_ops.cumsum`, tutel/custom/custom_kernel.cpp:822-872)
 size_t cumsum_workspace_ints(int S, int E);

@@ -129,6 +129,21 @@ class FusedExpertsNetwork(torch.nn.Module):
         w1, b1, w2, b2 = self.materialize(ctx)
         return self.compute(x, w1, b1, w2, b2, row_counts)
 
+    def supports_packed(self, x) -> bool:
+        """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit ReLU / GELU / SiLU experts
+        without fp8 / MX, on weights of x's dtype."""
+        w1 = self.batched_fc1_w
+        return (not self.fp8 and not self.mx and self._act_kind in G.FWD_EPILOGUE and x.dtype in (torch.float16, torch.bfloat16)
+                and w1.dtype == x.dtype and x.is_cuda and self.sharded_count == 1 and
+                all(d % 8 == 0 for d in (self.model_dim, self.hidden_size, self.output_dim)))
+
+    def forward_packed(self, x, layout, ctx):
+        """x [R, M]: an expert-packed buffer (ops/packed.py) -> [R, Mout] in the same layout."""
+        if self.skip_expert:
+            return x
+        w1, b1, w2, b2 = self.materialize(ctx)
+        return G.fused_act_ffn(x, w1, b1, w2, b2, None, self._act_kind, layout=layout)
+
     def compute(self, x, w1, b1, w2, b2, row_counts=None):
         lead = x.shape
         if x.dim() > 3:

@@ -78,6 +78,18 @@ class LlamaFFNNetwork(torch.nn.Module):
         y2 = G.grouped_linear(x, w2, None, 'kn', fp8=self.fp8)
         return G.grouped_linear(self.activation_fn(y1) * y2, w3, None, 'kn', fp8=self.fp8)
 
+    def supports_packed(self, x) -> bool:
+        """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit experts without fp8."""
+        M, H = self.full_shapes['W_fc1'][1], self.full_shapes['W_fc1'][2]
+        return (not self.fp8 and x.dtype in (torch.float16, torch.bfloat16) and self.W_fc1.dtype == x.dtype and x.is_cuda and
+                self.sharded_count == 1 and G.classify_activation(self.activation_fn) in G.ACT_CODES and
+                M % 8 == 0 and H % 8 == 0)
+
+    def forward_packed(self, x, layout, ctx):
+        """x [R, M]: an expert-packed buffer (ops/packed.py) -> [R, M] in the same layout."""
+        w1, w2, w3 = (self._full(n, ctx.group) for n in ('W_fc1', 'W_fc2', 'W_fc3'))
+        return G.fused_glu_ffn(x, w1, w2, w3, G.classify_activation(self.activation_fn), False, None, layout=layout)
+
     def extra_repr(self):
         return 'full shapes: %s, sharded_count=%d' % ({k: tuple(v) for k, v in self.full_shapes.items()}, self.sharded_count)
 

@@ -256,7 +256,8 @@ class MOELayer(torch.nn.Module):
         self.protected_shape = y.shape
         return y.reshape(y.size(0), y.size(1), -1)
 
-    def _route(self, x, gctx, top_k, capacity_factor, a2a_ffn_overlap_degree, megablocks_size, inequivalent_tokens):
+    def _route(self, x, gctx, top_k, capacity_factor, a2a_ffn_overlap_degree, megablocks_size, inequivalent_tokens,
+               packed=False):
         logits = gctx(x)
         if self.training and gctx.gate_noise > 0:
             logits_w_noise = logits + gctx.gate_noise * torch.randn_like(logits) / self.num_global_experts
@@ -268,7 +269,7 @@ class MOELayer(torch.nn.Module):
             alignment = (alignment + 127) // 128 * 128
         if getattr(gctx, 'scoring_func', 'softmax') == 'sigmoid':
             return self._route_sigmoid(x, logits, logits_w_noise, gctx, top_k, capacity_factor, alignment,
-                                       megablocks_size, inequivalent_tokens)
+                                       megablocks_size, inequivalent_tokens, packed)
         fused_gate, gate_mode = None, fused_gate_mode()
         k_eff = min(top_k, self.num_global_experts)
         cuda_fused = (self.is_gshard_loss and gate_mode != 'off' and not self.batch_prioritized_routing and
@@ -279,7 +280,7 @@ class MOELayer(torch.nn.Module):
                 cf = capacity_factor or gctx.capacity_factor
                 bound = self._dropless_bound(logits_w_noise, x, cf, megablocks_size, inequivalent_tokens)
                 crit, l_aux = fused_extract_critical(logits_w_noise, top_k, cf, self.normalize_gate, alignment, self.group,
-                                                     inequivalent_tokens, rows_bound=bound)
+                                                     inequivalent_tokens, rows_bound=bound, packed=packed)
                 if getattr(crit, 'skip_padding', False) and not getattr(self.experts, 'rows_independent', False):
                     # experts that do not declare `rows_independent = True` may mix rows of the buffer: keep the zero padding
                     crit.skip_padding = False
@@ -299,7 +300,7 @@ class MOELayer(torch.nn.Module):
                                        capacity_factor=capacity_factor or gctx.capacity_factor,
                                        batch_prioritized_routing=self.batch_prioritized_routing,
                                        normalize_gate=self.normalize_gate, group=self.group, alignment=alignment,
-                                       inequivalent_tokens=inequivalent_tokens, _fused=fused_gate)
+                                       inequivalent_tokens=inequivalent_tokens, _fused=fused_gate, packed=packed)
         return logits.dtype, crit, l_aux
 
     def _dropless_bound(self, logits, x, cf, megablocks_size, inequivalent_tokens):
@@ -312,7 +313,7 @@ class MOELayer(torch.nn.Module):
         return 0
 
     def _route_sigmoid(self, x, logits, logits_w_noise, gctx, top_k, capacity_factor, alignment, megablocks_size,
-                       inequivalent_tokens):
+                       inequivalent_tokens, packed=False):
         """Sigmoid scoring with the gate's selection bias and group limit (ops/gating.py).  Training forwards with
         gradients add their all-choice counts to the gate's ``expert_load`` for the next bias update."""
         k_eff = min(top_k, self.num_global_experts)
@@ -328,7 +329,7 @@ class MOELayer(torch.nn.Module):
             bound = self._dropless_bound(logits_w_noise, x, cf, megablocks_size, inequivalent_tokens)
             crit, l_aux = fused_extract_critical(logits_w_noise, top_k, cf, self.normalize_gate, alignment, self.group,
                                                  inequivalent_tokens, rows_bound=bound,
-                                                 sigmoid=dict(args, expert_load=load))
+                                                 sigmoid=dict(args, expert_load=load), packed=packed)
             if getattr(crit, 'skip_padding', False) and not getattr(self.experts, 'rows_independent', False):
                 crit.skip_padding = False
         else:
@@ -339,7 +340,8 @@ class MOELayer(torch.nn.Module):
             crit, _ = extract_critical(logits_w_noise, top_k=top_k, loss_fn=None, capacity_factor=cf,
                                        batch_prioritized_routing=self.batch_prioritized_routing,
                                        normalize_gate=self.normalize_gate, group=self.group, alignment=alignment,
-                                       inequivalent_tokens=inequivalent_tokens, _fused=(idx, gates, l_aux, top1))
+                                       inequivalent_tokens=inequivalent_tokens, _fused=(idx, gates, l_aux, top1),
+                                       packed=packed)
         if accumulate:
             gctx.note_training_forward()
         return logits.dtype, crit, l_aux
@@ -381,13 +383,16 @@ class MOELayer(torch.nn.Module):
         top_k = top_k or gctx.top_k
         if megablocks_size > 0 and (self.num_local_experts <= 1 or torch.is_grad_enabled() or self.world_size > 1):
             megablocks_size = 0
+        packed = self._packed_eligible(x, gctx, capacity_factor, megablocks_size, reserve_dims)
 
         with stage('route'):
             if x.is_cuda or x.device.type == 'cpu':
                 with torch.amp.autocast(x.device.type, enabled=False):
-                    logits_dtype, crit, l_aux = self._route(x, gctx, top_k, capacity_factor, d, megablocks_size, inequivalent_tokens)
+                    logits_dtype, crit, l_aux = self._route(x, gctx, top_k, capacity_factor, d, megablocks_size, inequivalent_tokens,
+                                                            packed)
             else:
-                logits_dtype, crit, l_aux = self._route(x, gctx, top_k, capacity_factor, d, megablocks_size, inequivalent_tokens)
+                logits_dtype, crit, l_aux = self._route(x, gctx, top_k, capacity_factor, d, megablocks_size, inequivalent_tokens,
+                                                        packed)
 
         self.megablocks_size = megablocks_size
         self.dispatch_count = get_dispatch_count(crit)
@@ -397,8 +402,10 @@ class MOELayer(torch.nn.Module):
 
         x = x.contiguous()
         y = None
-        fused = self._fused_engine(x, crit, d, reserve_dims)
-        if fused is not None:
+        fused = None if packed else self._fused_engine(x, crit, d, reserve_dims)
+        if packed:
+            y = self._packed_forward(x, crit)
+        elif fused is not None:
             with stage('fused'):
                 y = fused.run(self, x, crit)
             self.protected_shape = y.shape
@@ -437,6 +444,35 @@ class MOELayer(torch.nn.Module):
         y = y.view(list(original_shape[:-reserve_dims]) + list(self.protected_shape[-reserve_dims:])).to(original_dtype)
         self.l_aux = y.l_aux = l_aux
         return self.result_func(y) if self.result_func is not None else y
+
+    # ---------------------------------------------------------------------------------------- packed dropless
+    def _packed_eligible(self, x, gctx, capacity_factor, megablocks_size, reserve_dims) -> bool:
+        """Dropless training on one GPU runs on the expert-packed layout (ops/packed.py): every expert GEMM costs
+        sum(count) rows instead of E * max(count), and nothing reads the counts back to the host.  Taken by forwards with
+        gradients when the resolved capacity factor is exactly 0, on one GPU, outside bound-based dropless decoding
+        (megablocks_size), with one reserved dim, 16-bit CUDA activations and experts that implement ``forward_packed``
+        for them.  Inference forwards keep the padded and bound-based paths."""
+        cf = capacity_factor or gctx.capacity_factor
+        if not (cf == 0 and torch.is_grad_enabled() and self.world_size == 1 and megablocks_size == 0 and reserve_dims == 1 and x.is_cuda and
+                x.dtype in (torch.float16, torch.bfloat16) and x.dim() == 2 and x.size(0) > 0):
+            return False
+        supports = getattr(self.experts, 'supports_packed', None)
+        if not callable(getattr(self.experts, 'forward_packed', None)) or supports is None or not supports(x):
+            return False
+        from ..ops import backend
+        return backend.has_cuda_ext()
+
+    def _packed_forward(self, x, crit):
+        from ..ops.dispatch import DispatchPlan, GatingDecoder, GatingEncoder
+        plan = DispatchPlan.from_critical(crit)
+        with stage('encode'):
+            y = GatingEncoder.apply(plan, x, None if self.is_postscore else crit.gates_ks)
+        with stage('experts'):
+            y = self.experts.forward_packed(y, crit.layout, self)
+        self.protected_shape = y.shape
+        with stage('decode'):
+            y = GatingDecoder.apply(plan, y, crit.gates_ks if self.is_postscore else None)
+        return y
 
     # ------------------------------------------------------------------------------------------- fused engine
     def _fused_engine(self, x, crit, d, reserve_dims):

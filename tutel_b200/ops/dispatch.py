@@ -33,6 +33,7 @@ class DispatchPlan:
         self.k, self.S = int(idx_ks.size(0)), int(idx_ks.size(1))
         self._slot_src = slot_src
         self.valid_rows = None        # int32 [E]: when set, encode leaves rows past the per-expert count untouched
+        self.layout = None            # PackedLayout (ops/packed.py): the buffer is the expert-packed [R, M]
 
     @property
     def slot_src(self) -> torch.Tensor:
@@ -48,6 +49,7 @@ class DispatchPlan:
                 plan = DispatchPlan(crit[0], crit[4], crit.idx_ks, crit.loc_ks, crit._slot_src)
                 if getattr(crit, 'skip_padding', False):
                     plan.valid_rows = crit[5]
+                plan.layout = getattr(crit, 'layout', None)
                 crit._plan = plan
             return plan
         E, indices_s, locations_s, _, capacity = crit[0], crit[1], crit[2], crit[3], crit[4]
@@ -76,6 +78,9 @@ def _slots(plan: DispatchPlan):
 
 def raw_encode(x: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchPlan) -> torch.Tensor:
     """x [S, M] -> [E*C, M];  row(slot) = gate * x[token(slot)]  or zeros."""
+    if plan.layout is not None:
+        from . import packed
+        return packed.encode(x, gates, plan.layout)
     x = x.contiguous()
     M = x.size(1)
     if _native_cuda(x):
@@ -98,6 +103,9 @@ def raw_encode(x: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchPla
 
 def raw_decode(buf: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchPlan) -> torch.Tensor:
     """buf [E*C, M] -> [S, M];  out[s] = sum_j gate_j[s] * buf[slot_j(s)]."""
+    if plan.layout is not None:
+        from . import packed
+        return packed.decode(buf.view(plan.layout.R, -1), gates, plan.idx_ks, plan.loc_ks, plan.layout)
     buf = buf.contiguous().view(plan.E * plan.C, -1)
     if _native_cuda(buf):
         g = None if gates is None else gates.to(torch.float32).contiguous()
@@ -118,6 +126,9 @@ def raw_decode(buf: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchP
 
 def raw_gate_grad(a: torch.Tensor, buf: torch.Tensor, plan: DispatchPlan) -> torch.Tensor:
     """[k, S] row dots  <a[s], buf[slot_j(s)]>  (0 for dropped choices); fp32 on CUDA."""
+    if plan.layout is not None:
+        from . import packed
+        return packed.gate_grad(a, buf.view(plan.layout.R, -1), plan.idx_ks, plan.loc_ks, plan.layout)
     a = a.contiguous()
     buf = buf.contiguous().view(plan.E * plan.C, -1)
     if _native_cuda(a) and a.dtype == buf.dtype:

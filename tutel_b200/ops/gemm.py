@@ -55,21 +55,39 @@ def raw_gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool
              wait_rows_per_flag: int = 0, wait_flags_per_group: int = 0, wait_target: int = 0,
              max_ctas: int = 0, group_rot: int = 0, group_mod: int = 1, scale_a: Optional[torch.Tensor] = None,
              scale_b: Optional[torch.Tensor] = None, colsum: Optional[torch.Tensor] = None,
-             d2: Optional[torch.Tensor] = None, act: int = 0) -> torch.Tensor:
+             d2: Optional[torch.Tensor] = None, act: int = 0, b_group_map: Optional[torch.Tensor] = None,
+             k_offsets: Optional[torch.Tensor] = None) -> torch.Tensor:
     """D[g] = epilogue(A[g] @ B[g // b_group_div]).
 
     ``a``: ``[G, M, K]`` (or ``[G, K, M]`` when ``a_mn``);  ``b``: ``[Gb, N, K]`` (or ``[Gb, K, N]`` when ``b_mn``).
+
+    Packed-layout launch modes (ops/packed.py):
+
+    * ``b_group_map`` (int32 [R / 128]): ``a`` is a K-major ``[R, K]`` buffer of 128-row blocks and block ``g`` is
+      multiplied by ``B[b_group_map[g]]``; the result is ``[R, N]``.  With ``row_counts`` (the blocks' valid rows), rows
+      of a block at or past its count are stored as zeros and blocks with no rows are skipped.
+    * ``k_offsets`` (int32 [E + 1]): ``a`` and ``b`` are single ``[R, *]`` tensors (``a_mn`` / ``b_mn``) and
+      ``D[g] = A[k_offsets[g]:k_offsets[g+1]]^T @ B[k_offsets[g]:k_offsets[g+1]]``, ``[E, M, N]`` (weight gradients).
     """
     C = backend.require_ext()
+    if b_group_map is not None:
+        assert not a_mn and a.dim() == 2 and a.size(0) % 128 == 0, 'b_group_map: a must be a K-major [R, K] buffer'
+        a = a.view(-1, 128, a.size(1))
+        if aux is not None:
+            aux = aux.view(-1, 128, aux.size(-1))
     a, b = _prep(a), _prep(b)
-    G = a.size(0)
+    G = a.size(0) if k_offsets is None else k_offsets.numel() - 1
     M = a.size(2) if a_mn else a.size(1)
     N = b.size(2) if b_mn else b.size(1)
     if out is None:
         if out_dtype is None:
             out_dtype = a.dtype if a.element_size() > 1 else torch.bfloat16
         out = torch.empty([G, M, N], dtype=out_dtype, device=a.device)
+    elif b_group_map is not None:
+        out = out.view(G, M, N)
     d = out if out.dim() == 3 else out.unsqueeze(0)
+    if d2 is not None and b_group_map is not None:
+        d2 = d2.view(G, M, N)
     if bias is not None:
         bias = _side(bias.reshape(b.size(0), N), a.dtype if a.element_size() > 1 else out.dtype)
     if scale_b is not None:
@@ -77,11 +95,14 @@ def raw_gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool
     if aux is not None:
         aux = _prep(aux)
     backend.count_launch()
-    C.gemm_ex(a, b, d, a_mn, b_mn, epilogue, bias, aux, row_counts, float(alpha), int(b_group_div), int(cta_group),
-              int(block_n), int(d_ptr_table), int(signal_ptr_table), int(wait_flags), int(wait_rows_per_flag),
-              int(wait_flags_per_group), int(wait_target), int(max_ctas), int(group_rot), int(group_mod), scale_a, scale_b, colsum,
-              d2, int(act))
-    return out
+    args = (a, b, d, a_mn, b_mn, epilogue, bias, aux, row_counts, float(alpha), int(b_group_div), int(cta_group), int(block_n),
+            int(d_ptr_table), int(signal_ptr_table), int(wait_flags), int(wait_rows_per_flag), int(wait_flags_per_group),
+            int(wait_target), int(max_ctas), int(group_rot), int(group_mod), scale_a, scale_b, colsum, d2, int(act))
+    if b_group_map is None and k_offsets is None:
+        C.gemm_ex(*args)
+    else:
+        C.gemm_ex(*args, b_group_map, k_offsets)
+    return out.view(-1, N) if b_group_map is not None else out
 
 
 def column_sums(t: torch.Tensor) -> torch.Tensor:
@@ -165,55 +186,74 @@ class FusedReluFFN(torch.autograd.Function):
     ``w1 [G, H, M]`` (nk), ``w2 [G, H, Mout]`` (kn) - the reference's ``batched_fc1_w`` / ``batched_fc2_w`` layout.
     ReLU keeps only the post-activation tensor (its sign doubles as the gradient mask fused into the dgrad epilogue);
     GELU / SiLU also store the pre-activation from the same epilogue and apply act'(pre) in the dgrad epilogue.
+
+    ``layout`` (:class:`tutel_b200.ops.packed.PackedLayout`): ``x [R, M]`` is an expert-packed buffer and so is the
+    result.  The same launches then run block-mapped (forward, data gradients: padding rows come out zero) and with
+    ragged K (weight gradients over each expert's segment); the fc2 bias gradient is a segmented column sum.  ``dy``'s
+    padding rows must be zero, as the packed decode's backward leaves them.
     """
 
     @staticmethod
-    def forward(ctx: Any, x, w1, b1, w2, b2, row_counts, act_kind='relu'):
+    def forward(ctx: Any, x, w1, b1, w2, b2, row_counts, act_kind='relu', layout=None):
         need_grad = any(ctx.needs_input_grad[:5])
+        pk = {} if layout is None else dict(b_group_map=layout.block_expert)
+        if layout is not None:
+            row_counts = layout.block_rows
         pre = None
         if act_kind == 'relu':
-            act = raw_gemm(x, w1, epilogue=EPI_BIAS_RELU, bias=b1, row_counts=row_counts)
+            act = raw_gemm(x, w1, epilogue=EPI_BIAS_RELU, bias=b1, row_counts=row_counts, **pk)
         else:
-            pre = torch.empty([x.size(0), x.size(1), w1.size(1)], dtype=x.dtype, device=x.device) if need_grad else None
-            act = raw_gemm(x, w1, epilogue=FWD_EPILOGUE[act_kind], bias=b1, row_counts=row_counts, d2=pre)
+            pre = torch.empty(list(x.shape[:-1]) + [w1.size(1)], dtype=x.dtype, device=x.device) if need_grad else None
+            act = raw_gemm(x, w1, epilogue=FWD_EPILOGUE[act_kind], bias=b1, row_counts=row_counts, d2=pre, **pk)
         y = raw_gemm(act, w2, b_mn=True, epilogue=EPI_BIAS if b2 is not None else EPI_NONE, bias=b2,
-                     row_counts=row_counts)
+                     row_counts=row_counts, **pk)
         ctx.save_for_backward(x, w1, w2, act, pre)
         ctx.has_b1, ctx.has_b2, ctx.act_kind = b1 is not None, b2 is not None, act_kind
         ctx.row_counts = row_counts
+        ctx.layout = layout
         return y
 
     @staticmethod
     def backward(ctx: Any, dy: torch.Tensor):
         x, w1, w2, act, pre = ctx.saved_tensors
         rc = ctx.row_counts
+        layout = ctx.layout
+        packed = layout is not None
+        pk = {} if layout is None else dict(b_group_map=layout.block_expert)
+        wk = {} if layout is None else dict(k_offsets=layout.seg_off)    # weight gradients: one K range per expert
         dy = dy if _ok_stride(dy) else dy.contiguous()
-        if rc is not None:
+        if rc is not None and not packed:
             dy = _zero_tail(dy, rc)
         # dh[T,H] = (dy[T,Mout] @ W2^T) * act'(.)           W2 [H,Mout] is "nk" for this product
         want_db1 = ctx.has_b1 and ctx.needs_input_grad[2]
         db1_acc = torch.zeros([w1.size(0), w1.size(1)], dtype=torch.float32, device=dy.device) if want_db1 else None
         if ctx.act_kind == 'relu':
-            dh = raw_gemm(dy, w2, epilogue=EPI_RELU_BWD, aux=act, row_counts=rc, colsum=db1_acc)   # db1 fused in the epilogue
+            dh = raw_gemm(dy, w2, epilogue=EPI_RELU_BWD, aux=act, row_counts=rc, colsum=db1_acc, **pk)   # db1 fused in the epilogue
         else:
-            dh = raw_gemm(dy, w2, epilogue=EPI_ACT_BWD, aux=pre, act=ACT_CODES[ctx.act_kind], row_counts=rc, colsum=db1_acc)
-        if rc is not None:
+            dh = raw_gemm(dy, w2, epilogue=EPI_ACT_BWD, aux=pre, act=ACT_CODES[ctx.act_kind], row_counts=rc, colsum=db1_acc, **pk)
+        if rc is not None and not packed:
             dh = _zero_tail(dh, rc)
             act = _zero_tail(act, rc)
-        dw2 = raw_gemm(act, dy, a_mn=True, b_mn=True) if ctx.needs_input_grad[3] else None      # [H,Mout] = act^T @ dy
-        db2 = column_sums(dy) if ctx.has_b2 and ctx.needs_input_grad[4] else None
-        dx = raw_gemm(dh, w1, b_mn=True, row_counts=rc) if ctx.needs_input_grad[0] else None    # [T,M] = dh @ W1
-        if dx is not None and rc is not None:
+        dw2 = raw_gemm(act, dy, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[3] else None      # [H,Mout] = act^T @ dy
+        db2 = None
+        if ctx.has_b2 and ctx.needs_input_grad[4]:
+            if packed:
+                from .packed import segment_colsum
+                db2 = segment_colsum(dy, layout)
+            else:
+                db2 = column_sums(dy)
+        dx = raw_gemm(dh, w1, b_mn=True, row_counts=rc, **pk) if ctx.needs_input_grad[0] else None    # [T,M] = dh @ W1
+        if dx is not None and rc is not None and not packed:
             dx = _zero_tail(dx, rc)
-        dw1 = raw_gemm(dh, x, a_mn=True, b_mn=True) if ctx.needs_input_grad[1] else None        # [H,M] = dh^T @ x
+        dw1 = raw_gemm(dh, x, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[1] else None        # [H,M] = dh^T @ x
         db1 = db1_acc.to(dh.dtype) if want_db1 else None
-        return dx, dw1, db1, dw2, db2, None, None
+        return dx, dw1, db1, dw2, db2, None, None, None
 
 
-def fused_relu_ffn(x, w1, b1, w2, b2, row_counts=None, act_kind='relu'):
+def fused_relu_ffn(x, w1, b1, w2, b2, row_counts=None, act_kind='relu', layout=None):
     b1 = None if b1 is None else b1.reshape(w1.size(0), -1)
     b2 = None if b2 is None else b2.reshape(w2.size(0), -1)
-    return FusedReluFFN.apply(x, w1, b1, w2, b2, row_counts, act_kind)
+    return FusedReluFFN.apply(x, w1, b1, w2, b2, row_counts, act_kind, layout)
 
 
 fused_act_ffn = fused_relu_ffn
@@ -474,12 +514,19 @@ def _glu_extra(kw):
             int(kw.get('group_rot', 0)), int(kw.get('group_mod', 1)))
 
 
+def _blocks(t: torch.Tensor) -> torch.Tensor:
+    """A packed ``[R, N]`` buffer as ``[R / 128, 128, N]``: the uniform groups of a block-mapped launch."""
+    return t.view(-1, 128, t.size(-1))
+
+
 def glu_gemm(a, b, b2, *, b_mn, act, save_pre=False, scale_a=None, scale_b=None, scale_b2=None, row_counts=None,
-             out_dtype=None, **kw):
+             out_dtype=None, b_group_map=None, **kw):
     """h = act(a @ B) * (a @ B2) in ONE wgmma launch (the two weight tiles share one stage of the operand ring; the
-    gate/up halves meet in the accumulator fragment).  ``save_pre`` also returns the pre-activations (g, u)."""
+    gate/up halves meet in the accumulator fragment).  ``save_pre`` also returns the pre-activations (g, u).
+    ``b_group_map``: ``a`` is a packed ``[R, K]`` buffer (see :func:`raw_gemm`), and so are the results."""
     C = backend.require_ext()
-    a, b, b2 = _prep(a), _prep(b), _prep(b2)
+    packed = b_group_map is not None
+    a, b, b2 = _prep(_blocks(a) if packed else a), _prep(b), _prep(b2)
     if b2.stride() != b.stride():
         b, b2 = b.contiguous(), b2.contiguous()
     N = b.size(2) if b_mn else b.size(1)
@@ -487,19 +534,30 @@ def glu_gemm(a, b, b2, *, b_mn, act, save_pre=False, scale_a=None, scale_b=None,
     h = torch.empty([a.size(0), a.size(1), N], dtype=dt, device=a.device)
     g, u = (torch.empty_like(h), torch.empty_like(h)) if save_pre else (None, None)
     backend.count_launch()
-    C.gemm_glu(a, b, b2, h, g, u, None, None, b_mn, ACT_CODES[act], scale_a, scale_b, scale_b2, row_counts, *_glu_extra(kw))
-    return h, g, u
+    args = (a, b, b2, h, g, u, None, None, b_mn, ACT_CODES[act], scale_a, scale_b, scale_b2, row_counts) + _glu_extra(kw)
+    if not packed:
+        C.gemm_glu(*args)
+        return h, g, u
+    C.gemm_glu(*args, b_group_map)
+    return h.view(-1, N), (g.view(-1, N) if save_pre else None), (u.view(-1, N) if save_pre else None)
 
 
-def glu_gemm_bwd(dy, w, g, u, *, b_mn, act, row_counts=None, scale_a=None, scale_b=None, **kw):
+def glu_gemm_bwd(dy, w, g, u, *, b_mn, act, row_counts=None, scale_a=None, scale_b=None, b_group_map=None, **kw):
     """(dg, du) for h = act(g) * u with dh = dy @ W formed in registers only (never written to memory); dy / W may be e4m3
-    with per-row scales."""
+    with per-row scales.  ``b_group_map``: packed ``[R, *]`` buffers (see :func:`raw_gemm`)."""
     C = backend.require_ext()
+    packed = b_group_map is not None
+    if packed:
+        dy, g, u = _blocks(dy), _blocks(g), _blocks(u)
     dy, w = _prep(dy), _prep(w)
     dg, du = torch.empty_like(g), torch.empty_like(g)
     backend.count_launch()
-    C.gemm_glu(dy, w, None, dg, du, None, g, u, b_mn, ACT_CODES[act], scale_a, scale_b, None, row_counts, *_glu_extra(kw))
-    return dg, du
+    args = (dy, w, None, dg, du, None, g, u, b_mn, ACT_CODES[act], scale_a, scale_b, None, row_counts) + _glu_extra(kw)
+    if not packed:
+        C.gemm_glu(*args)
+        return dg, du
+    C.gemm_glu(*args, b_group_map)
+    return dg.view(-1, dg.size(-1)), du.view(-1, du.size(-1))
 
 
 class FusedGLUFFN(torch.autograd.Function):
@@ -511,11 +569,24 @@ class FusedGLUFFN(torch.autograd.Function):
     ``w1, w2: [G, M, H]``, ``w3: [G, H, Mout]`` (all "kn", the reference's parameter layout).
     ``row_counts`` (int32 [G], dropless inference only): rows at or past the count of a group are skipped and left
     undefined in the result; there is no backward for it.
+    ``layout`` (:class:`tutel_b200.ops.packed.PackedLayout`, 16-bit only): ``x [R, M]`` is an expert-packed buffer, as in
+    :class:`FusedReluFFN`; forward and backward run block-mapped / ragged-K launches of the same kernels.
     """
 
     @staticmethod
-    def forward(ctx: Any, x, w1, w2, w3, act: str, fp8: bool, row_counts=None):
+    def forward(ctx: Any, x, w1, w2, w3, act: str, fp8: bool, row_counts=None, layout=None):
         need_grad = any(ctx.needs_input_grad[:4])
+        ctx.layout = layout
+        if layout is not None:
+            assert not fp8, 'FusedGLUFFN: the packed layout runs 16-bit operands only'
+            h, g, u = glu_gemm(x, w1, w2, b_mn=True, act=act, save_pre=need_grad, row_counts=layout.block_rows,
+                               b_group_map=layout.block_expert)
+            y = raw_gemm(h, w3, b_mn=True, row_counts=layout.block_rows, b_group_map=layout.block_expert)
+            ctx.act = act
+            ctx.has_row_counts = False
+            if need_grad:
+                ctx.save_for_backward(x, w1, w2, w3, g, u, h)
+            return y
         if fp8:
             xq, sx = quantize_rows(x)
             (q1, s1), (q2, s2), (q3, s3) = fp8_weight(w1, 'kn'), fp8_weight(w2, 'kn'), fp8_weight(w3, 'kn')
@@ -540,6 +611,19 @@ class FusedGLUFFN(torch.autograd.Function):
                                'supported')
         x, w1, w2, w3, g, u, h = ctx.saved_tensors
         dy = dy if _ok_stride(dy) else dy.contiguous()
+        layout = ctx.layout
+        if layout is not None:
+            pk = dict(row_counts=layout.block_rows, b_group_map=layout.block_expert)
+            wk = dict(k_offsets=layout.seg_off)
+            dg, du = glu_gemm_bwd(dy, w3, g, u, b_mn=False, act=ctx.act, **pk)    # dh = dy @ W3^T, padding rows zero
+            dw3 = raw_gemm(h, dy, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[3] else None
+            dw1 = raw_gemm(x, dg, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[1] else None
+            dw2 = raw_gemm(x, du, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[2] else None
+            dx = None
+            if ctx.needs_input_grad[0]:
+                dx = raw_gemm(dg, w1, **pk)
+                dx = raw_gemm(du, w2, epilogue=EPI_ADD, aux=dx, **pk)
+            return dx, dw1, dw2, dw3, None, None, None, None
         if getattr(ctx, 'fp8', False):
             # e4m3 data-gradient GEMMs: dh = dy @ W3^T uses W3 as stored ([H, Mout] is K-major for it), dx uses W1 / W2 as stored
             dyq, sdy = quantize_rows(dy)
@@ -559,8 +643,8 @@ class FusedGLUFFN(torch.autograd.Function):
         elif ctx.needs_input_grad[0]:
             dx = raw_gemm(dg, w1)                                            # [T,M] = dg @ W1^T
             dx = raw_gemm(du, w2, epilogue=EPI_ADD, aux=dx)                  # += du @ W2^T (add fused in the epilogue)
-        return dx, dw1, dw2, dw3, None, None, None
+        return dx, dw1, dw2, dw3, None, None, None, None
 
 
-def fused_glu_ffn(x, w1, w2, w3, act='silu', fp8=False, row_counts=None):
-    return FusedGLUFFN.apply(x, w1, w2, w3, act, fp8, row_counts)
+def fused_glu_ffn(x, w1, w2, w3, act='silu', fp8=False, row_counts=None, layout=None):
+    return FusedGLUFFN.apply(x, w1, w2, w3, act, fp8, row_counts, layout)

@@ -23,6 +23,7 @@ class CriticalData(tuple):
 
     Behaves like the reference's plain tuple; the extra attributes let the kernels consume ``[k, S]`` tensors
     without re-stacking: ``idx_ks``, ``loc_ks`` (int32), ``gates_ks`` (differentiable), ``slot_src`` (lazy).
+    ``layout``: the :class:`tutel_b200.ops.packed.PackedLayout` of a packed-mode routing (capacity 0), else None.
     """
 
     def __new__(cls, E, idx_ks, loc_ks, gates_ks, capacity, counts):
@@ -31,6 +32,7 @@ class CriticalData(tuple):
                                      [gates_ks[j] for j in range(k)], capacity, counts))
         self.idx_ks, self.loc_ks, self.gates_ks = idx_ks, loc_ks, gates_ks
         self._slot_src = None
+        self.layout = None
         return self
 
     @property
@@ -75,9 +77,12 @@ def build_slot_map(idx_ks: torch.Tensor, loc_ks: torch.Tensor, E: int, C: int) -
 
 def extract_critical(scores: torch.Tensor, top_k: int, loss_fn=losses.gshard_loss, capacity_factor: float = 1.0,
                      batch_prioritized_routing: bool = False, normalize_gate: bool = True, alignment: int = 1,
-                     group=None, inequivalent_tokens: bool = False, _fused=None):
+                     group=None, inequivalent_tokens: bool = False, _fused=None, packed: bool = False):
     """``_fused`` (internal): ``(idx_ks, gates_ks, l_aux, top1)`` from :func:`tutel_b200.ops.gating.fused_topk_gate` -
-    top-k selection, gate normalisation and the auxiliary loss were then already computed by the fused kernel."""
+    top-k selection, gate normalisation and the auxiliary loss were then already computed by the fused kernel.
+
+    ``packed`` (dropless on one GPU, CUDA): no capacity is computed - nothing is read back to the host - and the result
+    carries the :class:`tutel_b200.ops.packed.PackedLayout` built from the device counts; its capacity field is 0."""
     num_global_experts = int(scores.size(1))
     top_k_original, top_k = top_k, min(top_k, num_global_experts)
     if _fused is None:
@@ -104,10 +109,21 @@ def extract_critical(scores: torch.Tensor, top_k: int, loss_fn=losses.gshard_los
         denom = torch.clamp(gates_ks.sum(dim=0, keepdim=True), min=torch.finfo(gates_ks.dtype).eps)
         gates_ks = gates_ks / denom
 
+    if packed:
+        return _packed_critical(num_global_experts, idx_ks, loc_ks, gates_ks, counts), l_loss
+
     num_samples = _num_samples(int(scores.size(0)), scores.device, group, inequivalent_tokens)
     capacity = _capacity(num_samples, num_global_experts, top_k, top_k_original, capacity_factor, counts, group, alignment)
 
     return CriticalData(num_global_experts, idx_ks, loc_ks, gates_ks, capacity, counts), l_loss
+
+
+def _packed_critical(E, idx_ks, loc_ks, gates_ks, counts) -> CriticalData:
+    from .packed import PackedLayout
+    crit = CriticalData(E, idx_ks, loc_ks, gates_ks, 0, counts)
+    crit.layout = PackedLayout.build(idx_ks, loc_ks, counts)
+    crit._slot_src = crit.layout.slot_src
+    return crit
 
 
 def _num_samples(local: int, device, group, inequivalent_tokens: bool) -> int:
@@ -138,16 +154,25 @@ def _capacity(num_samples, num_global_experts, top_k, top_k_original, capacity_f
 
 def fused_extract_critical(logits: torch.Tensor, top_k: int, capacity_factor: float = 1.0, normalize_gate: bool = True,
                            alignment: int = 1, group=None, inequivalent_tokens: bool = False, rows_bound: int = 0,
-                           sigmoid: Optional[dict] = None):
+                           sigmoid: Optional[dict] = None, packed: bool = False):
     """CUDA fast path of :func:`extract_critical` for GShard-loss top-k gates: softmax, top-k, gate normalisation, the
     auxiliary loss, queue locations, counts and the inverse slot map come out of TWO kernel launches
     (:func:`tutel_b200.ops.gating.fused_gate_route`); with a positive capacity factor nothing touches the host.
 
     ``sigmoid``: sigmoid scoring instead (:func:`tutel_b200.ops.gating.sigmoid_gate_route`), a dict with ``bias``,
-    ``n_group``, ``topk_group``, ``scale`` and ``expert_load`` (or None)."""
+    ``n_group``, ``topk_group``, ``scale`` and ``expert_load`` (or None).
+
+    ``packed``: dropless into the expert-packed layout (see :func:`extract_critical`): no capacity, no host read."""
     from .gating import fused_gate_route, sigmoid_gate_route
     E = int(logits.size(1))
     top_k_original, top_k = top_k, min(top_k, E)
+    if packed:
+        if sigmoid is None:
+            idx, loc, gates, l_aux, counts, _top1, _ = fused_gate_route(logits, top_k, normalize_gate, 0)
+        else:
+            idx, loc, gates, l_aux, counts, _top1, _ = sigmoid_gate_route(logits, k=top_k, normalize=normalize_gate,
+                                                                          capacity=0, **sigmoid)
+        return _packed_critical(E, idx, loc, gates, counts), l_aux
     num_samples = _num_samples(int(logits.size(0)), logits.device, group, inequivalent_tokens)
     static_cap = _capacity(num_samples, E, top_k, top_k_original, capacity_factor, None, group, alignment) if capacity_factor > 0 else 0
     if capacity_factor <= 0 and rows_bound > 0:

@@ -67,6 +67,8 @@ class GraphedTrainStep:
     gradient accumulators bound to the eager stream, and the capture fails with ``cudaErrorStreamCaptureInvalidated``
     (``MOELayer`` releases its own ``l_aux`` at the start of every forward).  Multi-GPU steps are not capturable this way: the peer-to-peer protocol numbers its
     transactions with host-side epochs that would be frozen into the graph.
+    Dropless training steps (a gate with ``capacity_factor=0``) are capturable too: on one GPU they run on the
+    expert-packed layout (ops/packed.py), whose buffer shapes are static bounds and whose offsets stay on the device.
     The reference's step cannot be captured at all: its dispatch reads the capacity back to the host every forward
     (tutel/impls/fast_dispatch.py:192-193).
     """
