@@ -145,6 +145,8 @@ class GroupedLinear(torch.autograd.Function):
     def backward(ctx: Any, dy: torch.Tensor):
         x, w = ctx.saved_tensors
         dy = dy if _ok_stride(dy) else dy.contiguous()
+        if ctx.row_counts is not None:      # rows past the counts are not tokens: keep them out of dw and db
+            dy = _zero_tail(dy, ctx.row_counts)
         kn = ctx.w_layout == 'kn'
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
