@@ -298,10 +298,28 @@ const int* packed_seg_off(const c10::optional<at::Tensor>& seg_off, int64_t E) {
   return seg_off->data_ptr<int>();
 }
 
-// buf [E*C, M] (seg_off: [R, M]); gates float [k, S] or None; idx/loc int [k, S]; returns [S, M]
-at::Tensor decode_rows_packed(const at::Tensor& buf, const c10::optional<at::Tensor>& gates, const at::Tensor& idx,
+// Shared experts' terms of the combine: base [S, M] of `like`'s dtype; shared_logit float [S] or None.
+const void* shared_base(const c10::optional<at::Tensor>& base, const at::Tensor& like, int S, int64_t M) {
+  if (!base.has_value() || !base->defined()) return nullptr;
+  TORCH_CHECK(base->is_cuda() && base->is_contiguous() && base->scalar_type() == like.scalar_type() && base->dim() == 2 &&
+                  base->size(0) == S && base->size(1) == M,
+              "tutel_b200: the shared experts' output must be a contiguous [S, M] tensor of the routed buffer's dtype");
+  return base->data_ptr();
+}
+
+const float* shared_logits(const c10::optional<at::Tensor>& shared_logit, int S) {
+  if (!shared_logit.has_value() || !shared_logit->defined()) return nullptr;
+  TORCH_CHECK(shared_logit->is_cuda() && shared_logit->scalar_type() == at::kFloat && shared_logit->is_contiguous() &&
+                  shared_logit->numel() == S, "tutel_b200: shared_logit must be a contiguous float [S]");
+  return shared_logit->data_ptr<float>();
+}
+
+// buf [E*C, M] (seg_off: [R, M]); gates float [k, S] or None; idx/loc int [k, S]; returns [S, M].
+// base / shared_logit: the shared experts' output and gate logits (see tb::decode_rows), or None.
+at::Tensor decode_rows_shared(const at::Tensor& buf, const c10::optional<at::Tensor>& gates, const at::Tensor& idx,
                               const at::Tensor& loc, int64_t E, int64_t C, int64_t wait_flags, int64_t wait_target,
-                              const c10::optional<at::Tensor>& seg_off) {
+                              const c10::optional<at::Tensor>& seg_off, const c10::optional<at::Tensor>& base,
+                              const c10::optional<at::Tensor>& shared_logit) {
   TORCH_CHECK(buf.is_cuda() && buf.is_contiguous() && idx.is_cuda() && loc.is_cuda());
   TORCH_CHECK(idx.scalar_type() == at::kInt && loc.scalar_type() == at::kInt && idx.is_contiguous() && loc.is_contiguous());
   const c10::cuda::CUDAGuard guard(buf.device());
@@ -311,17 +329,29 @@ at::Tensor decode_rows_packed(const at::Tensor& buf, const c10::optional<at::Ten
     TORCH_CHECK(buf.dim() == 2, "decode_rows: a packed buffer is [R, M]");
     C = buf.size(0);
   }
-  const int M = static_cast<int>(buf.numel() / (so != nullptr ? C : E * C));
+  const int64_t rows = so != nullptr ? C : E * C;
+  const bool has_base = base.has_value() && base->defined();
+  // (an empty buffer, C = 0, takes the width from the shared experts' output or its own last dim)
+  const int M = static_cast<int>(rows > 0 ? buf.numel() / rows : (has_base ? base->size(-1) : buf.size(-1)));
   const void* g = nullptr;
   if (gates.has_value() && gates->defined()) {
     TORCH_CHECK(gates->is_cuda() && gates->scalar_type() == at::kFloat && gates->is_contiguous());
     g = gates->data_ptr();
   }
+  const void* b = shared_base(base, buf, S, M);
+  const float* sl = shared_logits(shared_logit, S);
+  TORCH_CHECK(sl == nullptr || b != nullptr, "decode_rows: shared_logit needs the shared experts' output");
   at::Tensor out = at::empty({S, M}, buf.options());
   TB_CHECK_CUDA(tb::decode_rows(buf.data_ptr(), g, idx.data_ptr<int>(), loc.data_ptr<int>(), out.data_ptr(),
                                 reinterpret_cast<const uint32_t*>(wait_flags), static_cast<uint32_t>(wait_target), S,
-                                static_cast<int>(E), k, static_cast<int>(C), M, elem_type_of(buf), cur_stream(), so));
+                                static_cast<int>(E), k, static_cast<int>(C), M, elem_type_of(buf), cur_stream(), so, b, sl));
   return out;
+}
+
+at::Tensor decode_rows_packed(const at::Tensor& buf, const c10::optional<at::Tensor>& gates, const at::Tensor& idx,
+                              const at::Tensor& loc, int64_t E, int64_t C, int64_t wait_flags, int64_t wait_target,
+                              const c10::optional<at::Tensor>& seg_off) {
+  return decode_rows_shared(buf, gates, idx, loc, E, C, wait_flags, wait_target, seg_off, c10::nullopt, c10::nullopt);
 }
 
 at::Tensor decode_rows(const at::Tensor& buf, const c10::optional<at::Tensor>& gates, const at::Tensor& idx,
@@ -351,6 +381,41 @@ at::Tensor gate_grad_packed(const at::Tensor& a, const at::Tensor& buf, const at
 at::Tensor gate_grad(const at::Tensor& a, const at::Tensor& buf, const at::Tensor& idx, const at::Tensor& loc,
                      int64_t E, int64_t C) {
   return gate_grad_packed(a, buf, idx, loc, E, C, c10::nullopt);
+}
+
+// Gated shared experts: a [S, M] (dy of the combine), buf as gate_grad (None when idx / loc are [0, S]), base [S, M],
+// shared_logit float [S] -> [dgate float [k, S], d_base [S, M] = w * a, d_shared_logit float [S]], one launch.
+std::vector<at::Tensor> gate_grad_shared(const at::Tensor& a, const c10::optional<at::Tensor>& buf, const at::Tensor& idx,
+                                         const at::Tensor& loc, int64_t E, int64_t C,
+                                         const c10::optional<at::Tensor>& seg_off, const at::Tensor& base,
+                                         const at::Tensor& shared_logit) {
+  TORCH_CHECK(a.is_cuda() && a.is_contiguous() && a.dim() == 2);
+  TORCH_CHECK(idx.scalar_type() == at::kInt && loc.scalar_type() == at::kInt && idx.is_contiguous() && loc.is_contiguous());
+  const c10::cuda::CUDAGuard guard(a.device());
+  const int k = static_cast<int>(idx.size(0)), S = static_cast<int>(idx.size(1));
+  TORCH_CHECK(a.size(0) == S, "gate_grad: a is [S, M]");
+  const void* bp = nullptr;
+  const int* so = nullptr;
+  if (k > 0) {
+    TORCH_CHECK(buf.has_value() && buf->defined() && buf->is_cuda() && buf->is_contiguous() &&
+                    buf->scalar_type() == a.scalar_type(), "gate_grad: the routed buffer is required when k > 0");
+    so = packed_seg_off(seg_off, E);
+    if (so != nullptr) {
+      TORCH_CHECK(buf->dim() == 2 && buf->size(1) == a.size(1), "gate_grad: a packed buffer is [R, M]");
+      C = buf->size(0);
+    }
+    bp = buf->data_ptr();
+  }
+  const void* b = shared_base(base, a, S, a.size(1));
+  const float* sl = shared_logits(shared_logit, S);
+  TORCH_CHECK(b != nullptr && sl != nullptr, "gate_grad: base and shared_logit are required");
+  at::Tensor dgate = at::empty({k, S}, a.options().dtype(at::kFloat));
+  at::Tensor d_base = at::empty_like(a);
+  at::Tensor d_logit = at::empty({S}, a.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::gate_grad(a.data_ptr(), bp, idx.data_ptr<int>(), loc.data_ptr<int>(), k > 0 ? dgate.data_ptr() : nullptr,
+                              S, static_cast<int>(E), k, static_cast<int>(C), static_cast<int>(a.size(1)), elem_type_of(a),
+                              cur_stream(), so, b, sl, d_base.data_ptr(), d_logit.data_ptr<float>()));
+  return {dgate, d_base, d_logit};
 }
 
 // Expert-packed layout (see tb::packed_layout): idx / loc int [k, S], counts int [E], R rows ->
@@ -924,8 +989,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("encode_rows_fp8", &encode_rows_fp8);
   m.def("decode_rows", &decode_rows);
   m.def("decode_rows", &decode_rows_packed);
+  m.def("decode_rows", &decode_rows_shared);
   m.def("gate_grad", &gate_grad);
   m.def("gate_grad", &gate_grad_packed);
+  m.def("gate_grad", &gate_grad_shared);
   m.def("packed_layout", &packed_layout);
   m.def("gate_route_forward", &gate_route_forward);
   m.def("gate_route_backward", &gate_route_backward);

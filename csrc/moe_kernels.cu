@@ -360,17 +360,31 @@ encode_rows_kernel(const T* __restrict__ x, const float* __restrict__ gates, con
 // ------------------------------------------------------------------------------------------------
 constexpr int kMaxK = 16;
 
-template <typename T, bool VEC, bool SEG>
+// Weight of the shared experts' output in the combine: sigmoid(logit) in fp32 (IEEE division and expf, no fast-math
+// intrinsics; a logit below about -88 gives exp = inf and weight 0).
+__device__ __forceinline__ float shared_weight(float logit) { return 1.0f / (1.0f + expf(-logit)); }
+
+// SH: shared experts.  After the routed fmaf chain (unchanged, choice order) one more fmaf adds w_s * base[s] with
+// w_s = 1 or shared_weight(shared_logit[s]); the sum is rounded to T once.  A token whose choices were all dropped gets
+// the shared term alone.
+template <typename T, bool VEC, bool SEG, bool SH>
 __global__ void __launch_bounds__(256)
 decode_rows_kernel(const T* __restrict__ buf, const float* __restrict__ gates, const int* __restrict__ idx,
                    const int* __restrict__ loc, T* __restrict__ out, const uint32_t* __restrict__ wait_flags,
-                   uint32_t wait_target, int S, int E, int k, int C, int M, const int* __restrict__ seg_off) {
+                   uint32_t wait_target, int S, int E, int k, int C, int M, const int* __restrict__ seg_off,
+                   const T* __restrict__ base, const float* __restrict__ shared_logit) {
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   for (long long s = static_cast<long long>(blockIdx.x) * 8 + warp; s < S; s += static_cast<long long>(gridDim.x) * 8) {
     const T* rows[kMaxK];
     float w[kMaxK];
     int nsel = 0;
+    const T* brow = nullptr;
+    float ws = 1.0f;
+    if constexpr (SH) {
+      brow = base + s * M;
+      if (shared_logit != nullptr) ws = shared_weight(shared_logit[s]);
+    }
     for (int j = 0; j < k; ++j) {
       const int e = idx[static_cast<long long>(j) * S + s];
       const int l = loc[static_cast<long long>(j) * S + s];
@@ -408,6 +422,17 @@ decode_rows_kernel(const T* __restrict__ buf, const float* __restrict__ gates, c
             }
           }
         }
+        if constexpr (SH) {
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            if (v0 + 32 * u < nv) {
+              float f[Vec<T>::N];
+              Vec<T>::unpack(ptx::ld_v4(reinterpret_cast<const uint4*>(brow) + v0 + 32 * u), f);
+#pragma unroll
+              for (int q = 0; q < Vec<T>::N; ++q) acc[u][q] = fmaf(ws, f[q], acc[u][q]);
+            }
+          }
+        }
 #pragma unroll
         for (int u = 0; u < 2; ++u)
           if (v0 + 32 * u < nv) ptx::st_na_v4(reinterpret_cast<uint4*>(orow) + v0 + 32 * u, Vec<T>::pack(acc[u]));
@@ -416,17 +441,22 @@ decode_rows_kernel(const T* __restrict__ buf, const float* __restrict__ gates, c
       for (int m = lane; m < M; m += 32) {
         float acc = 0.0f;
         for (int t = 0; t < nsel; ++t) acc = fmaf(w[t], to_f<T>(rows[t][m]), acc);
+        if constexpr (SH) acc = fmaf(ws, to_f<T>(brow[m]), acc);
         orow[m] = from_f<T>(acc);
       }
     }
   }
 }
 
-template <typename T, bool VEC, bool SEG>
+// SH: gated shared experts.  In the same pass over the tokens: d_base[s] = w_s * a[s] (rounded to T) and
+// d_shared_logit[s] = w_s (1 - w_s) <a[s], base[s]>, w_s = shared_weight(shared_logit[s]).  k may be 0 (pre-scored
+// routing, whose combine has no gate gradient): then only the shared terms are computed.
+template <typename T, bool VEC, bool SEG, bool SH>
 __global__ void __launch_bounds__(256)
 gate_grad_kernel(const T* __restrict__ a, const T* __restrict__ buf, const int* __restrict__ idx,
                  const int* __restrict__ loc, float* __restrict__ dgate, int S, int E, int k, int C, int M,
-                 const int* __restrict__ seg_off) {
+                 const int* __restrict__ seg_off, const T* __restrict__ base, const float* __restrict__ shared_logit,
+                 T* __restrict__ d_base, float* __restrict__ d_shared_logit) {
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   for (long long s = static_cast<long long>(blockIdx.x) * 8 + warp; s < S; s += static_cast<long long>(gridDim.x) * 8) {
@@ -453,6 +483,35 @@ gate_grad_kernel(const T* __restrict__ a, const T* __restrict__ buf, const int* 
         for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
       }
       if (lane == 0) dgate[static_cast<long long>(j) * S + s] = acc;
+    }
+    if constexpr (SH) {
+      const float ws = shared_weight(shared_logit[s]);
+      const T* brow = base + s * M;
+      T* drow = d_base + s * M;
+      float acc = 0.0f;
+      if constexpr (VEC) {
+        const int nv = M / Vec<T>::N;
+        for (int v = lane; v < nv; v += 32) {
+          float fa[Vec<T>::N], fb[Vec<T>::N];
+          Vec<T>::unpack(ptx::ld_v4(reinterpret_cast<const uint4*>(arow) + v), fa);
+          Vec<T>::unpack(ptx::ld_v4(reinterpret_cast<const uint4*>(brow) + v), fb);
+#pragma unroll
+          for (int q = 0; q < Vec<T>::N; ++q) {
+            acc = fmaf(fa[q], fb[q], acc);
+            fa[q] *= ws;
+          }
+          ptx::st_na_v4(reinterpret_cast<uint4*>(drow) + v, Vec<T>::pack(fa));
+        }
+      } else {
+        for (int m = lane; m < M; m += 32) {
+          const float fa = to_f<T>(arow[m]);
+          acc = fmaf(fa, to_f<T>(brow[m]), acc);
+          drow[m] = from_f<T>(fa * ws);
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+      if (lane == 0) d_shared_logit[s] = ws * (1.0f - ws) * acc;
     }
   }
 }
@@ -848,61 +907,77 @@ cudaError_t quantize_transpose_e4m3(const void* x, void* qT, float* scale, float
   return cudaGetLastError();
 }
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 template <typename T>
 static cudaError_t decode_rows_t(const void* buf, const void* gates, const int* idx, const int* loc, void* out,
                                  const uint32_t* wait_flags, uint32_t wait_target, int S, int E, int k, int C, int M,
-                                 const int* seg_off, cudaStream_t stream) {
+                                 const int* seg_off, const void* base, const float* shared_logit, cudaStream_t stream) {
   if (S <= 0 || M <= 0) return cudaSuccess;
   if (k > kMaxK) return cudaErrorInvalidValue;
+  if (base == nullptr && shared_logit != nullptr) return cudaErrorInvalidValue;
   const long long want = (static_cast<long long>(S) + 7) / 8;
   const int grid = static_cast<int>(want < 8LL * num_sms() ? want : 8LL * num_sms());
-  const bool vec = (M % Vec<T>::N == 0) && ((reinterpret_cast<uintptr_t>(buf) & 15) == 0) &&
-                   ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
-  // (expert-packed buffers run their own instantiations: the padded ones keep their address arithmetic)
-#define TB_DEC(VECv, SEGv)                                                                                            \
-  decode_rows_kernel<T, VECv, SEGv><<<grid, 256, 0, stream>>>(static_cast<const T*>(buf), static_cast<const float*>(gates), \
-                                                              idx, loc, static_cast<T*>(out), wait_flags, wait_target, S,  \
-                                                              E, k, C, M, seg_off)
-  if (seg_off != nullptr) { if (vec) TB_DEC(true, true); else TB_DEC(false, true); }
-  else { if (vec) TB_DEC(true, false); else TB_DEC(false, false); }
+  const bool vec = (M % Vec<T>::N == 0) && aligned16(buf) && aligned16(out) && (base == nullptr || aligned16(base));
+  // (expert-packed buffers and the shared-expert term run their own instantiations: the padded combine without shared
+  // experts keeps its code)
+#define TB_DEC(VECv, SEGv, SHv)                                                                                         \
+  decode_rows_kernel<T, VECv, SEGv, SHv><<<grid, 256, 0, stream>>>(                                                     \
+      static_cast<const T*>(buf), static_cast<const float*>(gates), idx, loc, static_cast<T*>(out), wait_flags,          \
+      wait_target, S, E, k, C, M, seg_off, static_cast<const T*>(base), shared_logit)
+#define TB_DEC_SEG(VECv, SHv) \
+  if (seg_off != nullptr) TB_DEC(VECv, true, SHv); else TB_DEC(VECv, false, SHv)
+  if (base != nullptr) { if (vec) TB_DEC_SEG(true, true); else TB_DEC_SEG(false, true); }
+  else { if (vec) TB_DEC_SEG(true, false); else TB_DEC_SEG(false, false); }
+#undef TB_DEC_SEG
 #undef TB_DEC
   return cudaGetLastError();
 }
 
 cudaError_t decode_rows(const void* buf, const void* gates, const int* idx, const int* loc, void* out,
                         const uint32_t* wait_flags, uint32_t wait_target, int S, int E, int k, int C, int M,
-                        int elem_type, cudaStream_t stream, const int* seg_off) {
+                        int elem_type, cudaStream_t stream, const int* seg_off, const void* base,
+                        const float* shared_logit) {
   switch (elem_type) {
-    case ET_F32: return decode_rows_t<float>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, stream);
-    case ET_F16: return decode_rows_t<__half>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, stream);
-    case ET_BF16: return decode_rows_t<__nv_bfloat16>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, stream);
+    case ET_F32: return decode_rows_t<float>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, base, shared_logit, stream);
+    case ET_F16: return decode_rows_t<__half>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, base, shared_logit, stream);
+    case ET_BF16: return decode_rows_t<__nv_bfloat16>(buf, gates, idx, loc, out, wait_flags, wait_target, S, E, k, C, M, seg_off, base, shared_logit, stream);
   }
   return cudaErrorInvalidValue;
 }
 
 template <typename T>
 static cudaError_t gate_grad_t(const void* a, const void* buf, const int* idx, const int* loc, void* dgate, int S, int E,
-                               int k, int C, int M, const int* seg_off, cudaStream_t stream) {
+                               int k, int C, int M, const int* seg_off, const void* base, const float* shared_logit,
+                               void* d_base, float* d_shared_logit, cudaStream_t stream) {
   if (S <= 0) return cudaSuccess;
+  const bool sh = shared_logit != nullptr;
+  if (sh && (base == nullptr || d_base == nullptr || d_shared_logit == nullptr)) return cudaErrorInvalidValue;
+  if (k > 0 && (buf == nullptr || dgate == nullptr)) return cudaErrorInvalidValue;
   const long long want = (static_cast<long long>(S) + 7) / 8;
   const int grid = static_cast<int>(want < 8LL * num_sms() ? want : 8LL * num_sms());
-  const bool vec = (M % Vec<T>::N == 0) && ((reinterpret_cast<uintptr_t>(a) & 15) == 0) &&
-                   ((reinterpret_cast<uintptr_t>(buf) & 15) == 0);
-#define TB_GG(VECv, SEGv)                                                                                             \
-  gate_grad_kernel<T, VECv, SEGv><<<grid, 256, 0, stream>>>(static_cast<const T*>(a), static_cast<const T*>(buf), idx, loc, \
-                                                            static_cast<float*>(dgate), S, E, k, C, M, seg_off)
-  if (seg_off != nullptr) { if (vec) TB_GG(true, true); else TB_GG(false, true); }
-  else { if (vec) TB_GG(true, false); else TB_GG(false, false); }
+  const bool vec = (M % Vec<T>::N == 0) && aligned16(a) && aligned16(buf) &&
+                   (!sh || (aligned16(base) && aligned16(d_base)));
+#define TB_GG(VECv, SEGv, SHv)                                                                                          \
+  gate_grad_kernel<T, VECv, SEGv, SHv><<<grid, 256, 0, stream>>>(                                                       \
+      static_cast<const T*>(a), static_cast<const T*>(buf), idx, loc, static_cast<float*>(dgate), S, E, k, C, M,         \
+      seg_off, static_cast<const T*>(base), shared_logit, static_cast<T*>(d_base), d_shared_logit)
+#define TB_GG_SEG(VECv, SHv) \
+  if (seg_off != nullptr) TB_GG(VECv, true, SHv); else TB_GG(VECv, false, SHv)
+  if (sh) { if (vec) TB_GG_SEG(true, true); else TB_GG_SEG(false, true); }
+  else { if (vec) TB_GG_SEG(true, false); else TB_GG_SEG(false, false); }
+#undef TB_GG_SEG
 #undef TB_GG
   return cudaGetLastError();
 }
 
 cudaError_t gate_grad(const void* a, const void* buf, const int* idx, const int* loc, void* dgate, int S, int E, int k,
-                      int C, int M, int elem_type, cudaStream_t stream, const int* seg_off) {
+                      int C, int M, int elem_type, cudaStream_t stream, const int* seg_off, const void* base,
+                      const float* shared_logit, void* d_base, float* d_shared_logit) {
   switch (elem_type) {
-    case ET_F32: return gate_grad_t<float>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, stream);
-    case ET_F16: return gate_grad_t<__half>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, stream);
-    case ET_BF16: return gate_grad_t<__nv_bfloat16>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, stream);
+    case ET_F32: return gate_grad_t<float>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, base, shared_logit, d_base, d_shared_logit, stream);
+    case ET_F16: return gate_grad_t<__half>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, base, shared_logit, d_base, d_shared_logit, stream);
+    case ET_BF16: return gate_grad_t<__nv_bfloat16>(a, buf, idx, loc, dgate, S, E, k, C, M, seg_off, base, shared_logit, d_base, d_shared_logit, stream);
   }
   return cudaErrorInvalidValue;
 }

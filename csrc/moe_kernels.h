@@ -43,13 +43,22 @@ cudaError_t encode_rows_fp8(const void* x, const void* gates, const int* slot_sr
 // wait_flags (optional): uint32[E] counters that must reach wait_target (acquire.sys) before expert e's rows
 // are read (combine fusion).
 // seg_off (optional, int[E]): expert-packed buffer, the row of (e, l) is seg_off[e] + l instead of e*C + l.
+// base (optional, [S, M] of the buffer's type, 16-byte aligned rows for the vector path): shared experts' output, added
+// after the routed terms as out[s] = T(fmaf(w_s, base[s], routed fp32 sum)) - one rounding - with w_s = 1, or
+// sigmoid(shared_logit[s]) in fp32 when shared_logit (optional, fp32 [S]) is given.
 cudaError_t decode_rows(const void* buf, const void* gates, const int* idx, const int* loc, void* out,
                         const uint32_t* wait_flags, uint32_t wait_target, int S, int E, int k, int C, int M,
-                        int elem_type, cudaStream_t stream, const int* seg_off = nullptr);
+                        int elem_type, cudaStream_t stream, const int* seg_off = nullptr, const void* base = nullptr,
+                        const float* shared_logit = nullptr);
 
 // dgate[j*S + s] = dot(a[s, :], buf[slot_j(s), :])   (fp32 accumulate, 0 for dropped choices).  seg_off: as decode_rows.
+// Gated shared experts (shared_logit fp32 [S] given; base, d_base [S, M] of a's type; d_shared_logit fp32 [S]), in the same
+// launch: d_base[s] = T(w_s * a[s]), d_shared_logit[s] = w_s (1 - w_s) dot(a[s], base[s]), w_s = sigmoid(shared_logit[s]).
+// k may then be 0 (buf and dgate unused).
 cudaError_t gate_grad(const void* a, const void* buf, const int* idx, const int* loc, void* dgate, int S, int E,
-                      int k, int C, int M, int elem_type, cudaStream_t stream, const int* seg_off = nullptr);
+                      int k, int C, int M, int elem_type, cudaStream_t stream, const int* seg_off = nullptr,
+                      const void* base = nullptr, const float* shared_logit = nullptr, void* d_base = nullptr,
+                      float* d_shared_logit = nullptr);
 
 // Expert-packed layout of R rows (R % 128 == 0, R >= sum_e roundup128(counts[e])), from device counts[E] with no host
 // read: seg_off[E + 1] = exclusive scan of roundup128(counts), block_expert / block_rows [R / 128] = the expert and the

@@ -20,10 +20,11 @@ def expert_param_keys(state: Dict[str, Any], prefix: str) -> List[str]:
 
 
 def legacy_prefixes(state: Dict[str, Any]) -> List[str]:
-    """Layers saved before `_num_global_experts` existed: detected through their `experts.batched_fc1_w` tensor."""
+    """Layers saved before `_num_global_experts` existed: detected through their `experts.batched_fc1_w` tensor.  (A
+    prefix is empty or ends with a dot: a layer's replicated `shared_experts.*` tensors are not a legacy layer.)"""
     out = set()
     for k in state:
-        m = re.match(r'^(.*?)experts\.[^.]+$', k)
+        m = re.match(r'^((?:.*\.)?)experts\.[^.]+$', k)
         if m and (m.group(1) + '_num_global_experts') not in state:
             out.add(m.group(1))
     return sorted(out)

@@ -33,6 +33,7 @@ def base_parser(**defaults):
     p.add_argument('--eval', default=False, action='store_true')
     p.add_argument('--capacity_factor', type=float, default=1.0)
     p.add_argument('--cap_factor', type=float, default=1.0)
+    p.add_argument('--num_shared_experts', type=int, default=0)    # > 0: shared experts (n x hidden_size), weight 1
     p.set_defaults(**defaults)
     return p
 
@@ -144,5 +145,7 @@ def default_layer(session, **overrides):
         parallel_type=a.parallel_type,
         use_2dh=a.use_2dh,
     )
+    if getattr(a, 'num_shared_experts', 0) > 0:
+        kw['shared_experts'] = {'num_experts': a.num_shared_experts}
     kw.update(overrides)
     return tutel_moe.moe_layer(**kw)

@@ -117,7 +117,14 @@ class MOELayer(torch.nn.Module):
     # -------------------------------------------------------------------------------------------- construction
     def __init__(self, gate_type, model_dim: int, experts=None, scan_expert_func=None, result_func=None, group=None,
                  seeds=None, a2a_ffn_overlap_degree=1, is_postscore=True, batch_prioritized_routing=False,
-                 normalize_gate=True, is_gshard_loss=True, parallel_type='adaptive:1', use_2dh=False, **kwargs):
+                 normalize_gate=True, is_gshard_loss=True, parallel_type='adaptive:1', use_2dh=False, shared_experts=None,
+                 **kwargs):
+        """``shared_experts`` (optional): ``{'num_experts': n}`` adds shared experts that every token passes through,
+        added to the routed output with weight 1 (DeepSeek-V2/V3, Kimi-K2, GLM-4.5, Moonlight, Llama-4).  n experts of
+        ``hidden_size_per_expert`` H that are always selected with weight 1 are one dense expert of hidden size nH, of the
+        routed experts' type (``ffn`` or ``llama_ffn``) and options, replicated on every rank: ``shared_experts.*``.
+        ``'gate': True`` adds ``shared_expert_gate`` (``Linear(model_dim, 1, bias=False)``) and scales the shared output
+        by sigmoid(x . w) per token (Qwen1.5/2-MoE).  The shared term is added inside the combine kernel."""
         super().__init__()
         assert model_dim % 2 == 0, 'Model_dim (%s) must be even value, while this Model_dim mod 2 > 0.' % model_dim
         if 'pad_samples' in kwargs:
@@ -135,6 +142,7 @@ class MOELayer(torch.nn.Module):
         self.world_size = C.get_world_size(self.group)
 
         experts = dict(experts or {})
+        shared_spec = self._shared_spec(shared_experts, experts)
         local = experts.pop('count_per_node', None)
         local2 = experts.pop('num_experts_per_device', None)
         self.num_local_experts = local if local is not None else (local2 if local2 is not None else 1)
@@ -166,7 +174,7 @@ class MOELayer(torch.nn.Module):
         # ---- experts (RNG: seeds[1]) ----
         if seeds is not None and seeds[1] is not None:
             torch.manual_seed(seeds[1])
-        self.experts = self._build_experts(experts)
+        self.experts = self._build_experts(dict(experts))
         if scan_expert_func is not None:
             for n, p in self.experts.named_parameters():
                 scan_expert_func(n, p)
@@ -194,14 +202,45 @@ class MOELayer(torch.nn.Module):
                                      'loss is defined on softmax scores')
                 gate.balance_group = self.group
 
+        # ---- shared experts (after the gates: the RNG stream of the experts and gates is unchanged; replicated
+        # parameters, so with `seeds` they draw from the gates' stream, which is the same on every rank) ----
+        self.shared_experts, self.shared_expert_gate = None, None
+        if shared_spec is not None:
+            spec = dict(experts, hidden_size_per_expert=experts['hidden_size_per_expert'] * shared_spec['num_experts'])
+            self.shared_experts = self._build_experts(spec, num_experts_per_device=1, sharded_count=1)
+            if shared_spec.get('gate', False):
+                self.shared_expert_gate = torch.nn.Linear(model_dim, 1, bias=False)
+
         if seeds is not None and len(seeds) > 2 and seeds[2] is not None:
             torch.manual_seed(seeds[2])
 
-    def _build_experts(self, experts: dict):
+    @staticmethod
+    def _shared_spec(shared_experts, experts: dict):
+        """Validated ``shared_experts`` option, or None."""
+        if shared_experts is None:
+            return None
+        if not isinstance(shared_experts, dict):
+            raise ValueError("shared_experts must be None or a dict like {'num_experts': 2, 'gate': False}")
+        unknown = set(shared_experts) - {'num_experts', 'gate'}
+        if unknown:
+            raise ValueError('Unrecognized shared_experts option(s): %s' % sorted(unknown))
+        n = shared_experts.get('num_experts')
+        if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+            raise ValueError('shared_experts: num_experts must be a positive int (got %r)' % (n,))
+        kind = experts.get('type')
+        if kind == 'custom':
+            raise ValueError('shared_experts are not supported with custom experts: their hidden size cannot be derived')
+        if kind not in ('ffn', 'llama_ffn'):
+            raise ValueError("shared_experts need 'ffn' or 'llama_ffn' experts (got %r)" % (kind,))
+        if 'hidden_size_per_expert' not in experts:
+            raise ValueError('shared_experts need the routed experts\' hidden_size_per_expert')
+        return dict(shared_experts)
+
+    def _build_experts(self, experts: dict, num_experts_per_device=None, sharded_count=None):
         kind = experts.pop('type')
         experts['model_dim'] = self.model_dim
-        experts['num_experts_per_device'] = self.num_local_experts
-        experts['sharded_count'] = self.sharded_count
+        experts['num_experts_per_device'] = self.num_local_experts if num_experts_per_device is None else num_experts_per_device
+        experts['sharded_count'] = self.sharded_count if sharded_count is None else sharded_count
         if kind == 'custom':
             factory = experts.pop('module')
         else:
@@ -248,7 +287,11 @@ class MOELayer(torch.nn.Module):
             return self.gates.named_parameters()
         if param_type == 'local_experts':
             return self.experts.named_parameters()
-        raise Exception('Specified parameter type is not recognized: %s. Valid `param_type` includes: gate, local_experts.' % param_type)
+        if param_type == 'shared_experts':
+            mods = [m for m in (self.shared_experts, self.shared_expert_gate) if m is not None]
+            return torch.nn.ModuleList(mods).named_parameters()
+        raise Exception('Specified parameter type is not recognized: %s. Valid `param_type` includes: gate, local_experts, '
+                        'shared_experts.' % param_type)
 
     # ------------------------------------------------------------------------------------------------- forward
     def expert_local(self, x, reserve_shape):
@@ -359,6 +402,9 @@ class MOELayer(torch.nn.Module):
             out = input
             out.l_aux = None
             return self.result_func(out) if self.result_func is not None else out
+        if self.shared_experts is not None and reserve_dims != 1:
+            raise ValueError('shared_experts need reserve_dims=1 (got %d): the shared experts run on [tokens, model_dim]'
+                             % reserve_dims)
 
         # Let go of the previous call's auxiliary loss BEFORE building a new autograd graph: it is the one tensor of a step
         # that outlives it, and through it the gate weight's gradient accumulator - which remembers the stream it was
@@ -401,13 +447,17 @@ class MOELayer(torch.nn.Module):
             self.adaptive_degree = adaptive_r
 
         x = x.contiguous()
+        base, shared_logit = None, None
+        if self.shared_experts is not None:
+            with stage('shared'):
+                base, shared_logit = self._shared_forward(x)
         y = None
         fused = None if packed else self._fused_engine(x, crit, d, reserve_dims)
         if packed:
-            y = self._packed_forward(x, crit)
+            y = self._packed_forward(x, crit, base, shared_logit)
         elif fused is not None:
             with stage('fused'):
-                y = fused.run(self, x, crit)
+                y = fused.run(self, x, crit, base, shared_logit)
             self.protected_shape = y.shape
         else:
             with stage('encode'):
@@ -439,7 +489,7 @@ class MOELayer(torch.nn.Module):
                     else:
                         y = y.view(self.num_global_experts, -1, y.size(2))
             with stage('decode'):
-                y = fast_decode(y.contiguous(), crit, self.is_postscore)
+                y = fast_decode(y.contiguous(), crit, self.is_postscore, base, shared_logit)
 
         y = y.view(list(original_shape[:-reserve_dims]) + list(self.protected_shape[-reserve_dims:])).to(original_dtype)
         self.l_aux = y.l_aux = l_aux
@@ -462,7 +512,7 @@ class MOELayer(torch.nn.Module):
         from ..ops import backend
         return backend.has_cuda_ext()
 
-    def _packed_forward(self, x, crit):
+    def _packed_forward(self, x, crit, base=None, shared_logit=None):
         from ..ops.dispatch import DispatchPlan, GatingDecoder, GatingEncoder
         plan = DispatchPlan.from_critical(crit)
         with stage('encode'):
@@ -471,8 +521,32 @@ class MOELayer(torch.nn.Module):
             y = self.experts.forward_packed(y, crit.layout, self)
         self.protected_shape = y.shape
         with stage('decode'):
-            y = GatingDecoder.apply(plan, y, crit.gates_ks if self.is_postscore else None)
+            gates = crit.gates_ks if self.is_postscore else None
+            if base is None:
+                y = GatingDecoder.apply(plan, y, gates)
+            else:
+                y = GatingDecoder.apply(plan, y, gates, base, shared_logit)
         return y
+
+    # ------------------------------------------------------------------------------------------------ shared experts
+    def _shared_forward(self, x):
+        """(shared experts' output [S, Mout], shared-gate logits [S] or None) for the tokens x [S, M].  The expert runs
+        on x viewed as one expert's [1, S, M] block; no-grad forwards of up to 64 tokens on CUDA give it a device row
+        count of S, so that it takes the dropless decoding kernels of its type (the weight-streaming skinny kernels)."""
+        S = x.size(0)
+        rows = _shared_rows(S, x.device) if (x.is_cuda and 0 < S <= 64 and not torch.is_grad_enabled()) else None
+        base = self.shared_experts(x.view(1, S, x.size(1)), _SharedExpertContext(self, rows))
+        base = base.reshape(S, -1)
+        logit = None
+        if self.shared_expert_gate is not None:
+            w = self.shared_expert_gate.weight
+            if x.is_cuda or x.device.type == 'cpu':           # the gate's rules (forward: _route runs without autocast)
+                with torch.amp.autocast(x.device.type, enabled=False):
+                    logit = F.linear(x.to(w.dtype), w)
+            else:
+                logit = F.linear(x.to(w.dtype), w)
+            logit = logit.view(S)
+        return base, logit
 
     # ------------------------------------------------------------------------------------------- fused engine
     def _fused_engine(self, x, crit, d, reserve_dims):
@@ -481,6 +555,36 @@ class MOELayer(torch.nn.Module):
             return None
         from ..parallel import fused
         return fused.engine_for(self, x, crit, d)
+
+
+class _SharedExpertContext:
+    """What an expert module reads from its layer, for the shared experts: one dense expert, not sharded, in this
+    rank's replica.  ``rows`` (device int32 [1] or None) turns on the expert's dropless decoding path."""
+
+    def __init__(self, layer: MOELayer, rows: Optional[Tensor]):
+        self.group = layer.group
+        self.model_dim = layer.model_dim
+        self.num_global_experts = 1
+        self.num_local_experts = 1
+        self.sharded_count = 1
+        self.adaptive_degree = 1
+        self.top_k = 1
+        self.megablocks_size = 1 if rows is not None else 0
+        self.dispatch_count = rows
+
+
+_SHARED_ROWS = {}
+
+
+def _shared_rows(S: int, device) -> Tensor:
+    """int32 [1] device tensor holding S (cached per device and S; not cached while a CUDA graph is being captured)."""
+    key = (str(device), S)
+    t = _SHARED_ROWS.get(key)
+    if t is None:
+        t = torch.full([1], S, dtype=torch.int32, device=device)
+        if not torch.cuda.is_current_stream_capturing():
+            _SHARED_ROWS[key] = t
+    return t
 
 
 moe_layer = MOELayer

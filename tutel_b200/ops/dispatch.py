@@ -101,19 +101,50 @@ def raw_encode(x: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchPla
     return out.to(x.dtype)
 
 
-def raw_decode(buf: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchPlan) -> torch.Tensor:
-    """buf [E*C, M] -> [S, M];  out[s] = sum_j gate_j[s] * buf[slot_j(s)]."""
+def shared_weight(shared_logit: Optional[torch.Tensor], dtype: torch.dtype = torch.float32):
+    """Per-token weight ``[S, 1]`` of the shared experts' output: sigmoid of the shared-gate logit computed in ``dtype``
+    (fp32 as in the kernels, or fp64 for fp64 tensors), or None for weight 1."""
+    if shared_logit is None:
+        return None
+    return torch.sigmoid(shared_logit.to(dtype).view(-1, 1))
+
+
+def _add_shared(out: torch.Tensor, base: Optional[torch.Tensor], shared_logit: Optional[torch.Tensor]) -> torch.Tensor:
+    """out + w_s * base in out's (fp32 or fp64) precision: the shared term of the torch combine paths."""
+    if base is None:
+        return out
+    b = base.to(out.dtype).view_as(out)
+    ws = shared_weight(shared_logit, out.dtype)
+    return out + (b if ws is None else ws * b)
+
+
+def _shared_args(base: Optional[torch.Tensor], shared_logit: Optional[torch.Tensor]):
+    """The shared terms as the native kernels take them: contiguous base, fp32 logits [S]."""
+    b = None if base is None else base.contiguous()
+    sl = None if shared_logit is None else shared_logit.to(torch.float32).contiguous().view(-1)
+    return b, sl
+
+
+def raw_decode(buf: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchPlan, base: Optional[torch.Tensor] = None,
+               shared_logit: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """buf [E*C, M] -> [S, M];  out[s] = sum_j gate_j[s] * buf[slot_j(s)]  (+ w_s * base[s]).
+
+    ``base [S, M]`` (optional): the shared experts' output, added with weight w_s = 1, or sigmoid(shared_logit[s]) when
+    ``shared_logit [S]`` is given; on CUDA in the same launch and with one rounding (csrc/moe_kernels.cu: decode_rows)."""
     if plan.layout is not None:
         from . import packed
-        return packed.decode(buf.view(plan.layout.R, -1), gates, plan.idx_ks, plan.loc_ks, plan.layout)
+        return packed.decode(buf.view(plan.layout.R, -1), gates, plan.idx_ks, plan.loc_ks, plan.layout, base, shared_logit)
     buf = buf.contiguous().view(plan.E * plan.C, -1)
     if _native_cuda(buf):
         g = None if gates is None else gates.to(torch.float32).contiguous()
         backend.count_launch()
-        return backend.require_ext().decode_rows(buf, g, plan.idx_ks, plan.loc_ks, plan.E, plan.C, 0, 0)
+        if base is None:
+            return backend.require_ext().decode_rows(buf, g, plan.idx_ks, plan.loc_ks, plan.E, plan.C, 0, 0)
+        b, sl = _shared_args(base, shared_logit)
+        return backend.require_ext().decode_rows(buf, g, plan.idx_ks, plan.loc_ks, plan.E, plan.C, 0, 0, None, b, sl)
     if _cpu_native(buf):
         g = None if gates is None else gates.to(buf.dtype).contiguous()
-        return backend.ext().cpu_decode(buf, g, plan.idx_ks, plan.loc_ks, plan.E, plan.C)
+        return _add_shared(backend.ext().cpu_decode(buf, g, plan.idx_ks, plan.loc_ks, plan.E, plan.C), base, shared_logit)
     work = buf if buf.dtype in (torch.float32, torch.float64) else buf.float()
     out = torch.zeros([plan.S, work.size(1)], dtype=work.dtype, device=buf.device)
     slot, valid = _slots(plan)
@@ -121,7 +152,35 @@ def raw_decode(buf: torch.Tensor, gates: Optional[torch.Tensor], plan: DispatchP
         rows = work.index_select(0, slot[j])
         w = valid[j].to(work.dtype) if gates is None else valid[j].to(work.dtype) * gates[j].to(work.dtype)
         out += rows * w.unsqueeze(1)
-    return out.to(buf.dtype)
+    return _add_shared(out, base, shared_logit).to(buf.dtype)
+
+
+def raw_shared_grad(a: torch.Tensor, buf: Optional[torch.Tensor], plan: DispatchPlan, base: torch.Tensor,
+                    shared_logit: torch.Tensor, routed: bool = True):
+    """Backward of a combine with gated shared experts: ``(dgate [k, S] or None, d_base [S, M], d_shared_logit [S])`` with
+    dgate as :func:`raw_gate_grad`, d_base = w_s * a[s] and d_shared_logit = w_s (1 - w_s) <a[s], base[s]> (fp32 on
+    CUDA).  On CUDA one launch computes all three; ``routed=False`` skips the routed dots (``buf`` unused)."""
+    if _native_cuda(a) and a.dtype == base.dtype and (not routed or a.dtype == buf.dtype):
+        b, sl = _shared_args(base, shared_logit)
+        a = a.contiguous()
+        seg_off = None
+        if routed and plan.layout is not None:
+            bufv, seg_off = buf.contiguous().view(plan.layout.R, -1), plan.layout.seg_off
+            E, C = plan.layout.E, plan.layout.R
+        elif routed:
+            bufv, E, C = buf.contiguous().view(plan.E * plan.C, -1), plan.E, plan.C
+        else:
+            bufv, E, C = None, plan.E, plan.C
+        idx, loc = (plan.idx_ks, plan.loc_ks) if routed else (plan.idx_ks[:0], plan.loc_ks[:0])
+        backend.count_launch()
+        dg, d_base, d_sl = backend.require_ext().gate_grad(a, bufv, idx, loc, E, C, seg_off, b, sl)
+        return (dg if routed else None), d_base, d_sl
+    dg = raw_gate_grad(a, buf, plan) if routed else None
+    work = a.double() if a.dtype == torch.float64 else a.float()
+    ws = shared_weight(shared_logit, work.dtype)
+    d_base = (ws * work).to(a.dtype)
+    d_sl = (ws * (1 - ws)).view(-1) * (work * base.to(work.dtype)).sum(1)
+    return dg, d_base, d_sl
 
 
 def raw_gate_grad(a: torch.Tensor, buf: torch.Tensor, plan: DispatchPlan) -> torch.Tensor:
@@ -169,26 +228,51 @@ class GatingEncoder(torch.autograd.Function):
 
 
 class GatingDecoder(torch.autograd.Function):
-    """expert outputs [E*C, M] (+ optional gates [k, S]) -> tokens [S, M]."""
+    """expert outputs [E*C, M] (+ optional gates [k, S]) -> tokens [S, M].
+
+    Optional shared experts: ``base [S, M]`` (their output) is added with weight 1, or sigmoid(``shared_logit [S]``)
+    per token, inside the same combine launch.  Backward: without the shared gate d_base is the output gradient itself
+    (no launch); with it, d_base and d_shared_logit come from the gate-gradient launch (with zero routed choices when
+    the routed gates were applied before the experts)."""
 
     @staticmethod
-    def forward(ctx: Any, plan: DispatchPlan, buf: torch.Tensor, gates: Optional[torch.Tensor]):
+    def forward(ctx: Any, plan: DispatchPlan, buf: torch.Tensor, gates: Optional[torch.Tensor],
+                base: Optional[torch.Tensor] = None, shared_logit: Optional[torch.Tensor] = None):
         ctx.plan = plan
         ctx.has_gates = gates is not None
-        if ctx.has_gates:
-            ctx.save_for_backward(buf, gates)
-        return raw_decode(buf, gates, plan)
+        ctx.n_inputs = 3 if base is None else 5
+        ctx.shared_gated = shared_logit is not None
+        if ctx.has_gates or ctx.shared_gated:
+            ctx.save_for_backward(buf if ctx.has_gates else None, gates, base if ctx.shared_gated else None, shared_logit)
+        return raw_decode(buf, gates, plan, base, shared_logit)
 
     @staticmethod
     def backward(ctx: Any, dout: torch.Tensor):
         plan = ctx.plan
         dout = dout.contiguous()
+        if ctx.n_inputs == 3:
+            if ctx.has_gates:
+                buf, gates = ctx.saved_tensors[:2]
+                dbuf = raw_encode(dout, gates, plan).view_as(buf)
+                dg = raw_gate_grad(dout, buf, plan).to(gates.dtype)
+                return None, dbuf, dg
+            return None, raw_encode(dout, None, plan), None
+        dg = d_logit = None
+        if ctx.shared_gated:
+            buf, gates, base, shared_logit = ctx.saved_tensors
+            dbuf = raw_encode(dout, gates, plan)
+            dg, d_base, d_logit = raw_shared_grad(dout, buf, plan, base, shared_logit, routed=ctx.has_gates)
+            d_logit = d_logit.to(shared_logit.dtype).view_as(shared_logit)
+        else:
+            gates = ctx.saved_tensors[1] if ctx.has_gates else None
+            dbuf = raw_encode(dout, gates, plan)
+            if ctx.has_gates:
+                dg = raw_gate_grad(dout, ctx.saved_tensors[0], plan)
+            d_base = dout
         if ctx.has_gates:
-            buf, gates = ctx.saved_tensors
-            dbuf = raw_encode(dout, gates, plan).view_as(buf)
-            dg = raw_gate_grad(dout, buf, plan).to(gates.dtype)
-            return None, dbuf, dg
-        return None, raw_encode(dout, None, plan), None
+            dbuf = dbuf.view_as(ctx.saved_tensors[0])
+            dg = dg.to(gates.dtype)
+        return None, dbuf, dg, d_base, d_logit
 
 
 def _stack_gates(gates_s: Sequence[torch.Tensor]) -> torch.Tensor:
@@ -225,9 +309,12 @@ class TutelMoeFastDispatcher:
         gates = None if self.is_postscore else self.gates
         return GatingEncoder.apply(self.plan, data, gates)
 
-    def decode(self, data: torch.Tensor) -> torch.Tensor:
+    def decode(self, data: torch.Tensor, base: Optional[torch.Tensor] = None,
+               shared_logit: Optional[torch.Tensor] = None) -> torch.Tensor:
         gates = self.gates if self.is_postscore else None
-        return GatingDecoder.apply(self.plan, data.reshape(self.plan.E * self.plan.C, -1), gates)
+        if base is None:
+            return GatingDecoder.apply(self.plan, data.reshape(self.plan.E * self.plan.C, -1), gates)
+        return GatingDecoder.apply(self.plan, data.reshape(self.plan.E * self.plan.C, -1), gates, base, shared_logit)
 
 
 fast_dispatcher = TutelMoeFastDispatcher
@@ -250,7 +337,9 @@ def fast_encode(data: torch.Tensor, critical_data, is_postscore: bool = True) ->
     return _dispatcher_for(data, critical_data, is_postscore).encode(data).view(E, -1, data.size(-1))
 
 
-def fast_decode(data: torch.Tensor, critical_data, is_postscore: bool = True) -> torch.Tensor:
-    """[E, C, M'] expert outputs -> [S, M'] tokens (weighted sum over the k choices)."""
+def fast_decode(data: torch.Tensor, critical_data, is_postscore: bool = True, base: Optional[torch.Tensor] = None,
+                shared_logit: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """[E, C, M'] expert outputs -> [S, M'] tokens (weighted sum over the k choices).  ``base [S, M']`` (optional): the
+    shared experts' output, added with weight 1 or sigmoid(``shared_logit [S]``) in the same combine."""
     assert data.is_contiguous(), 'Input tensor for encode/decode should be in contiguous memory format.'
-    return _dispatcher_for(data, critical_data, is_postscore).decode(data).view(-1, data.size(-1))
+    return _dispatcher_for(data, critical_data, is_postscore).decode(data, base, shared_logit).view(-1, data.size(-1))

@@ -74,11 +74,17 @@ def encode(x: torch.Tensor, gates, layout: PackedLayout) -> torch.Tensor:
     return out
 
 
-def decode(buf: torch.Tensor, gates, idx_ks: torch.Tensor, loc_ks: torch.Tensor, layout: PackedLayout) -> torch.Tensor:
-    """packed [R, M] -> [S, M]: out[s] = sum_j gate_j[s] * buf[seg_off[idx_j[s]] + loc_j[s]]."""
+def decode(buf: torch.Tensor, gates, idx_ks: torch.Tensor, loc_ks: torch.Tensor, layout: PackedLayout, base=None,
+           shared_logit=None) -> torch.Tensor:
+    """packed [R, M] -> [S, M]: out[s] = sum_j gate_j[s] * buf[seg_off[idx_j[s]] + loc_j[s]]  (+ w_s * base[s], the shared
+    experts' term of ops/dispatch.py: raw_decode)."""
     g = None if gates is None else gates.to(torch.float32).contiguous()
     backend.count_launch()
-    return backend.require_ext().decode_rows(buf.contiguous(), g, idx_ks, loc_ks, layout.E, layout.R, 0, 0, layout.seg_off)
+    if base is None:
+        return backend.require_ext().decode_rows(buf.contiguous(), g, idx_ks, loc_ks, layout.E, layout.R, 0, 0, layout.seg_off)
+    sl = None if shared_logit is None else shared_logit.to(torch.float32).contiguous().view(-1)
+    return backend.require_ext().decode_rows(buf.contiguous(), g, idx_ks, loc_ks, layout.E, layout.R, 0, 0, layout.seg_off,
+                                             base.contiguous(), sl)
 
 
 def gate_grad(a: torch.Tensor, buf: torch.Tensor, idx_ks: torch.Tensor, loc_ks: torch.Tensor,

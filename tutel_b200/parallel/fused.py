@@ -370,12 +370,16 @@ class _Txn:
         g = self.geo
         return self.eng.t.view(self.bufs.off_out, [g.E * g.C, width], self.dtype)
 
-    def decode(self, gates_v: Optional[torch.Tensor], width: int) -> torch.Tensor:
-        """Weighted sum of each token's (virtual) choices once their experts have delivered."""
+    def decode(self, gates_v: Optional[torch.Tensor], width: int, shared: Optional[tuple] = None) -> torch.Tensor:
+        """Weighted sum of each token's (virtual) choices once their experts have delivered (+ the shared experts' term
+        ``shared = (base, fp32 logits or None)`` in the same launch, ops/dispatch.py: raw_decode)."""
         g = self.geo
         backend.count_launch()
+        if shared is None:
+            return backend.require_ext().decode_rows(self.comb_view(width), gates_v, self.plan.idx_ks, self.plan.loc_ks, g.E,
+                                                     g.C, self.base + self.bufs.f_out, self.out_target)
         return backend.require_ext().decode_rows(self.comb_view(width), gates_v, self.plan.idx_ks, self.plan.loc_ks, g.E, g.C,
-                                                 self.base + self.bufs.f_out, self.out_target)
+                                                 self.base + self.bufs.f_out, self.out_target, None, shared[0], shared[1])
 
 
 def _gate_grad(a: torch.Tensor, buf: torch.Tensor, plan: _Plan, geo: _Geometry) -> torch.Tensor:
@@ -389,6 +393,33 @@ def _gate_grad(a: torch.Tensor, buf: torch.Tensor, plan: _Plan, geo: _Geometry) 
 
 def _virtual_gates(gates_f32: torch.Tensor, geo: _Geometry) -> torch.Tensor:
     return gates_f32 if geo.copies == 1 else gates_f32.repeat(geo.copies, 1)
+
+
+def _shared_in(base: Optional[torch.Tensor], shared_logit: Optional[torch.Tensor]) -> Optional[tuple]:
+    """The shared experts' terms as decode_rows takes them, or None."""
+    if base is None:
+        return None
+    return base.contiguous(), (None if shared_logit is None else shared_logit.detach().to(torch.float32).contiguous().view(-1))
+
+
+def _shared_grads(ctx: Any, dout: torch.Tensor):
+    """(d_base, d_shared_logit) of the shared experts' term: dout itself without the shared gate; with it, the
+    gate-gradient kernel with zero routed choices (csrc/moe_kernels.cu: gate_grad_kernel)."""
+    if not ctx.has_shared:
+        return ()
+    if not ctx.shared_gated:
+        return dout, None
+    base, shared_logit = ctx.shared_saved
+    idx = torch.empty([0, dout.size(0)], dtype=torch.int32, device=dout.device)
+    backend.count_launch()
+    _, d_base, d_logit = backend.require_ext().gate_grad(dout, None, idx, idx, 1, 1, None, base.contiguous(),
+                                                         shared_logit.detach().to(torch.float32).contiguous().view(-1))
+    return d_base, d_logit.to(shared_logit.dtype).view_as(shared_logit)
+
+
+def _save_shared(ctx: Any, base: Optional[torch.Tensor], shared_logit: Optional[torch.Tensor]) -> None:
+    ctx.has_shared, ctx.shared_gated = base is not None, shared_logit is not None
+    ctx.shared_saved = (base.detach(), shared_logit.detach()) if ctx.shared_gated else None
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -452,7 +483,10 @@ class _Runner:
     def __init__(self, eng: FusedEngine, ring: _Ring, geo: _Geometry, d: int, plan: DispatchPlan):
         self.eng, self.ring, self.geo, self.d, self.plan = eng, ring, geo, d, plan
 
-    def run(self, layer, x: torch.Tensor, crit) -> torch.Tensor:
+    def run(self, layer, x: torch.Tensor, crit, base: Optional[torch.Tensor] = None,
+            shared_logit: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The fused MoE call; ``base`` / ``shared_logit``: the shared experts' output and gate logits, added in the
+        combine launch.  (Multi-GPU only: not exercised on a single-GPU machine.)"""
         geo, plan = self.geo, self.plan
         ex = layer.experts
         gates = crit.gates_ks if hasattr(crit, 'gates_ks') else torch.stack([g.view(-1) for g in crit[3]])
@@ -463,9 +497,13 @@ class _Runner:
         call = (self.eng, self.ring, geo, kplan, self.d, layer.is_postscore, bool(getattr(ex, 'fp8', False)))
         if hasattr(ex, 'full_shapes'):
             w1, w2, w3 = (ex._full(n, layer.group) for n in ('W_fc1', 'W_fc2', 'W_fc3'))
-            return _FusedGLUMoE.apply(call, G.classify_activation(ex.activation_fn), x, gates, w1, w2, w3)
+            if base is None:
+                return _FusedGLUMoE.apply(call, G.classify_activation(ex.activation_fn), x, gates, w1, w2, w3)
+            return _FusedGLUMoE.apply(call, G.classify_activation(ex.activation_fn), x, gates, w1, w2, w3, base, shared_logit)
         w1, b1, w2, b2 = ex.materialize(layer)
-        return _FusedMoE.apply(call, ex._act_kind, x, gates, w1, b1, w2, b2)
+        if base is None:
+            return _FusedMoE.apply(call, ex._act_kind, x, gates, w1, b1, w2, b2)
+        return _FusedMoE.apply(call, ex._act_kind, x, gates, w1, b1, w2, b2, base, shared_logit)
 
 
 def _begin(call, dtype) -> _Txn:
@@ -477,10 +515,11 @@ class _FusedMoE(torch.autograd.Function):
     """``ffn`` experts: y = act(x W1^T + b1) W2 + b2 between a fused dispatch and a fused combine."""
 
     @staticmethod
-    def forward(ctx: Any, call, act_kind: str, x, gates, w1, b1, w2, b2):
+    def forward(ctx: Any, call, act_kind: str, x, gates, w1, b1, w2, b2, base=None, shared_logit=None):
         eng, ring, geo, kplan, d, is_postscore, fp8 = call
         M, H, Mo = geo.M, geo.H, geo.Mo
         need_grad = any(ctx.needs_input_grad[2:])
+        _save_shared(ctx, base, shared_logit)
         gates_f32 = gates.detach().to(torch.float32).contiguous()
         tx = _begin(call, x.dtype)
 
@@ -523,8 +562,8 @@ class _FusedMoE(torch.autograd.Function):
             G.raw_gemm(act, w2, b_mn=True, epilogue=G.EPI_BIAS if b2 is not None else G.EPI_NONE, bias=b2v,
                        **tx.combine_kwargs(Mo))
 
-        # (4) combine: weighted sum of each token's k rows once their experts have delivered
-        out = tx.decode(_virtual_gates(gates_f32, geo) if is_postscore else None, Mo)
+        # (4) combine: weighted sum of each token's k rows once their experts have delivered (+ the shared experts)
+        out = tx.decode(_virtual_gates(gates_f32, geo) if is_postscore else None, Mo, _shared_in(base, shared_logit))
         torch.cuda.current_stream().wait_event(ev)
 
         ctx.call, ctx.act_kind = call, act_kind
@@ -603,7 +642,7 @@ class _FusedMoE(torch.autograd.Function):
                 dgates = _gate_grad(x, tx.comb_view(M), kplan, geo).to(gates.dtype)
         torch.cuda.current_stream().wait_event(ev)
         lease.release()
-        return None, None, dx, dgates, dw1, db1, dw2, db2
+        return (None, None, dx, dgates, dw1, db1, dw2, db2) + _shared_grads(ctx, dout)
 
 
 class _FusedGLUMoE(torch.autograd.Function):
@@ -612,10 +651,11 @@ class _FusedGLUMoE(torch.autograd.Function):
     (reference: tutel/experts/llama_ffn.py:38-41 between the two all-to-alls of tutel/impls/moe_layer.py:349-351)"""
 
     @staticmethod
-    def forward(ctx: Any, call, act: str, x, gates, w1, w2, w3):
+    def forward(ctx: Any, call, act: str, x, gates, w1, w2, w3, base=None, shared_logit=None):
         eng, ring, geo, kplan, d, is_postscore, fp8 = call
         M, H, Mo = geo.M, geo.H, geo.Mo
         need_grad = any(ctx.needs_input_grad[2:])
+        _save_shared(ctx, base, shared_logit)
         gates_f32 = gates.detach().to(torch.float32).contiguous()
         tx = _begin(call, x.dtype)
         cg, _, _ = eng.tile_counts(geo.C, H)
@@ -642,7 +682,7 @@ class _FusedGLUMoE(torch.autograd.Function):
             x_recv = tx.recv_view(M)
             h, g, u = G.glu_gemm(x_recv, w1, w2, b_mn=True, act=act, save_pre=need_grad, cta_group=cg, **tx.wait_kwargs())
             G.raw_gemm(h, w3, b_mn=True, **tx.combine_kwargs(Mo))
-        out = tx.decode(_virtual_gates(gates_f32, geo) if is_postscore else None, Mo)
+        out = tx.decode(_virtual_gates(gates_f32, geo) if is_postscore else None, Mo, _shared_in(base, shared_logit))
         torch.cuda.current_stream().wait_event(ev)
         ctx.call, ctx.act = call, act
         if need_grad:
@@ -703,4 +743,4 @@ class _FusedGLUMoE(torch.autograd.Function):
                 dgates = _gate_grad(x, tx.comb_view(M), kplan, geo).to(gates.dtype)
         torch.cuda.current_stream().wait_event(ev)
         lease.release()
-        return None, None, dx, dgates, dw1, dw2, dw3
+        return (None, None, dx, dgates, dw1, dw2, dw3) + _shared_grads(ctx, dout)
