@@ -13,6 +13,8 @@
 //     (combine all-to-all fused into the GEMM epilogue on the producer side).
 #include "moe_kernels.h"
 
+#include <cfloat>
+
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
@@ -536,7 +538,8 @@ quantize_rows_kernel(const T* __restrict__ x, uint8_t* __restrict__ q, float* __
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-    const float s = amax > 0.0f ? amax * (1.0f / 448.0f) : 1.0f;
+    // (at least FLT_MIN: below it 1 / s overflows, and a row of tiny values would turn its zeros into 0 * inf = NaN)
+    const float s = amax > 0.0f ? fmaxf(amax * (1.0f / 448.0f), FLT_MIN) : 1.0f;
     const float inv = 1.0f / s;
     if (lane == 0) scale[r] = s;
     uint8_t* qrow = q + r * K;
@@ -612,7 +615,7 @@ encode_rows_fp8_kernel(const T* __restrict__ x, const float* __restrict__ gates,
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
       amax *= fabsf(g);
-      const float sc = amax > 0.0f ? amax * (1.0f / 448.0f) : 1.0f;
+      const float sc = amax > 0.0f ? fmaxf(amax * (1.0f / 448.0f), FLT_MIN) : 1.0f;     // (FLT_MIN: see quantize_rows)
       const float inv = g / sc;
       if (lane == 0) sc_e[r] = sc;
       for (int v = lane; v < n16; v += 32) {                 // second pass hits L1/L2: 2 x 16 B in, 16 B out
@@ -730,7 +733,7 @@ quantize_transpose_kernel(const T* __restrict__ x, const float* __restrict__ ama
   }
   const int k = threadIdx.x & 63;
   const float am = amax[static_cast<long long>(g) * K + k0 + k];
-  const float sc = am > 0.0f ? am * (1.0f / 448.0f) : 1.0f;
+  const float sc = am > 0.0f ? fmaxf(am * (1.0f / 448.0f), FLT_MIN) : 1.0f;      // (FLT_MIN: see quantize_rows)
   const float inv = 1.0f / sc;
   if (blockIdx.y == 0 && threadIdx.x < 64) scale[static_cast<long long>(g) * K + k0 + k] = sc;
   __syncthreads();

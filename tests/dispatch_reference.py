@@ -30,6 +30,7 @@ SLACK = 1.01                      # second-order terms of the first-order bounds
 TINY = 2.0 ** -147                # four fp32 subnormal spacings: expf / products whose result is subnormal
 INVALID_LOC = 0x3fffffff          # loc of a choice that routes nowhere
 F448 = torch.tensor(1.0 / 448.0, dtype=torch.float32)   # the kernels' fp32 constant 1.0f / 448.0f
+FLT_MIN = 2.0 ** -126             # smallest e4m3 row scale: 1 / scale must not overflow
 E4M3_MAX = 448.0
 OBSERVED: Dict[str, float] = {}
 
@@ -339,14 +340,14 @@ def to_e4m3(v: torch.Tensor) -> torch.Tensor:
 
 
 def ref_encode_fp8(x, gates, slot, k, E, C):
-    """fp8 dispatch rows in fp32, bit for bit: amax = max|x|, amax *= |g|, sc = amax * fp32(1/448) (1 when amax = 0),
+    """fp8 dispatch rows in fp32, bit for bit: amax = max|x|, amax *= |g|, sc = max(amax * fp32(1/448), FLT_MIN) (1 when amax = 0),
     inv = g / sc, q = e4m3(x * inv).  An empty slot has zero bytes and scale 1.  Returns (q uint8 [E*C, M], sc)."""
     empty, tok, g = _slot_sources(slot, k, gates)
     xf = x.float()[tok]
     if g is None:
         g = torch.ones(xf.size(0), dtype=torch.float32, device=x.device)
     amax = xf.abs().amax(1) * g.abs()
-    sc = torch.where(amax > 0, amax * F448.to(x.device), torch.ones_like(amax))
+    sc = torch.where(amax > 0, (amax * F448.to(x.device)).clamp_min(FLT_MIN), torch.ones_like(amax))
     inv = g / sc
     q = to_e4m3(xf * inv[:, None])
     q = torch.where(empty[:, None], torch.zeros_like(q), q)
@@ -366,11 +367,11 @@ def ref_dequant(q, scale, dtype):
 
 
 def ref_quantize_transpose(x):
-    """x [G, R, K] 16 bit -> (qT uint8 [G, K, R], scale [G, K]): column amax, sc = amax * fp32(1/448) (1 when 0),
+    """x [G, R, K] 16 bit -> (qT uint8 [G, K, R], scale [G, K]): column amax, sc = max(amax * fp32(1/448), FLT_MIN) (1 when 0),
     inv = 1 / sc, e4m3(x * inv) transposed."""
     xf = x.float()
     amax = xf.abs().amax(1)
-    sc = torch.where(amax > 0, amax * F448.to(x.device), torch.ones_like(amax))
+    sc = torch.where(amax > 0, (amax * F448.to(x.device)).clamp_min(FLT_MIN), torch.ones_like(amax))
     inv = 1.0 / sc
     return to_e4m3(xf * inv[:, None, :]).transpose(1, 2).contiguous(), sc
 

@@ -111,11 +111,12 @@ def zero_tail(t: torch.Tensor, counts: Optional[torch.Tensor]) -> torch.Tensor:
 
 
 def quantize_rows_reference(t: torch.Tensor):
-    """The row quantisation of csrc/moe_kernels.h, in fp32 as the kernels compute it: s = max|row| * fp32(1/448)
-    (1 for an all-zero row), q = e4m3_rn(x * fp32(1 / s)).  NaN elements do not count towards the maximum."""
+    """The row quantisation of csrc/moe_kernels.h, in fp32 as the kernels compute it: s = max(max|row| * fp32(1/448),
+    FLT_MIN) (1 for an all-zero row), q = e4m3_rn(x * fp32(1 / s)).  NaN elements do not count towards the maximum."""
     f = t.float()
     a = torch.where(torch.isnan(f), torch.zeros_like(f), f.abs()).amax(-1)
-    s = torch.where(a > 0, a * torch.tensor(1.0 / 448.0, dtype=torch.float32, device=f.device), torch.ones_like(a))
+    s = torch.where(a > 0, (a * torch.tensor(1.0 / 448.0, dtype=torch.float32, device=f.device)).clamp_min(2.0 ** -126),
+                    torch.ones_like(a))
     inv = torch.ones((), dtype=torch.float32, device=f.device) / s
     return (f * inv.unsqueeze(-1)).to(torch.float8_e4m3fn), s
 

@@ -110,7 +110,7 @@ def emulate_encode_fp8(x, gates, slot, k, E, C, miss=None):
     amax = xf.abs().amax(1)
     if miss != 'fp8_scale_without_gate':
         amax = amax * g.abs()
-    sc = torch.where(amax > 0, amax * R.F448, torch.ones_like(amax))
+    sc = torch.where(amax > 0, (amax * R.F448).clamp_min(R.FLT_MIN), torch.ones_like(amax))
     q = (xf * (g / sc)[:, None]).clamp(-448, 448).to(torch.float8_e4m3fn).view(torch.uint8)
     q[empty] = 0
     sc[empty] = 1.0
