@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "cpu_kernels.h"
+#include "gemm_block_fp8.h"
 #include "gemm_mx.h"
 #include "gemm_sm90.h"
 #include "jit_nvrtc.h"
@@ -731,6 +732,117 @@ at::Tensor mx_gemm(const at::Tensor& a, const at::Tensor& sfa, const at::Tensor&
   return d;
 }
 
+// Block-scaled fp8 (DeepSeek-V3: 1 x 128 activation tiles, 128 x 128 weight blocks, fp32 scales); see csrc/gemm_block_fp8.cu.
+// x [G, R, K] bf16 (K % 128 == 0) -> [q e4m3 [G, R, K], s fp32 [G, K / 128, roundup(R, 128)]]
+std::vector<at::Tensor> block_fp8_quantize_act(const at::Tensor& x) {
+  TORCH_CHECK(x.is_cuda() && x.is_contiguous() && x.dim() == 3 && x.scalar_type() == at::kBFloat16 && x.size(2) % 128 == 0,
+              "block_fp8_quantize_act: contiguous bf16 CUDA tensor [G, R, K] with K % 128 == 0 expected");
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int G = static_cast<int>(x.size(0)), R = static_cast<int>(x.size(1)), K = static_cast<int>(x.size(2));
+  at::Tensor q = at::empty({G, R, K}, x.options().dtype(at::kFloat8_e4m3fn));
+  at::Tensor s = at::empty({G, K / 128, (R + 127) / 128 * 128}, x.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::block_fp8_quantize_act(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), G, R, K, cur_stream()));
+  return {q, s};
+}
+
+// w [G, R, C] bf16 (R, C % 128 == 0) -> [q [G, R, C], s [G, R / 128, C / 128], qT [G, C, R], sT [G, C / 128, R / 128]]
+std::vector<at::Tensor> block_fp8_quantize_weight(const at::Tensor& w) {
+  TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.dim() == 3 && w.scalar_type() == at::kBFloat16 && w.size(1) % 128 == 0 &&
+                  w.size(2) % 128 == 0,
+              "block_fp8_quantize_weight: contiguous bf16 CUDA tensor [G, R, C] with R % 128 == 0 and C % 128 == 0 expected");
+  const c10::cuda::CUDAGuard guard(w.device());
+  const int G = static_cast<int>(w.size(0)), R = static_cast<int>(w.size(1)), C = static_cast<int>(w.size(2));
+  at::Tensor q = at::empty({G, R, C}, w.options().dtype(at::kFloat8_e4m3fn));
+  at::Tensor qT = at::empty({G, C, R}, w.options().dtype(at::kFloat8_e4m3fn));
+  at::Tensor s = at::empty({G, R / 128, C / 128}, w.options().dtype(at::kFloat));
+  at::Tensor sT = at::empty({G, C / 128, R / 128}, w.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::block_fp8_quantize_weight(w.data_ptr(), q.data_ptr(), s.data_ptr<float>(), qT.data_ptr(), sT.data_ptr<float>(),
+                                              G, R, C, cur_stream()));
+  return {q, s, qT, sT};
+}
+
+// SwiGLU gate / up weights w1, w2 [G, M, H] bf16 -> [qcat [G, M, 2H], scat [G, M / 128, 2H / 128],
+// qglu [G, 2H, M] (interleaved every 64 rows), sglu [G, 2H / 64, M / 128]]  (csrc/gemm_block_fp8.h)
+std::vector<at::Tensor> block_fp8_quantize_glu_weight(const at::Tensor& w1, const at::Tensor& w2) {
+  TORCH_CHECK(w1.is_cuda() && w1.is_contiguous() && w2.is_contiguous() && w1.dim() == 3 && w1.sizes() == w2.sizes() &&
+                  w1.scalar_type() == at::kBFloat16 && w2.scalar_type() == at::kBFloat16 && w2.device() == w1.device() &&
+                  w1.size(1) % 128 == 0 && w1.size(2) % 128 == 0,
+              "block_fp8_quantize_glu_weight: two contiguous bf16 CUDA tensors [G, M, H] with M % 128 == 0 and H % 128 == 0 expected");
+  const c10::cuda::CUDAGuard guard(w1.device());
+  const int G = static_cast<int>(w1.size(0)), M = static_cast<int>(w1.size(1)), H = static_cast<int>(w1.size(2));
+  at::Tensor qcat = at::empty({G, M, 2 * H}, w1.options().dtype(at::kFloat8_e4m3fn));
+  at::Tensor qglu = at::empty({G, 2 * H, M}, w1.options().dtype(at::kFloat8_e4m3fn));
+  at::Tensor scat = at::empty({G, M / 128, 2 * H / 128}, w1.options().dtype(at::kFloat));
+  at::Tensor sglu = at::empty({G, 2 * H / 64, M / 128}, w1.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::block_fp8_quantize_glu_weight(w1.data_ptr(), w2.data_ptr(), qcat.data_ptr(), scat.data_ptr<float>(),
+                                                  qglu.data_ptr(), sglu.data_ptr<float>(), G, M, H, cur_stream()));
+  return {qcat, scat, qglu, sglu};
+}
+
+// d[g] = epilogue(a[g] * b[g]^T):  a e4m3 [G, M, K] + sa, b e4m3 [G, N, K] + sb (shapes above) -> bf16.
+// epilogue 0 none / 1 ReLU (+ bias [G, N]) -> [d [G, M, N]];  2 ReLU backward (aux = forward activation) -> [d];
+// 3 GLU (b = the interleaved gate / up copy, sb [G, N / 64, K / 128]) -> [h, g, u], each [G, M, N / 2];
+// 4 GLU backward (acc = dh, aux = g, aux2 = u) -> [dgu [G, M, 2N]] with dg in columns [0, N) and du in [N, 2N).
+std::vector<at::Tensor> block_fp8_gemm(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                       const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
+                                       const c10::optional<at::Tensor>& aux2, int64_t epilogue, int64_t act, int64_t max_ctas) {
+  TORCH_CHECK(a.is_cuda() && b.is_cuda() && sa.is_cuda() && sb.is_cuda() && a.dim() == 3 && b.dim() == 3 && sa.dim() == 3 &&
+              sb.dim() == 3, "block_fp8_gemm: 3-D CUDA tensors expected");
+  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && sa.is_contiguous() && sb.is_contiguous(),
+              "block_fp8_gemm: contiguous operands expected");
+  TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn &&
+              sa.scalar_type() == at::kFloat && sb.scalar_type() == at::kFloat, "block_fp8_gemm: e4m3 operands and fp32 scales expected");
+  TORCH_CHECK(a.size(0) == b.size(0) && a.size(2) == b.size(2), "block_fp8_gemm: a [G, M, K] and b [G, N, K] expected");
+  TORCH_CHECK(epilogue >= tb::BF8_EPI_NONE && epilogue <= tb::BF8_EPI_GLU_BWD, "block_fp8_gemm: unknown epilogue");
+  const c10::cuda::CUDAGuard guard(a.device());
+  tb::BlockFp8GemmProblem p;
+  p.G = static_cast<int>(a.size(0)); p.M = static_cast<int>(a.size(1)); p.K = static_cast<int>(a.size(2));
+  p.N = static_cast<int>(b.size(1));
+  const bool glu = epilogue == tb::BF8_EPI_GLU, glu_bwd = epilogue == tb::BF8_EPI_GLU_BWD;
+  const int64_t kb = (p.K + 127) / 128, mp = (p.M + 127) / 128 * 128, nb = glu ? (p.N + 63) / 64 : (p.N + 127) / 128;
+  TORCH_CHECK(sa.size(0) == p.G && sa.size(1) == kb && sa.size(2) == mp && sb.size(0) == p.G && sb.size(1) == nb && sb.size(2) == kb,
+              glu ? "block_fp8_gemm: scale arrays do not match the operand shapes (sa [G, K / 128, roundup(M, 128)], sb [G, N / 64, K / 128] expected)"
+                  : "block_fp8_gemm: scale arrays do not match the operand shapes (sa [G, K / 128, roundup(M, 128)], sb [G, N / 128, K / 128] expected)");
+  const auto bf = a.options().dtype(at::kBFloat16);
+  auto check_mn = [&](const c10::optional<at::Tensor>& t, const char* name) -> const void* {
+    if (!t.has_value() || !t->defined()) return nullptr;
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->dim() == 3 && t->size(0) == p.G &&
+                t->size(1) == p.M && t->size(2) == p.N, "block_fp8_gemm: ", name, " must be a contiguous bf16 [G, M, N]");
+    return t->data_ptr();
+  };
+  p.aux = check_mn(aux, "aux");
+  p.aux2 = check_mn(aux2, "aux2");
+  p.ld_aux = p.N; p.aux_group_stride = static_cast<long long>(p.M) * p.N;
+  if (bias.has_value() && bias->defined()) {
+    TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == at::kBFloat16 && bias->is_contiguous() && bias->numel() == static_cast<long long>(p.G) * p.N,
+                "block_fp8_gemm: bias must be a contiguous bf16 [G, N]");
+    p.bias = bias->data_ptr(); p.bias_group_stride = p.N;
+  }
+  std::vector<at::Tensor> out;
+  if (glu) {
+    for (int i = 0; i < 3; ++i) out.push_back(at::empty({p.G, p.M, p.N / 2}, bf));
+    p.d = out[0].data_ptr(); p.d2 = out[1].data_ptr(); p.d3 = out[2].data_ptr();
+    p.ldd = p.N / 2;
+  } else if (glu_bwd) {
+    out.push_back(at::empty({p.G, p.M, 2LL * p.N}, bf));
+    p.d = out[0].data_ptr(); p.d2 = static_cast<__nv_bfloat16*>(p.d) + p.N;
+    p.ldd = 2LL * p.N;
+  } else {
+    out.push_back(at::empty({p.G, p.M, p.N}, bf));
+    p.d = out[0].data_ptr();
+    p.ldd = p.N;
+  }
+  p.d_group_stride = p.ldd * p.M;
+  p.a = a.data_ptr(); p.sa = sa.data_ptr<float>(); p.b = b.data_ptr(); p.sb = sb.data_ptr<float>();
+  p.epilogue = static_cast<int>(epilogue);
+  p.act = static_cast<int>(act);
+  p.max_ctas = static_cast<int>(max_ctas);
+  const char* why = nullptr;
+  cudaError_t e = tb::block_fp8_gemm_launch(p, cur_stream(), &why);
+  TORCH_CHECK(e == cudaSuccess, "block_fp8_gemm: ", why ? why : cudaGetErrorString(e));
+  return out;
+}
+
 // Gated-linear-unit GEMMs (SwiGLU / GeGLU / ReGLU experts; reference: tutel/experts/llama_ffn.py:38-41 runs three
 // cuBLAS GEMMs plus separate activation and multiply kernels).
 //   forward  (b2 given):  h = act(a*b) .* (a*b2)   [+ g = a*b -> d2, u = a*b2 -> d3 when given]   ONE launch
@@ -1013,6 +1125,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mx_quantize", &mx_quantize);
   m.def("mx_quantize_transpose", &mx_quantize_transpose);
   m.def("mx_gemm", &mx_gemm);
+  m.def("block_fp8_quantize_act", &block_fp8_quantize_act);
+  m.def("block_fp8_quantize_weight", &block_fp8_quantize_weight);
+  m.def("block_fp8_quantize_glu_weight", &block_fp8_quantize_glu_weight);
+  m.def("block_fp8_gemm", &block_fp8_gemm);
   register_symm_bindings(m);
   register_cpu_bindings(m);
   register_jit_bindings(m);

@@ -114,6 +114,7 @@ cudaError_t set_spin_timeout_moe(unsigned long long ns);
 cudaError_t set_spin_timeout_p2p(unsigned long long ns);
 cudaError_t set_spin_timeout_gemm(unsigned long long ns);
 cudaError_t set_spin_timeout_mx(unsigned long long ns);
+cudaError_t set_spin_timeout_block_fp8(unsigned long long ns);
 
 // q[r, :] = e4m3(x[r, :] / scale[r]),  scale[r] = max|x[r, :]| / 448   (one scale per row; rows are K-major GEMM
 // operands, so the scale factors out of the dot product and is applied in the GEMM epilogue).

@@ -283,6 +283,7 @@ void register_symm_bindings(pybind11::module& m) {
     TB_CHECK_CUDA(tb::set_spin_timeout_p2p(ns));
     TB_CHECK_CUDA(tb::set_spin_timeout_gemm(ns));
     TB_CHECK_CUDA(tb::set_spin_timeout_mx(ns));
+    TB_CHECK_CUDA(tb::set_spin_timeout_block_fp8(ns));
   });
   m.def("p2p_barrier", [](int64_t peer_table, int64_t bar_off, int64_t rank, int64_t world, int64_t epoch) {
     TB_CHECK_CUDA(tb::p2p_barrier(reinterpret_cast<const unsigned long long*>(peer_table), bar_off,

@@ -16,6 +16,7 @@ import os
 import torch
 import torch.nn.functional as F
 
+from ...ops import block_fp8 as BF8
 from ...ops import gemm as G
 from ...ops import mx as MX
 from ...parallel import communicate as C
@@ -40,11 +41,15 @@ class FusedExpertsNetwork(torch.nn.Module):
         # fp8=True / 'row' (or TUTEL_B200_FP8=1): forward and data-gradient expert GEMMs in e4m3 with per-row / per-channel
         # scales (also inside the fused engine).  fp8='mx' (TUTEL_B200_FP8=mx): OCP MX - e4m3 with one power-of-two scale
         # per 32 elements, applied by the tensor core (ops/mx.py, csrc/gemm_mx.cu); runs on the unfused path.
+        # fp8='block' (TUTEL_B200_FP8=block): DeepSeek-V3 block scales - one fp32 scale per 1 x 128 activation tile and per
+        # 128 x 128 weight block (ops/block_fp8.py, csrc/gemm_block_fp8.cu); ReLU experts, unfused path.
         mode = os.environ.get('TUTEL_B200_FP8', '0') if fp8 is None else fp8
         mode = str(mode).lower()
-        assert mode in ('0', '1', 'true', 'false', 'none', 'row', 'mx'), 'fp8 must be a bool, "row" or "mx" (got %r)' % (fp8,)
+        assert mode in ('0', '1', 'true', 'false', 'none', 'row', 'mx', 'block'), \
+            'fp8 must be a bool, "row", "mx" or "block" (got %r)' % (fp8,)
         self.fp8 = mode in ('1', 'true', 'row')
         self.mx = mode == 'mx'
+        self.block = mode == 'block'
 
         if activation_fn_with_self is not None:
             assert activation_fn is None, 'Option `activation_fn_with_self` has been specified, please keep exactly one of them.'
@@ -131,9 +136,9 @@ class FusedExpertsNetwork(torch.nn.Module):
 
     def supports_packed(self, x) -> bool:
         """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit ReLU / GELU / SiLU experts
-        without fp8 / MX, on weights of x's dtype."""
+        without fp8 / MX / block fp8, on weights of x's dtype."""
         w1 = self.batched_fc1_w
-        return (not self.fp8 and not self.mx and self._act_kind in G.FWD_EPILOGUE and x.dtype in (torch.float16, torch.bfloat16)
+        return (not self.fp8 and not self.mx and not self.block and self._act_kind in G.FWD_EPILOGUE and x.dtype in (torch.float16, torch.bfloat16)
                 and w1.dtype == x.dtype and x.is_cuda and self.sharded_count == 1 and
                 all(d % 8 == 0 for d in (self.model_dim, self.hidden_size, self.output_dim)))
 
@@ -163,6 +168,8 @@ class FusedExpertsNetwork(torch.nn.Module):
             return G.skinny_linear(y, w2, b2, 'kn', row_counts)
         if self.mx and self._act_kind == 'relu' and row_counts is None and MX.can_use_mx(x, w1, w2):
             y = MX.fused_relu_ffn_mx(x, w1, b1, w2, b2)
+        elif self.block and self._act_kind == 'relu' and row_counts is None and BF8.can_use_block_fp8(x, w1, w2):
+            y = BF8.fused_relu_ffn_block_fp8(x, w1, b1, w2, b2)
         elif self._act_kind in G.FWD_EPILOGUE and G.can_use_wgmma(x, w1) and G.can_use_wgmma(x, w2):
             if self.fp8 and self._act_kind == 'relu' and x.size(-1) % 16 == 0 and w1.size(1) % 16 == 0:
                 y = G.fused_relu_ffn_fp8(x, w1, b1, w2, b2, row_counts)

@@ -8,6 +8,7 @@ weights (csrc/skinny_gemm.cu), above that the wgmma kernels skip the rows past t
 """
 import torch
 
+from ...ops import block_fp8 as BF8
 from ...ops import gemm as G
 from ...parallel import communicate as C
 from . import dropless_row_counts
@@ -21,11 +22,13 @@ class LlamaFFNNetwork(torch.nn.Module):
         super().__init__()
         import os
         # fp8=True / 'row' (or TUTEL_B200_FP8=1 / true / row): e4m3 weights with per-row scales on every path, as in `ffn`.
-        # OCP MX ('mx') has no SwiGLU kernel.
+        # fp8='block' (TUTEL_B200_FP8=block): DeepSeek-V3 block scales for the training GEMMs (ops/block_fp8.py); dropless
+        # decoding keeps the 16-bit kernels.  OCP MX ('mx') has no SwiGLU kernel.
         mode = str(os.environ.get('TUTEL_B200_FP8', '0') if fp8 is None else fp8).lower()
-        assert mode in ('0', '1', 'true', 'false', 'none', 'row'), \
-            'llama_ffn: fp8 must be a bool or "row" (got %r); "mx" has no SwiGLU path' % (mode,)
+        assert mode in ('0', '1', 'true', 'false', 'none', 'row', 'block'), \
+            'llama_ffn: fp8 must be a bool, "row" or "block" (got %r); "mx" has no SwiGLU path' % (mode,)
         self.fp8 = mode in ('1', 'true', 'row')
+        self.block = mode == 'block'
         self.sharded_count = sharded_count
         self.full_shapes = {
             'W_fc1': torch.Size([num_experts_per_device, model_dim, hidden_size_per_expert]),
@@ -69,6 +72,8 @@ class LlamaFFNNetwork(torch.nn.Module):
             if self.fp8 and G.can_use_skinny_glu_ffn_fp8(x, w1, w2, w3, kind):
                 return G.skinny_glu_ffn_fp8(x, w1, w2, w3, row_counts, kind)
             return G.skinny_glu_ffn(x, w1, w2, w3, row_counts, kind)
+        if self.block and row_counts is None and kind in BF8.ACT_CODES and BF8.can_use_block_fp8(x, w1, w2, w3):
+            return BF8.fused_glu_ffn_block_fp8(x, w1, w2, w3, kind)
         if kind in G.ACT_CODES and G.can_use_wgmma(x, w1) and w3.size(-1) % 8 == 0:
             # gate/up GEMMs + activation + multiply in one dual-B wgmma launch; backward without elementwise passes
             return G.fused_glu_ffn(x, w1, w2, w3, kind, self.fp8 and x.size(-1) % 16 == 0 and w3.size(1) % 16 == 0,
@@ -79,9 +84,9 @@ class LlamaFFNNetwork(torch.nn.Module):
         return G.grouped_linear(self.activation_fn(y1) * y2, w3, None, 'kn', fp8=self.fp8)
 
     def supports_packed(self, x) -> bool:
-        """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit experts without fp8."""
+        """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit experts without fp8 or block fp8."""
         M, H = self.full_shapes['W_fc1'][1], self.full_shapes['W_fc1'][2]
-        return (not self.fp8 and x.dtype in (torch.float16, torch.bfloat16) and self.W_fc1.dtype == x.dtype and x.is_cuda and
+        return (not self.fp8 and not self.block and x.dtype in (torch.float16, torch.bfloat16) and self.W_fc1.dtype == x.dtype and x.is_cuda and
                 self.sharded_count == 1 and G.classify_activation(self.activation_fn) in G.ACT_CODES and
                 M % 8 == 0 and H % 8 == 0)
 

@@ -1,0 +1,335 @@
+"""Block-scaled fp8 expert GEMMs, the DeepSeek-V3 recipe (also that of DeepGEMM and of the block-scaled fp8 checkpoints
+DeepSeek-V3, Kimi-K2, GLM-4.5 and Moonlight ship with, ``weight_scale_inv`` per 128 x 128 block):
+
+* activations ``[G, R, K]``: e4m3 with one fp32 scale per row and 128-element K tile (1 x 128);
+* weights ``[G, N, K]``: e4m3 with one fp32 scale per 128 x 128 block;
+* the GEMM (csrc/gemm_block_fp8.cu) runs each 128-deep K step as four e4m3 ``wgmma`` into a scratch fragment and promotes
+  it into the fp32 accumulator with the step's two scales: ``acc += scratch * (sa[row] * sb)``.
+
+A 128 x 128 block is the same block in ``W`` and ``W^T``, so the data-gradient copy of a weight is the forward copy
+transposed, scales included; one launch writes both.
+
+Everything here also has a pure PyTorch definition (``*_reference``) that runs on CPU: the tests compare the kernels
+against it, and it documents the format:
+
+* block scale      ``amax`` = the largest magnitude in the block that is not NaN,
+                   ``s = max(amax * (1 / 448), FLT_MIN)`` if ``amax > 0`` else ``1`` (fp32 arithmetic, the rule of
+                   ``quantize_rows_kernel``, csrc/moe_kernels.cu)
+* elements         ``q = e4m3_rn_satfinite(x * (1 / s))`` (+-inf saturate to +-448, NaN stays NaN)
+* activation scales ``[G, K / 128, roundup(R, 128)]`` fp32, MN-major (one K step of a 128-row tile is 512 contiguous
+                   bytes); pad rows have scale 0
+* weight scales    ``[G, N / 128, K / 128]`` fp32
+* SwiGLU gate / up ``w1, w2 [G, M, H]``: the data-gradient operand is ``[W1 W2]`` ``[G, M, 2H]`` with scales
+                   ``[G, M / 128, 2H / 128]``; the forward operand is ``W1^T`` and ``W2^T`` interleaved every 64 rows,
+                   ``[G, 2H, M]`` (rows ``128 t + j`` = gate column ``64 t + j``, rows ``128 t + 64 + j`` = up column
+                   ``64 t + j``) with one scale per 64 rows, ``[G, 2H / 64, M / 128]``, so that one 128-wide N tile holds
+                   a gate column and its up partner in the same thread and the GLU epilogue stays in registers.
+
+Every GEMM dimension but the token count must be a multiple of 128; the operands are bf16.
+"""
+from __future__ import annotations
+
+from typing import Any, Optional, Tuple
+
+import torch
+
+from . import backend
+
+TILE = 128
+E4M3_MAX = 448.0
+FLT_MIN = 2.0 ** -126
+EPI_NONE, EPI_RELU, EPI_RELU_BWD, EPI_GLU, EPI_GLU_BWD = 0, 1, 2, 3, 4
+ACT_CODES = {'relu': 1, 'gelu': 2, 'silu': 3}
+
+
+def _f32(v: float, like: torch.Tensor) -> torch.Tensor:
+    return torch.tensor(v, dtype=torch.float32, device=like.device)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# number format (pure PyTorch)
+# ------------------------------------------------------------------------------------------------------------------
+def block_scale_reference(amax: torch.Tensor) -> torch.Tensor:
+    """fp32 scales of blocks whose largest non-NaN magnitude is ``amax`` (fp32)."""
+    s = torch.maximum(amax * _f32(1.0 / E4M3_MAX, amax), _f32(FLT_MIN, amax))
+    return torch.where(amax > 0, s, torch.ones_like(s))
+
+
+def _nan_abs(x: torch.Tensor) -> torch.Tensor:
+    a = x.float().abs()
+    return torch.where(torch.isnan(a), torch.zeros_like(a), a)
+
+
+def _e4m3(v: torch.Tensor) -> torch.Tensor:
+    return v.clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+
+
+def quantize_act_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """x [G, R, K] -> (q e4m3 [G, R, K], s fp32 [G, K / 128, roundup(R, 128)])."""
+    G, R, K = x.shape
+    _check(K % TILE == 0, 'block fp8 activations need K %% 128 == 0 (got %d)' % K)
+    KT, Rp = K // TILE, -(-R // TILE) * TILE
+    xf = x.float().view(G, R, KT, TILE)
+    s = block_scale_reference(_nan_abs(xf).amax(-1))                                  # [G, R, KT]
+    q = _e4m3(xf * (1.0 / s).unsqueeze(-1)).view(G, R, K)
+    st = torch.zeros(G, KT, Rp, dtype=torch.float32, device=x.device)
+    st[:, :, :R] = s.transpose(1, 2)
+    return q, st
+
+
+def quantize_weight_reference(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """w [G, R, C] -> (q [G, R, C], s [G, R / 128, C / 128], qT [G, C, R], sT [G, C / 128, R / 128])."""
+    G, R, C = w.shape
+    _check(R % TILE == 0 and C % TILE == 0, 'block fp8 weights need both dims %% 128 == 0 (got %s)' % (tuple(w.shape),))
+    wf = w.float().view(G, R // TILE, TILE, C // TILE, TILE)
+    s = block_scale_reference(_nan_abs(wf).amax(dim=(2, 4)))                         # [G, RB, CB]
+    q = _e4m3(wf * (1.0 / s)[:, :, None, :, None]).view(G, R, C)
+    return q, s, q.transpose(1, 2).contiguous(), s.transpose(1, 2).contiguous()
+
+
+def interleave_glu_reference(t1: torch.Tensor, t2: torch.Tensor, rows_per: int = 64) -> torch.Tensor:
+    """[G, H, *] gate and up rows -> [G, 2H, *]: blocks of ``rows_per`` rows, gate then up."""
+    G, H = t1.shape[:2]
+    pair = torch.stack([t1.reshape(G, H // rows_per, rows_per, -1), t2.reshape(G, H // rows_per, rows_per, -1)], dim=2)
+    return pair.reshape(G, 2 * H, *t1.shape[2:])
+
+
+def quantize_glu_weight_reference(w1: torch.Tensor, w2: torch.Tensor):
+    """Gate / up weights w1, w2 [G, M, H] -> (qcat [G, M, 2H], scat [G, M / 128, 2H / 128], qglu [G, 2H, M],
+    sglu [G, 2H / 64, M / 128])."""
+    q1, s1, q1t, s1t = quantize_weight_reference(w1)
+    q2, s2, q2t, s2t = quantize_weight_reference(w2)
+    qcat, scat = torch.cat([q1, q2], dim=2), torch.cat([s1, s2], dim=2)
+    # one scale per 64 interleaved rows: each 128-row scale block of W^T covers two of them
+    qglu = interleave_glu_reference(q1t.view(torch.uint8), q2t.view(torch.uint8)).view(torch.float8_e4m3fn)
+    sglu = interleave_glu_reference(s1t.repeat_interleave(2, dim=1), s2t.repeat_interleave(2, dim=1), rows_per=1)
+    return qcat, scat, qglu, sglu
+
+
+def dequantize_act(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """fp32 values of an activation operand."""
+    G, R, K = q.shape
+    return (q.float().view(G, R, K // TILE, TILE) * s[:, :, :R].transpose(1, 2).unsqueeze(-1)).view(G, R, K)
+
+
+def dequantize_weight(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """fp32 values of a weight operand [G, N, K] with one scale per 128 x 128 block (or per 64 x 128, GLU layout)."""
+    G, N, K = q.shape
+    rows = N // s.size(1)
+    return (q.float().view(G, s.size(1), rows, K // TILE, TILE) * s[:, :, None, :, None]).view(G, N, K)
+
+
+def _act(g: torch.Tensor, act: str) -> Tuple[torch.Tensor, torch.Tensor]:
+    if act == 'relu':
+        return g.clamp_min(0), (g > 0).to(g.dtype)
+    if act == 'gelu':
+        cdf = 0.5 * (1 + torch.erf(g * 0.70710678118654752))
+        return g * cdf, cdf + g * 0.3989422804014327 * torch.exp(-0.5 * g * g)
+    sg = torch.sigmoid(g)
+    return g * sg, sg * (1 + g * (1 - sg))
+
+
+def block_fp8_gemm_reference(a, sa, b, sb, bias=None, aux=None, aux2=None, epilogue=EPI_NONE, act='silu'):
+    """fp32 emulation of one ``block_fp8_gemm`` launch, in the kernel's order: one fresh fp32 sum per 128-deep K step,
+    promoted with a single rounding, ``acc = fma(part, sa * sb, acc)``; then the epilogue in fp32 and one bf16 rounding.
+    Returns what the binding returns (a list)."""
+    G, M, K = a.shape
+    N = b.size(1)
+    rows_b = N // sb.size(1)
+    acc = torch.zeros(G, M, N, dtype=torch.float32, device=a.device)
+    af, bf = a.float(), b.float()
+    for kb in range(K // TILE):
+        k = slice(kb * TILE, (kb + 1) * TILE)
+        part = af[:, :, k] @ bf[:, :, k].transpose(1, 2)
+        sab = sa[:, kb, :M].unsqueeze(-1) * sb[:, :, kb].repeat_interleave(rows_b, dim=1).unsqueeze(1)   # fp32 product
+        acc = (part.double() * sab.double() + acc.double()).float()
+    if epilogue == EPI_GLU:
+        H = N // 2
+        t = acc.view(G, M, H // 64, 2, 64)
+        g, u = t[:, :, :, 0].reshape(G, M, H), t[:, :, :, 1].reshape(G, M, H)
+        h = _act(g, act)[0] * u
+        return [h.bfloat16(), g.bfloat16(), u.bfloat16()]
+    if epilogue == EPI_GLU_BWD:
+        a_, da = _act(aux.float(), act)
+        return [torch.cat([acc * aux2.float() * da, acc * a_], dim=2).bfloat16()]
+    if bias is not None:
+        acc = acc + bias.float().reshape(G, 1, N)
+    if epilogue == EPI_RELU:
+        acc = acc.clamp_min(0)
+    elif epilogue == EPI_RELU_BWD:
+        acc = torch.where(aux.float() > 0, acc, torch.zeros_like(acc))
+    return [acc.bfloat16()]
+
+
+def _check(ok: bool, msg: str):
+    if not ok:
+        raise ValueError(msg)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# kernels
+# ------------------------------------------------------------------------------------------------------------------
+def _native(x: torch.Tensor, what: str) -> bool:
+    if x.is_cuda and backend.has_ext():
+        return True
+    if x.is_cuda and not backend.allow_fallback():
+        raise RuntimeError('%s: the native extension is required on a GPU' % what)
+    return False
+
+
+def quantize_act(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """x [G, R, K] bf16 -> (q, s).  One launch of ``block_fp8_quantize_act_kernel`` on a GPU."""
+    if _native(x, 'block_fp8.quantize_act'):
+        backend.count_launch()
+        return backend.require_ext().block_fp8_quantize_act(x.contiguous())
+    return quantize_act_reference(x)
+
+
+def quantize_weight(w: torch.Tensor):
+    """w [G, R, C] bf16 -> (q, s, qT, sT), both orientations from one launch."""
+    if _native(w, 'block_fp8.quantize_weight'):
+        backend.count_launch()
+        return tuple(backend.require_ext().block_fp8_quantize_weight(w.contiguous()))
+    return quantize_weight_reference(w)
+
+
+def quantize_glu_weight(w1: torch.Tensor, w2: torch.Tensor):
+    """Gate / up weights [G, M, H] bf16 -> (qcat, scat, qglu, sglu) from one launch."""
+    if _native(w1, 'block_fp8.quantize_glu_weight'):
+        backend.count_launch()
+        return tuple(backend.require_ext().block_fp8_quantize_glu_weight(w1.contiguous(), w2.contiguous()))
+    return quantize_glu_weight_reference(w1, w2)
+
+
+def block_fp8_gemm(a, sa, b, sb, bias=None, aux=None, aux2=None, epilogue: int = EPI_NONE, act: str = 'silu',
+                   max_ctas: int = 0):
+    """``epilogue(a [G, M, K] @ b [G, N, K]^T)`` -> a list of bf16 results (see csrc/bindings.cpp: block_fp8_gemm)."""
+    if _native(a, 'block_fp8_gemm'):
+        backend.count_launch()
+        if bias is not None:
+            bias = bias.reshape(a.size(0), b.size(1)).to(torch.bfloat16).contiguous()
+        return backend.require_ext().block_fp8_gemm(a, sa, b, sb, bias, aux, aux2, int(epilogue), ACT_CODES[act], int(max_ctas))
+    return block_fp8_gemm_reference(a, sa, b, sb, bias, aux, aux2, epilogue, act)
+
+
+_WEIGHT_CACHE = {}
+
+
+def _cached(tensors, make):
+    """``make()`` cached like ``ops.mx.mx_weight``: valid until the next optimizer step or in-place change of any of
+    ``tensors`` (stamp ``(w._version, gemm._FP8_STEP)``, weakly anchored to the parameter)."""
+    import weakref
+    from . import gemm as _gemm
+    _gemm._ensure_step_hook()
+    anchors = tuple(w._base if w._base is not None else w for w in tensors)
+    key = tuple((id(a), w.data_ptr(), tuple(w.shape), tuple(w.stride())) for a, w in zip(anchors, tensors))
+    stamp = (tuple(w._version for w in tensors), _gemm._FP8_STEP[0])
+    hit = _WEIGHT_CACHE.get(key)
+    if hit is not None and hit[0] == stamp and all(r() is a for r, a in zip(hit[2], anchors)):
+        return hit[1]
+    val = make()
+    if len(_WEIGHT_CACHE) > 256:
+        for k in [k for k, v in _WEIGHT_CACHE.items() if any(r() is None for r in v[2])]:
+            del _WEIGHT_CACHE[k]
+    _WEIGHT_CACHE[key] = (stamp, val, tuple(weakref.ref(a) for a in anchors))
+    return val
+
+
+def weight(w: torch.Tensor):
+    """Cached (q, s, qT, sT) of a weight [G, R, C]."""
+    return _cached((w,), lambda: quantize_weight(w.detach()))
+
+
+def glu_weight(w1: torch.Tensor, w2: torch.Tensor):
+    """Cached (qcat, scat, qglu, sglu) of the gate / up weights [G, M, H]."""
+    return _cached((w1, w2), lambda: quantize_glu_weight(w1.detach(), w2.detach()))
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# expert FFNs
+# ------------------------------------------------------------------------------------------------------------------
+def can_use_block_fp8(x: torch.Tensor, *weights: torch.Tensor) -> bool:
+    """bf16 tensors on a GPU with the native extension, and every weight dimension a multiple of 128."""
+    return (x.is_cuda and backend.has_ext() and x.dtype == torch.bfloat16 and x.dim() == 3 and x.size(-1) % TILE == 0 and
+            all(w.dtype == torch.bfloat16 and w.dim() == 3 and w.size(1) % TILE == 0 and w.size(2) % TILE == 0 for w in weights))
+
+
+class FusedReluFFNBlockFp8(torch.autograd.Function):
+    """ReLU expert FFN ``relu(x @ w1^T + b1) @ w2 + b2`` (x [E, C, M], w1 [E, H, M], w2 [E, H, Mo]: the layout of
+    models/experts/ffn.py) with block-scaled e4m3 forward and data-gradient GEMMs and 16-bit weight-gradient GEMMs on the
+    master weights.  Same structure as ``ops.mx.FusedReluFFNMx``."""
+
+    @staticmethod
+    def forward(ctx: Any, x, w1, b1, w2, b2):
+        q1, s1, _, _ = weight(w1)
+        _, _, q2t, s2t = weight(w2)                                     # y = act @ W2: W2^T [Mo, H] K-major
+        act = block_fp8_gemm(*quantize_act(x), q1, s1, bias=b1, epilogue=EPI_RELU)[0]
+        y = block_fp8_gemm(*quantize_act(act), q2t, s2t, bias=b2)[0]
+        ctx.save_for_backward(x, w1, w2, act)
+        ctx.has_b1, ctx.has_b2 = b1 is not None, b2 is not None
+        return y
+
+    @staticmethod
+    def backward(ctx: Any, dy: torch.Tensor):
+        from . import gemm as _gemm
+        x, w1, w2, act = ctx.saved_tensors
+        dy = dy.contiguous()
+        q2, s2, _, _ = weight(w2)                                       # dh = dy @ W2^T: W2 [H, Mo] is K-major for it
+        dh = block_fp8_gemm(*quantize_act(dy), q2, s2, aux=act, epilogue=EPI_RELU_BWD)[0]
+        dw2 = _gemm.raw_gemm(act, dy, a_mn=True, b_mn=True) if ctx.needs_input_grad[3] else None
+        db2 = _gemm.column_sums(dy) if ctx.has_b2 and ctx.needs_input_grad[4] else None
+        dx = None
+        if ctx.needs_input_grad[0]:
+            _, _, q1t, s1t = weight(w1)                                 # dx = dh @ W1: W1^T [M, H] K-major
+            dx = block_fp8_gemm(*quantize_act(dh), q1t, s1t)[0]
+        dw1 = _gemm.raw_gemm(dh, x, a_mn=True, b_mn=True) if ctx.needs_input_grad[1] else None
+        db1 = _gemm.column_sums(dh) if ctx.has_b1 and ctx.needs_input_grad[2] else None
+        return dx, dw1, db1, dw2, db2
+
+
+def fused_relu_ffn_block_fp8(x, w1, b1, w2, b2):
+    b1 = None if b1 is None else b1.reshape(w1.size(0), -1)
+    b2 = None if b2 is None else b2.reshape(w2.size(0), -1)
+    return FusedReluFFNBlockFp8.apply(x, w1, b1, w2, b2)
+
+
+class FusedGLUFFNBlockFp8(torch.autograd.Function):
+    """SwiGLU expert ``(act(x @ W1) * (x @ W2)) @ W3`` (w1, w2 [E, M, H], w3 [E, H, Mo]: the layout of
+    models/experts/llama_ffn.py) with block-scaled e4m3 forward and data-gradient GEMMs:
+
+    * forward: one GLU launch on the interleaved gate / up copy writes h and the 16-bit g and u; then the down projection;
+    * backward: ``dy @ W3^T`` with the GLU-backward epilogue writes ``[dg du]`` side by side into one ``[E, C, 2H]``
+      buffer, and ``dx = [dg du] @ [W1 W2]^T`` is one GEMM with K = 2H on the same quantised blocks as the forward;
+      ``dW1``, ``dW2`` and ``dW3`` are 16-bit GEMMs on the master weights."""
+
+    @staticmethod
+    def forward(ctx: Any, x, w1, w2, w3, act: str):
+        _, _, qglu, sglu = glu_weight(w1, w2)
+        _, _, q3t, s3t = weight(w3)
+        h, g, u = block_fp8_gemm(*quantize_act(x), qglu, sglu, epilogue=EPI_GLU, act=act)
+        y = block_fp8_gemm(*quantize_act(h), q3t, s3t)[0]
+        ctx.act = act
+        ctx.save_for_backward(x, w1, w2, w3, g, u, h)
+        return y
+
+    @staticmethod
+    def backward(ctx: Any, dy: torch.Tensor):
+        from . import gemm as _gemm
+        x, w1, w2, w3, g, u, h = ctx.saved_tensors
+        dy = dy.contiguous()
+        H = g.size(-1)
+        q3, s3, _, _ = weight(w3)                                       # dh = dy @ W3^T: W3 [H, Mo] is K-major for it
+        dgu = block_fp8_gemm(*quantize_act(dy), q3, s3, aux=g, aux2=u, epilogue=EPI_GLU_BWD, act=ctx.act)[0]
+        dg, du = dgu[..., :H], dgu[..., H:]
+        dw3 = _gemm.raw_gemm(h, dy, a_mn=True, b_mn=True) if ctx.needs_input_grad[3] else None
+        dw1 = _gemm.raw_gemm(x, dg, a_mn=True, b_mn=True) if ctx.needs_input_grad[1] else None
+        dw2 = _gemm.raw_gemm(x, du, a_mn=True, b_mn=True) if ctx.needs_input_grad[2] else None
+        dx = None
+        if ctx.needs_input_grad[0]:
+            qcat, scat, _, _ = glu_weight(w1, w2)
+            dx = block_fp8_gemm(*quantize_act(dgu), qcat, scat)[0]
+        return dx, dw1, dw2, dw3, None
+
+
+def fused_glu_ffn_block_fp8(x, w1, w2, w3, act='silu'):
+    return FusedGLUFFNBlockFp8.apply(x, w1, w2, w3, act)

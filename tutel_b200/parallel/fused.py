@@ -443,8 +443,8 @@ def engine_for(layer, x: torch.Tensor, crit, d: int):
     if isinstance(ex, FusedExpertsNetwork):
         if ex._act_kind not in G.FWD_EPILOGUE or ex.skip_expert or (ex.fp8 and ex._act_kind != 'relu'):
             return None
-        if getattr(ex, 'mx', False):
-            return None     # MX block-scaled experts run on the unfused path (ops/mx.py)
+        if getattr(ex, 'mx', False) or getattr(ex, 'block', False):
+            return None     # MX and block-fp8 experts run on the unfused path (ops/mx.py, ops/block_fp8.py)
         if ex.fp8 and (layer.model_dim % 16 or ex.hidden_size % 16 or ex.output_dim % 16):
             return None
         if ex.batched_fc1_w.dtype != x.dtype or (layer.model_dim % 8) or (ex.hidden_size % 8) or (ex.output_dim % 8):
@@ -453,6 +453,8 @@ def engine_for(layer, x: torch.Tensor, crit, d: int):
     elif isinstance(ex, LlamaFFNNetwork):
         if G.classify_activation(ex.activation_fn) not in G.ACT_CODES or ex.W_fc1.dtype != x.dtype:
             return None
+        if getattr(ex, 'block', False):
+            return None     # block-fp8 experts run on the unfused path (ops/block_fp8.py)
         align = 16 if ex.fp8 else 8
         if any(int(v) % align for v in ex.full_shapes['W_fc1'][1:]) or int(ex.full_shapes['W_fc3'][2]) % align:
             return None
