@@ -21,6 +21,14 @@ module alone is timed the same way on the dispatch buffer of one call (`experts_
 kernels `skinny_ffn_fp8_kernel` / `skinny_glu_ffn_fp8_kernel` stream those copies, x stays 16 bit).  With it,
 `active_weight_bytes` and both `*_GBps` count the bytes that path needs - the e4m3 copies, their fp32 scales and any
 biases - not the bytes of the 16-bit master parameters.  `rel_err_vs_padded` then compares with the padded fp8 path.
+
+`--fp8_weights` (`llama_ffn`, bfloat16) builds the experts with `weight_format='fp8_block'`: block-scaled e4m3 weights
+(DeepSeek-V3 checkpoint format, one fp32 scale per 128 x 128 block) and no 16-bit copy, loaded from the export of a bf16
+`fp8='block'` layer.  Dropless decoding streams them with `skinny_glu_ffn_block_fp8_kernel`; larger steps run the block
+GEMMs with device row counts.  `active_weight_bytes` counts the e4m3 bytes and their scales.  `expert_memory_bytes` is
+what the expert module holds; with `--fp8_weights`, `bf16_block_expert_memory_bytes` is what the source bf16
+`fp8='block'` layer held after one forward (its parameters and the cached e4m3 copies).
+`--shared_experts N` adds N shared experts (DeepSeek-V3: 1).
 """
 import argparse
 import json
@@ -40,10 +48,15 @@ ap.add_argument('--hidden', type=int, default=0, help='hidden size per expert (d
 ap.add_argument('--dtype', default='float32')
 ap.add_argument('--iters', type=int, default=50)
 ap.add_argument('--fp8', action='store_true', help='fp8 experts (e4m3 weights with per-row scales); 16-bit --dtype only')
+ap.add_argument('--fp8_weights', action='store_true',
+                help="llama_ffn, bfloat16: stored block-fp8 experts (weight_format='fp8_block') with no 16-bit copy")
+ap.add_argument('--shared_experts', type=int, default=0, help='shared experts of the routed type (0: none)')
 ap.add_argument('--graph', action='store_true', help='ours only: replay the forward as one CUDA graph (tutel_b200.utils.graph)')
 args = ap.parse_args()
 hidden = args.hidden or args.dim
 assert not args.fp8 or (args.impl == 'ours' and args.dtype in ('bfloat16', 'float16')), '--fp8: ours, with a 16-bit --dtype'
+assert not args.fp8_weights or (args.impl == 'ours' and args.dtype == 'bfloat16' and args.expert_type == 'llama_ffn' and
+                                not args.fp8), '--fp8_weights: ours, llama_ffn, bfloat16, without --fp8'
 if args.impl == 'reference':
     sys.path.insert(0, os.path.join(ROOT, 'baseline', '_ref'))
     from tutel import moe, system
@@ -62,9 +75,38 @@ if args.expert_type == 'ffn':
     experts['activation_fn'] = lambda x: F.relu(x)
 if args.fp8:
     experts['fp8'] = True
-with torch.device(dev):        # initialise the (multi-GB) weights on the GPU
-    layer = moe.moe_layer(gate_type={'type': 'top', 'k': args.top_k, 'capacity_factor': 0.0}, model_dim=args.dim,
-                          experts=experts, seeds=(1, 1, 1)).eval()
+shared = {'shared_experts': {'num_experts': args.shared_experts}} if args.shared_experts else {}
+
+
+def build(spec):
+    with torch.device(dev):        # initialise the (multi-GB) weights on the GPU
+        return moe.moe_layer(gate_type={'type': 'top', 'k': args.top_k, 'capacity_factor': 0.0}, model_dim=args.dim,
+                             experts=spec, seeds=(1, 1, 1), **shared).eval()
+
+
+def module_bytes(m):
+    return sum(t.numel() * t.element_size() for t in list(m.parameters()) + list(m.buffers()))
+
+
+bf16_block_bytes = None
+if args.fp8_weights:
+    from tutel_b200.ops import block_fp8 as BF8
+    src = build(dict(experts, fp8='block'))
+    with torch.no_grad():
+        src(torch.randn(1, 256, args.dim, device=dev))        # one padded forward: the block path caches its e4m3 copies
+    cached = sum(t.numel() * t.element_size() for v in BF8._WEIGHT_CACHE.values() for t in v[1])
+    bf16_block_bytes = module_bytes(src.experts) + cached
+    layer = build(dict(experts, weight_format='fp8_block'))
+    layer.load_state_dict({k: v for k, v in src.state_dict().items() if not k.startswith(('experts.', 'shared_experts.'))},
+                          strict=False)
+    layer.experts.load_fp8_block_weights(*src.experts.export_fp8_block_weights())
+    if args.shared_experts:
+        layer.shared_experts.load_fp8_block_weights(*src.shared_experts.export_fp8_block_weights())
+    del src
+    BF8._WEIGHT_CACHE.clear()
+    torch.cuda.empty_cache()
+else:
+    layer = build(experts)
 x = torch.randn(1, args.tokens, args.dim, device=dev)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 eager = (lambda t: layer(t, megablocks_size=args.megablocks_size)) if args.megablocks_size > 0 else (lambda t: layer(t))
@@ -105,6 +147,8 @@ def expert_bytes():
     """Weight bytes one expert's forward reads: the parameters, or with --fp8 the e4m3 copies (1 byte per weight), one
     fp32 scale per quantised row (ops/gemm.py: fp8_weight) and the 16-bit biases."""
     e = layer.experts
+    if args.fp8_weights:                   # e4m3 W_gate_up [2H, M] + W_down [M, H] and their fp32 block scales
+        return module_bytes(e) // args.experts
     if not args.fp8:
         return sum(p.numel() * p.element_size() for p in e.parameters()) // args.experts
     M, H, N = args.dim, hidden, args.dim
@@ -119,9 +163,12 @@ median, expert_median = times[len(times) // 2], expert_times[len(expert_times) /
 config = 'dropless cf=0 top-%d E=%d tokens=%d dim=%d hidden=%d %s %s megablocks_size=%d%s%s' % (
     args.top_k, args.experts, args.tokens, args.dim, hidden, args.expert_type, args.dtype, args.megablocks_size,
     ' fp8' if args.fp8 else '', ' cuda-graph' if args.graph and args.impl == 'ours' else '')
+config += ' fp8_weights' if args.fp8_weights else ''
+config += ' shared=%d' % args.shared_experts if args.shared_experts else ''
 print(json.dumps({'impl': args.impl, 'config': config, 'median_ms': median, 'min_ms': times[0], 'max_ms': times[-1],
     'experts_median_ms': expert_median, 'active_experts': active, 'active_weight_bytes': active * bytes_per_expert,
     'active_weight_GBps': active * bytes_per_expert / (median * 1e-3) / 1e9,
     'experts_active_weight_GBps': active * bytes_per_expert / (expert_median * 1e-3) / 1e9,
     'rel_err_vs_padded': float((y.float() - padded.float()).norm() / padded.float().norm()),
-    'checksum': float(y.float().abs().sum())}))
+    'checksum': float(y.float().abs().sum()), 'expert_memory_bytes': module_bytes(layer.experts),
+    'bf16_block_expert_memory_bytes': bf16_block_bytes}))

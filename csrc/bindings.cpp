@@ -783,9 +783,10 @@ std::vector<at::Tensor> block_fp8_quantize_glu_weight(const at::Tensor& w1, cons
 // epilogue 0 none / 1 ReLU (+ bias [G, N]) -> [d [G, M, N]];  2 ReLU backward (aux = forward activation) -> [d];
 // 3 GLU (b = the interleaved gate / up copy, sb [G, N / 64, K / 128]) -> [h, g, u], each [G, M, N / 2];
 // 4 GLU backward (acc = dh, aux = g, aux2 = u) -> [dgu [G, M, 2N]] with dg in columns [0, N) and du in [N, 2N).
-std::vector<at::Tensor> block_fp8_gemm(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
-                                       const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
-                                       const c10::optional<at::Tensor>& aux2, int64_t epilogue, int64_t act, int64_t max_ctas) {
+std::vector<at::Tensor> block_fp8_gemm_impl(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                            const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
+                                            const c10::optional<at::Tensor>& aux2, int64_t epilogue, int64_t act, int64_t max_ctas,
+                                            const int* row_counts) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && sa.is_cuda() && sb.is_cuda() && a.dim() == 3 && b.dim() == 3 && sa.dim() == 3 &&
               sb.dim() == 3, "block_fp8_gemm: 3-D CUDA tensors expected");
   TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && sa.is_contiguous() && sb.is_contiguous(),
@@ -837,10 +838,29 @@ std::vector<at::Tensor> block_fp8_gemm(const at::Tensor& a, const at::Tensor& sa
   p.epilogue = static_cast<int>(epilogue);
   p.act = static_cast<int>(act);
   p.max_ctas = static_cast<int>(max_ctas);
+  p.row_counts = row_counts;
   const char* why = nullptr;
   cudaError_t e = tb::block_fp8_gemm_launch(p, cur_stream(), &why);
   TORCH_CHECK(e == cudaSuccess, "block_fp8_gemm: ", why ? why : cudaGetErrorString(e));
   return out;
+}
+
+std::vector<at::Tensor> block_fp8_gemm(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                       const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
+                                       const c10::optional<at::Tensor>& aux2, int64_t epilogue, int64_t act, int64_t max_ctas) {
+  return block_fp8_gemm_impl(a, sa, b, sb, bias, aux, aux2, epilogue, act, max_ctas, nullptr);
+}
+
+// block_fp8_gemm with device row counts (int32 [G]): rows r >= row_counts[g] of every output are zero, and tiles that
+// start at or past the count are skipped.
+std::vector<at::Tensor> block_fp8_gemm_counts(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                              const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
+                                              const c10::optional<at::Tensor>& aux2, int64_t epilogue, int64_t act, int64_t max_ctas,
+                                              const at::Tensor& row_counts) {
+  TORCH_CHECK(row_counts.is_cuda() && row_counts.scalar_type() == at::kInt && row_counts.is_contiguous() &&
+                  row_counts.numel() == a.size(0) && row_counts.device() == a.device(),
+              "block_fp8_gemm: row_counts must be a contiguous int32 CUDA tensor [G] on a's device");
+  return block_fp8_gemm_impl(a, sa, b, sb, bias, aux, aux2, epilogue, act, max_ctas, row_counts.data_ptr<int>());
 }
 
 // Gated-linear-unit GEMMs (SwiGLU / GeGLU / ReGLU experts; reference: tutel/experts/llama_ffn.py:38-41 runs three
@@ -1081,6 +1101,36 @@ at::Tensor skinny_glu_ffn_fp8(const at::Tensor& x, const at::Tensor& q1t, const 
   return y;
 }
 
+// x [G, R, M] bf16, qglu [G, 2H, M] e4m3 (gate / up interleaved every 64 rows) + sglu [G, 2H / 64, M / 128],
+// q3t [G, N, H] e4m3 + s3t [G, N / 128, H / 128], counts int [G] or None -> fp32 [G, R, N], rows past the counts zero
+at::Tensor skinny_glu_ffn_block_fp8(const at::Tensor& x, const at::Tensor& qglu, const at::Tensor& sglu, const at::Tensor& q3t,
+                                    const at::Tensor& s3t, const c10::optional<at::Tensor>& counts, int64_t act) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 3 && x.is_contiguous() && x.scalar_type() == at::kBFloat16,
+              "skinny_glu_ffn_block_fp8: x must be a contiguous bf16 CUDA tensor [G, R, M]");
+  const int64_t G = x.size(0), R = x.size(1), M = x.size(2);
+  TORCH_CHECK(qglu.dim() == 3 && q3t.dim() == 3, "skinny_glu_ffn_block_fp8: 3-D weights expected");
+  const int64_t H = qglu.size(1) / 2, N = q3t.size(1);
+  TORCH_CHECK(M % 128 == 0 && H % 128 == 0 && N % 128 == 0, "skinny_glu_ffn_block_fp8: M, H and N must be multiples of 128");
+  auto ok = [&](const at::Tensor& t, at::ScalarType dt, int64_t d0, int64_t d1, int64_t d2) {
+    return t.is_cuda() && t.device() == x.device() && t.is_contiguous() && t.scalar_type() == dt && t.dim() == 3 &&
+           t.size(0) == d0 && t.size(1) == d1 && t.size(2) == d2;
+  };
+  TORCH_CHECK(ok(qglu, at::kFloat8_e4m3fn, G, 2 * H, M), "skinny_glu_ffn_block_fp8: qglu must be a contiguous e4m3 CUDA tensor [G, 2H, M]");
+  TORCH_CHECK(ok(sglu, at::kFloat, G, 2 * H / 64, M / 128),
+              "skinny_glu_ffn_block_fp8: sglu must be a contiguous fp32 CUDA tensor [G, 2H / 64, M / 128]");
+  TORCH_CHECK(ok(q3t, at::kFloat8_e4m3fn, G, N, H), "skinny_glu_ffn_block_fp8: q3t must be a contiguous e4m3 CUDA tensor [G, N, H]");
+  TORCH_CHECK(ok(s3t, at::kFloat, G, N / 128, H / 128),
+              "skinny_glu_ffn_block_fp8: s3t must be a contiguous fp32 CUDA tensor [G, N / 128, H / 128]");
+  TORCH_CHECK(act >= 1 && act <= 3, "skinny_glu_ffn_block_fp8: act must be 1 (relu), 2 (gelu) or 3 (silu)");
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor y = at::zeros({G, R, N}, x.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::skinny_grouped_glu_ffn_block_fp8(x.data_ptr(), qglu.data_ptr(), sglu.data_ptr<float>(), q3t.data_ptr(),
+                                                     s3t.data_ptr<float>(), y.data_ptr<float>(), opt_counts(counts, G),
+                                                     static_cast<int>(G), static_cast<int>(R), static_cast<int>(M),
+                                                     static_cast<int>(H), static_cast<int>(N), static_cast<int>(act), cur_stream()));
+  return y;
+}
+
 }  // namespace
 
 void register_symm_bindings(pybind11::module& m);  // symm_heap.cpp / p2p bindings
@@ -1129,6 +1179,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("block_fp8_quantize_weight", &block_fp8_quantize_weight);
   m.def("block_fp8_quantize_glu_weight", &block_fp8_quantize_glu_weight);
   m.def("block_fp8_gemm", &block_fp8_gemm);
+  m.def("block_fp8_gemm", &block_fp8_gemm_counts);   // + row_counts
+  m.def("skinny_glu_ffn_block_fp8", &skinny_glu_ffn_block_fp8);
   register_symm_bindings(m);
   register_cpu_bindings(m);
   register_jit_bindings(m);

@@ -64,6 +64,7 @@ struct Args {
   long long ld_aux, aux_group_stride;
   long long num_tiles;
   int epi, act;
+  const int* row_counts;               // COUNTS: live rows of each group (device); null otherwise
 };
 
 __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
@@ -102,6 +103,14 @@ __device__ __forceinline__ void act_and_grad(int act, float g, float& a, float& 
   }
 }
 
+// Live rows of group g: all M, or min(row_counts[g], M) with device row counts (dropless prefill).  The producer and the
+// consumers both derive a tile's skip from this one value, so they walk the same stages of the mbarrier ring.
+template <bool COUNTS>
+__device__ __forceinline__ int live_rows(const Args& args, int g) {
+  return COUNTS ? max(0, min(args.row_counts[g], args.M)) : args.M;
+}
+
+template <bool COUNTS>
 __global__ void __launch_bounds__(kThreads, 1)
 block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Args args) {
   using C = Cfg;
@@ -143,6 +152,7 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         int g, m_blk, n_blk;
         decode_tile(t, args.tiles_m, args.tiles_n, g, m_blk, n_blk);
         const int m0 = m_blk * kBM, n0 = n_blk * kBN;
+        if (COUNTS && m0 >= live_rows<COUNTS>(args, g)) continue;      // no stage is filled for a tile past the count
         const float* sa_g = args.sa + static_cast<long long>(g) * num_kb * args.sa_rows + m0;
         for (int kb = 0; kb < num_kb; ++kb) {
           ptx::mbar_wait_quiet(empty_bar(s), ph ^ 1u);
@@ -180,7 +190,10 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       float acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < num_kb; ++kb) {
+      const int live = live_rows<COUNTS>(args, g);
+      // a tile past the count takes no stage (as in the producer) and stores zeros
+      const int steps = COUNTS && m_blk * kBM >= live ? 0 : num_kb;
+      for (int kb = 0; kb < steps; ++kb) {
         ptx::mbar_wait_quiet(full_bar(s), ph);
         const uint32_t a_lo = (((smem_a(s) + static_cast<uint32_t>(wg) * 8192u) >> 4) & 0x3FFFu) | (1u << 16);
         const uint32_t b_lo = ((smem_b(s) >> 4) & 0x3FFFu) | (1u << 16);
@@ -194,7 +207,7 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         const float sa0 = __uint_as_float(lds_u32(smem_sa(s) + 4u * r0));
         const float sa1 = __uint_as_float(lds_u32(smem_sa(s) + 4u * (r0 + 8)));
         const float s00 = sa0 * sbl, s01 = sa0 * sbh, s10 = sa1 * sbl, s11 = sa1 * sbh;
-        if (kb + 1 < num_kb) { sbl = __ldg(sb_lo + kb + 1); sbh = __ldg(sb_hi + kb + 1); }
+        if (kb + 1 < steps) { sbl = __ldg(sb_lo + kb + 1); sbh = __ldg(sb_hi + kb + 1); }
         ptx::wgmma_wait<0>();
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(empty_bar(s));
@@ -218,6 +231,18 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         const int row = m_blk * kBM + r0 + 8 * h;
         if (row >= args.M) continue;
         const long long drow = goff + static_cast<long long>(row) * args.ldd;
+        if (COUNTS && row >= live) {
+          // rows past the count are zero in every output (their A rows are never read into the result)
+          const __nv_bfloat162 z = __floats2bfloat162_rn(0.f, 0.f);
+          const int w = epi == BF8_EPI_GLU ? 8 : 16;
+          const long long o = drow + (epi == BF8_EPI_GLU ? n_blk * 64 : n_blk * kBN) + c0;
+          for (int j = 0; j < w; ++j) {
+            *reinterpret_cast<__nv_bfloat162*>(args.d + o + 8 * j) = z;
+            if (epi == BF8_EPI_GLU || epi == BF8_EPI_GLU_BWD) *reinterpret_cast<__nv_bfloat162*>(args.d2 + o + 8 * j) = z;
+            if (epi == BF8_EPI_GLU) *reinterpret_cast<__nv_bfloat162*>(args.d3 + o + 8 * j) = z;
+          }
+          continue;
+        }
         if (epi == BF8_EPI_GLU) {
           // column 8 j + c0 (j < 8) is gate column n_blk * 64 + 8 j + c0; its up partner sits 64 columns on, at j + 8
           const long long o = drow + n_blk * 64 + c0;
@@ -494,10 +519,13 @@ cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t str
   a.aux_group_stride = p.aux_group_stride;
   a.epi = p.epilogue;
   a.act = p.act;
+  a.row_counts = p.row_counts;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    if (attr_err == cudaSuccess)
+      attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
   });
   if (attr_err != cudaSuccess) return attr_err;
   a.num_tiles = static_cast<long long>(a.tiles_m) * a.tiles_n * p.G;
@@ -510,7 +538,10 @@ cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t str
   long long ctas = sms;                                                    // one resident CTA per SM
   if (p.max_ctas > 0) ctas = std::max<long long>(1, std::min<long long>(ctas, p.max_ctas));
   const unsigned grid = static_cast<unsigned>(std::min<long long>(a.num_tiles, ctas));
-  block_fp8_gemm_kernel<<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
+  if (p.row_counts != nullptr)
+    block_fp8_gemm_kernel<true><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
+  else
+    block_fp8_gemm_kernel<false><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
   return cudaGetLastError();
 }
 

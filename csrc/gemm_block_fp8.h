@@ -53,6 +53,10 @@ struct BlockFp8GemmProblem {
   int epilogue = 0;              // BlockFp8Epilogue
   int act = 3;                   // GLU / GLU_BWD: 1 ReLU, 2 GELU, 3 SiLU
   int max_ctas = 0;              // 0: one CTA per SM
+  // Optional device int32 [G]: only rows r < row_counts[g] of group g are live (dropless prefill).  Tiles whose first row
+  // is at or past the count are skipped (no operand is loaded for them); every output row past the count is stored as
+  // zero.  Null: all M rows, the same kernel as without the field.
+  const int* row_counts = nullptr;
 };
 
 cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t stream, const char** why = nullptr);

@@ -167,5 +167,12 @@ cudaError_t skinny_grouped_ffn_fp8(const void* x, const void* q1, const float* s
 cudaError_t skinny_grouped_glu_ffn_fp8(const void* x, const void* q1t, const float* s1, const void* q2t, const float* s2,
                                        const void* q3t, const float* s3, float* y, const int* counts, int G, int rows_cap,
                                        int M, int H, int N, int act, int elem_type, cudaStream_t stream);
+//   skinny_grouped_glu_ffn_block_fp8: the same SwiGLU expert on block-scaled e4m3 weights (DeepSeek-V3 format), x bf16:
+//       Qglu [G, 2H, M]: W1^T and W2^T interleaved every 64 rows, Sglu fp32 [G, 2H / 64, M / 128];
+//       Q3t [G, N, H], S3t fp32 [G, N / 128, H / 128]  (one scale per 128 x 128 block, applied per 128-deep K block).
+// cudaErrorInvalidValue for unaligned pointers, M, H or N not a multiple of 128, or act outside 1..3.
+cudaError_t skinny_grouped_glu_ffn_block_fp8(const void* x, const void* qglu, const float* sglu, const void* q3t,
+                                             const float* s3t, float* y, const int* counts, int G, int rows_cap, int M, int H,
+                                             int N, int act, cudaStream_t stream);
 
 }  // namespace tb

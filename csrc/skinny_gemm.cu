@@ -581,10 +581,12 @@ __device__ __forceinline__ void fp8_row_dots(const float* __restrict__ xs, const
 // q points at the slice's first column of the [N, H] matrix; hsm holds h [ROWS][kHS8] in the chunk-split layout.  Lane
 // (sub, c) of a warp takes hidden units [16c, 16c + 16) of output sub (4 outputs per warp and load, each a whole line); its
 // 16 h values per row stay in registers for the whole pass.  After the 8-lane reduction lane c adds row c.
-template <typename T, int ROWS>
+// BLOCK: q is block-scaled (128 x 128) and the slice is one 128-deep K block of it, so output n's reduced partial takes the
+// single scale s[(n / 128) * s_ld] (s points at the slice's block column, s_ld = H / 128); otherwise the row scale s[n].
+template <typename T, int ROWS, bool BLOCK = false>
 __device__ __forceinline__ void fp8_layer2(const float* __restrict__ hsm, const uint8_t* __restrict__ q,
                                            const float* __restrict__ s, const T* __restrict__ bias,
-                                           float* __restrict__ yrow0, int nr, int hs, int H, int N) {
+                                           float* __restrict__ yrow0, int nr, int hs, int H, int N, int s_ld = 0) {
   constexpr int U = ROWS <= 2 ? 8 : 4;          // loads in flight per lane
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = lane & 7, sub = lane >> 3;
@@ -622,7 +624,7 @@ __device__ __forceinline__ void fp8_layer2(const float* __restrict__ hsm, const 
         float v = acc[0];
 #pragma unroll
         for (int r = 1; r < ROWS; ++r) if (c == r) v = acc[r];
-        v *= s[n];
+        v *= s[BLOCK ? (n >> 7) * s_ld : n];
         if (bias != nullptr) v += ldf<T>(bias + n);
         atomicAdd(yrow0 + static_cast<long long>(c) * N + n, v);
       }
@@ -742,6 +744,157 @@ skinny_glu_ffn_fp8_kernel(const T* __restrict__ x, const uint8_t* __restrict__ q
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Block-scaled fp8 SwiGLU expert (the DeepSeek-V3 checkpoint format), W8A16, one launch
+// ------------------------------------------------------------------------------------------------
+// Operands are the stored weights of LlamaFFNNetwork(weight_format='fp8_block'), which are also the B operands of the
+// block GEMM's forward (ops/block_fp8.py):
+//   qglu [G, 2H, M] e4m3: W1^T and W2^T interleaved every 64 rows (row 128 t + j = gate unit 64 t + j, row 128 t + 64 + j
+//        = its up partner), sglu [G, 2H / 64, M / 128] fp32, one scale per 64 rows and 128-deep K block;
+//   q3t  [G, N, H] e4m3 (the down projection, K = H contiguous), s3t [G, N / 128, H / 128] fp32.
+// Block (g, s) owns hidden units [128 s, 128 s + 128): rows [256 s, 256 s + 256) of qglu, two whole interleave groups, so
+// a gate row and its up partner are read by the same warp in one loop.
+//   layer 1: one hidden unit per warp and pass; lanes stride M in 16-byte (16-element) chunks.  A chunk lies inside one
+//            128-deep K block (chunk c in block c / 8): its 16-term fp32 partial sum is multiplied once by that block's
+//            scale and added to the lane's sum, the per-block promotion of the GEMM, never a per-element dequantisation;
+//   layer 2: fp8_layer2<BLOCK>: the block's 128-unit slice of q3t row n is one 128-byte line and one 128-deep K block, so
+//            the 8-lane reduced partial takes the one scale s3t[n / 128, s] before its fp32 atomic add.
+// x stays bf16 in shared memory (two 16-byte halves of a chunk K/16 uint4s apart, so lanes read consecutive 16 bytes):
+// 8 M + 2 KB bytes per block, 58 KB at M = 7168 (DeepSeek-V3, Kimi-K2), under the 100 KB of two resident blocks of 256
+// threads per SM (<= 128 registers: __launch_bounds__(256, 2)); fp32 staging (16 M + 2 KB) would not fit M = 7168.
+// Every active expert's bytes are read once per kFfnRows rows; an expert without rows costs one block exit.
+__device__ __forceinline__ void bf16x8(const uint4 u, float* f) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    f[2 * i] = __uint_as_float(w[i] << 16);
+    f[2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+  }
+}
+
+// Rows [0, nr) of x (bf16 [nr, K], K % 16 == 0) into xs [kFfnRows][K]; half p of chunk c of a row at uint4 p * K/16 + c.
+// Passes of 3 rows run the kFfnRows specialisation, so the missing row is zeroed.
+__device__ __forceinline__ void stage_rows_bf16(uint4* __restrict__ xs, const __nv_bfloat16* __restrict__ xrow0, int nr, int K) {
+  const int K8 = K >> 3, K16 = K >> 4;
+  __syncthreads();
+  for (int i = threadIdx.x; i < nr * K8; i += 256) {
+    const int r = i / K8, h = i - r * K8;              // h: 8-element half-chunk of row r
+    xs[r * K8 + (h & 1) * K16 + (h >> 1)] = __ldg(reinterpret_cast<const uint4*>(xrow0) + i);
+  }
+  if (nr > 2)
+    for (int i = threadIdx.x + nr * K8; i < kFfnRows * K8; i += 256) xs[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+}
+
+// Warp-wide gate and up dot products of ROWS staged rows with one gate row and one up row of K e4m3 weights whose K-block
+// scales are sg[K / 128] and su[K / 128]; every lane gets the full sums.
+template <int ROWS>
+__device__ __forceinline__ void block_glu_dots(const uint4* __restrict__ xs, const uint8_t* __restrict__ qg,
+                                               const uint8_t* __restrict__ qu, const float* __restrict__ sg,
+                                               const float* __restrict__ su, int K, float (&acc)[2][ROWS]) {
+  const int lane = threadIdx.x & 31;
+  const int K16 = K >> 4, K8 = K >> 3;
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) acc[m][r] = 0.0f;
+  for (int c = lane; c < K16; c += 32 * 4) {
+    uint4 raw[4][2];
+    float sc[4][2];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int cc = c + 32 * u;
+      const bool in = cc < K16;
+      raw[u][0] = in ? __ldcs(reinterpret_cast<const uint4*>(qg) + cc) : make_uint4(0, 0, 0, 0);
+      raw[u][1] = in ? __ldcs(reinterpret_cast<const uint4*>(qu) + cc) : make_uint4(0, 0, 0, 0);
+      sc[u][0] = in ? __ldg(sg + (cc >> 3)) : 0.0f;
+      sc[u][1] = in ? __ldg(su + (cc >> 3)) : 0.0f;
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int cc = c + 32 * u;
+      if (cc < K16) {
+        float wv[2][16];
+        e4m3x16(raw[u][0], wv[0]);
+        e4m3x16(raw[u][1], wv[1]);
+#pragma unroll
+        for (int r = 0; r < ROWS; ++r) {
+          float xf[16];
+          bf16x8(xs[r * K8 + cc], xf);
+          bf16x8(xs[r * K8 + K16 + cc], xf + 8);
+#pragma unroll
+          for (int m = 0; m < 2; ++m) {
+            float part = 0.0f;
+#pragma unroll
+            for (int e = 0; e < 16; ++e) part = fmaf(xf[e], wv[m][e], part);
+            acc[m][r] = fmaf(part, sc[u][m], acc[m][r]);
+          }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc[m][r] += __shfl_xor_sync(0xffffffffu, acc[m][r], o);
+}
+
+template <int ROWS>
+__device__ __forceinline__ void glu_block_fp8_pass(const uint4* __restrict__ xs, float* __restrict__ hsm,
+                                                   const uint8_t* __restrict__ qglu_s, const float* __restrict__ sglu_s,
+                                                   const uint8_t* __restrict__ q3g, const float* __restrict__ s3g,
+                                                   float* __restrict__ yrow0, int nr, int M, int H, int N, int act) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int KB = M >> 7;
+  for (int j = warp; j < kHS8; j += 8) {
+    const int t = j >> 6, jj = j & 63;                 // interleave group of the slice, unit inside it
+    const uint8_t* qg = qglu_s + static_cast<long long>(128 * t + jj) * M;
+    float acc[2][ROWS];
+    block_glu_dots<ROWS>(xs, qg, qg + 64LL * M, sglu_s + (2 * t) * KB, sglu_s + (2 * t + 1) * KB, M, acc);
+    if (lane < ROWS) {
+      float gv = acc[0][0], uv = acc[1][0];
+#pragma unroll
+      for (int r = 1; r < ROWS; ++r)
+        if (lane == r) { gv = acc[0][r]; uv = acc[1][r]; }
+      hsm[lane * kHS8 + split_index(j, kHS8)] = ffn_act(gv, act) * uv;
+    }
+  }
+  __syncthreads();
+  fp8_layer2<__nv_bfloat16, ROWS, true>(hsm, q3g, s3g, nullptr, yrow0, nr, kHS8, H, N, H >> 7);
+}
+
+__global__ void __launch_bounds__(256, 2)
+skinny_glu_ffn_block_fp8_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict__ qglu,
+                                const float* __restrict__ sglu, const uint8_t* __restrict__ q3t,
+                                const float* __restrict__ s3t, float* __restrict__ y, const int* __restrict__ counts,
+                                int rows_cap, int M, int H, int N, int act) {
+  extern __shared__ __align__(16) uint4 smb[];   // x rows [kFfnRows][M] bf16, chunk-split | hidden slice [kFfnRows][kHS8] fp32
+  const int g = blockIdx.y;
+  const int count = counts != nullptr ? min(counts[g], rows_cap) : rows_cap;
+  if (count <= 0) return;
+  const int s = blockIdx.x, h0 = s * kHS8;
+  uint4* xs = smb;
+  float* hsm = reinterpret_cast<float*>(smb + kFfnRows * (M >> 3));
+  const __nv_bfloat16* xg = x + static_cast<long long>(g) * rows_cap * M;
+  const uint8_t* qglu_s = qglu + (static_cast<long long>(g) * 2 * H + 2 * h0) * M;
+  const float* sglu_s = sglu + (static_cast<long long>(g) * (H >> 5) + (h0 >> 5)) * (M >> 7);
+  const uint8_t* q3g = q3t + static_cast<long long>(g) * N * H + h0;
+  const float* s3g = s3t + static_cast<long long>(g) * (N >> 7) * (H >> 7) + s;
+  float* yg = y + static_cast<long long>(g) * rows_cap * N;
+
+  for (int r0 = 0; r0 < count; r0 += kFfnRows) {
+    const int nr = min(kFfnRows, count - r0);
+    stage_rows_bf16(xs, xg + static_cast<long long>(r0) * M, nr, M);
+    float* yrow0 = yg + static_cast<long long>(r0) * N;
+    if (nr == 1) glu_block_fp8_pass<1>(xs, hsm, qglu_s, sglu_s, q3g, s3g, yrow0, nr, M, H, N, act);
+    else if (nr == 2) glu_block_fp8_pass<2>(xs, hsm, qglu_s, sglu_s, q3g, s3g, yrow0, nr, M, H, N, act);
+    else glu_block_fp8_pass<kFfnRows>(xs, hsm, qglu_s, sglu_s, q3g, s3g, yrow0, nr, M, H, N, act);
+  }
+}
+
+
 // Dynamic shared memory of both fp8 kernels: the staged x rows and the hidden slice (K % 16 == 0 keeps both 16-byte aligned).
 size_t fp8_smem_bytes(int K) { return sizeof(float) * (static_cast<size_t>(kFfnRows) * K + kFfnRows * kHS8); }
 
@@ -781,6 +934,9 @@ cudaError_t launch_glu_ffn_fp8(const void* x, const void* q1t, const float* s1, 
                                     rows_cap, M, H, N, act);
   return cudaGetLastError();
 }
+
+// Dynamic shared memory of the block-scaled kernel: bf16 x rows and the fp32 hidden slice.
+size_t block_fp8_smem_bytes(int M) { return 2 * static_cast<size_t>(kFfnRows) * M + sizeof(float) * kFfnRows * kHS8; }
 
 }  // namespace
 
@@ -846,6 +1002,23 @@ cudaError_t skinny_grouped_glu_ffn_fp8(const void* x, const void* q1t, const flo
       return launch_glu_ffn_fp8<__nv_bfloat16>(x, q1t, s1, q2t, s2, q3t, s3, y, counts, G, rows_cap, M, H, N, act, stream);
   }
   return cudaErrorInvalidValue;
+}
+
+cudaError_t skinny_grouped_glu_ffn_block_fp8(const void* x, const void* qglu, const float* sglu, const void* q3t,
+                                             const float* s3t, float* y, const int* counts, int G, int rows_cap, int M, int H,
+                                             int N, int act, cudaStream_t stream) {
+  if (G <= 0 || rows_cap <= 0 || M <= 0 || H <= 0 || N <= 0) return cudaSuccess;
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(qglu) | reinterpret_cast<uintptr_t>(q3t)) & 15)
+    return cudaErrorInvalidValue;
+  if (M % 128 || H % 128 || N % 128 || act < 1 || act > 3) return cudaErrorInvalidValue;
+  const size_t smem = block_fp8_smem_bytes(M);
+  auto* kern = skinny_glu_ffn_block_fp8_kernel;
+  cudaError_t e = fp8_opt_in(kern, smem);
+  if (e != cudaSuccess) return e;
+  dim3 grid(H / kHS8, G);
+  kern<<<grid, 256, smem, stream>>>(static_cast<const __nv_bfloat16*>(x), static_cast<const uint8_t*>(qglu), sglu,
+                                    static_cast<const uint8_t*>(q3t), s3t, y, counts, rows_cap, M, H, N, act);
+  return cudaGetLastError();
 }
 
 }  // namespace tb

@@ -27,8 +27,12 @@ class FusedExpertsNetwork(torch.nn.Module):
     rows_independent = True      # each output row depends on its input row alone: dispatch may skip the zero padding
 
     def __init__(self, model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count, activation_fn=None,
-                 activation_fn_with_self=None, output_dim=None, has_fc1_bias=True, has_fc2_bias=True, fp8=None):
+                 activation_fn_with_self=None, output_dim=None, has_fc1_bias=True, has_fc2_bias=True, fp8=None,
+                 weight_format=None):
         super().__init__()
+        if weight_format is not None:
+            raise ValueError("ffn experts have no stored weight format (got weight_format=%r): the block-fp8 checkpoints "
+                             "hold SwiGLU experts, use type 'llama_ffn'" % (weight_format,))
         self.skip_expert = int(os.environ.get('SKIP_EXPERT', '0')) != 0
         assert hidden_size_per_expert % sharded_count == 0, \
             "Can't evenly divide hidden_size_per_expert (%d) to %d slices." % (hidden_size_per_expert, sharded_count)

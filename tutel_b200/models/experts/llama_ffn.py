@@ -5,6 +5,10 @@ over the ``Sh`` sharers each forward (ZeRO-style; gradient = reduce-scatter).  T
 grouped kernel when the dtype allows.  In dropless ("Megablocks") inference the per-expert token counts stay on the
 device: up to 64 rows per expert the whole expert is one weight-streaming launch that reads only the active experts'
 weights (csrc/skinny_gemm.cu), above that the wgmma kernels skip the rows past the counts.
+
+``weight_format='fp8_block'`` stores the experts as the block-scaled e4m3 checkpoints of DeepSeek-V3, Kimi-K2, GLM-4.5,
+Moonlight and Qwen3-FP8 do, 1 byte per weight plus one fp32 scale per 128 x 128 block, with no 16-bit master copy and
+no parameters: inference only (``load_fp8_block_weights``, doc/CHECKPOINT.md).
 """
 import torch
 
@@ -16,11 +20,18 @@ from . import dropless_row_counts
 
 class LlamaFFNNetwork(torch.nn.Module):
     rows_independent = True      # each output row depends on its input row alone: dispatch may skip the zero padding
+    # weight_format='fp8_block': the stored buffers, kept e4m3 / fp32 by _apply
+    FP8_BLOCK_BUFFERS = ('W_gate_up', 'W_gate_up_scale', 'W_down', 'W_down_scale')
 
     def __init__(self, model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count,
-                 activation_fn=torch.nn.functional.silu, fp8=None):
+                 activation_fn=torch.nn.functional.silu, fp8=None, weight_format=None):
         super().__init__()
         import os
+        self.weight_format = weight_format
+        if weight_format is not None:
+            self._init_fp8_block(model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count,
+                                 activation_fn, fp8, weight_format)
+            return
         # fp8=True / 'row' (or TUTEL_B200_FP8=1 / true / row): e4m3 weights with per-row scales on every path, as in `ffn`.
         # fp8='block' (TUTEL_B200_FP8=block): DeepSeek-V3 block scales for the training GEMMs (ops/block_fp8.py); dropless
         # decoding keeps the 16-bit kernels.  OCP MX ('mx') has no SwiGLU kernel.
@@ -43,7 +54,68 @@ class LlamaFFNNetwork(torch.nn.Module):
         self.activation_fn = activation_fn
         self.reset_parameters()
 
+    def _init_fp8_block(self, M, H, E, sharded_count, activation_fn, fp8, weight_format):
+        # Stored block-fp8 experts: exactly what the block GEMM's forward reads, one copy per weight (ops/block_fp8.py):
+        #   W_gate_up [E, 2H, M] e4m3 (W1^T and W2^T interleaved every 64 rows) + W_gate_up_scale [E, 2H / 64, M / 128],
+        #   W_down [E, M, H] e4m3 (the checkpoint's down_proj.weight orientation) + W_down_scale [E, M / 128, H / 128].
+        if weight_format != 'fp8_block':
+            raise ValueError("llama_ffn: weight_format must be None or 'fp8_block' (got %r)" % (weight_format,))
+        if M % 128 or H % 128:
+            raise ValueError("llama_ffn: weight_format='fp8_block' needs model_dim and hidden_size_per_expert to be "
+                             "multiples of 128 (got %d, %d)" % (M, H))
+        if sharded_count != 1:
+            raise ValueError("llama_ffn: weight_format='fp8_block' keeps whole experts on each GPU (sharded_count must be "
+                             "1, got %d): use at least as many experts as GPUs" % sharded_count)
+        if fp8 is not None and str(fp8).lower() != 'block':
+            raise ValueError("llama_ffn: weight_format='fp8_block' runs the block-scaled kernels; fp8 must be unset or "
+                             "'block' (got %r)" % (fp8,))
+        self.fp8, self.block, self.sharded_count = False, True, sharded_count
+        self.activation_fn = activation_fn
+        self.model_dim, self.hidden_size = M, H
+        e4m3 = torch.float8_e4m3fn
+        self.register_buffer('W_gate_up', torch.zeros(E, 2 * H, M, dtype=e4m3))
+        self.register_buffer('W_gate_up_scale', torch.ones(E, 2 * H // 64, M // 128, dtype=torch.float32))
+        self.register_buffer('W_down', torch.zeros(E, M, H, dtype=e4m3))
+        self.register_buffer('W_down_scale', torch.ones(E, M // 128, H // 128, dtype=torch.float32))
+
+    def _apply(self, fn, recurse=True):
+        # .bfloat16() / .half() / .to(dtype) would cast the e4m3 and fp32 buffers (torch treats e4m3 as a floating
+        # dtype): they only follow device moves.  An empty probe tells where fn sends them without converting them.
+        keep = {n: self._buffers.pop(n) for n in self.FP8_BLOCK_BUFFERS if n in self._buffers}
+        try:
+            super()._apply(fn, recurse)
+        finally:
+            for n, b in keep.items():
+                probe = fn(b.new_empty(0))
+                self._buffers[n] = fn(b) if probe.dtype == b.dtype else b.to(probe.device)
+        return self
+
+    @torch.no_grad()
+    def load_fp8_block_weights(self, gate, gate_scale, up, up_scale, down, down_scale):
+        """Load block-scaled e4m3 experts in the checkpoint orientation, stacked over this module's E experts:
+        ``gate``, ``up`` e4m3 [E, H, M] with scales fp32 [E, H / 128, M / 128], ``down`` e4m3 [E, M, H] with scale fp32
+        [E, M / 128, H / 128]; the scales are HF's ``weight_scale_inv`` (``w ~= q * s`` per 128 x 128 block)."""
+        if self.weight_format != 'fp8_block':
+            raise ValueError("load_fp8_block_weights needs weight_format='fp8_block'")
+        qglu, sglu, q3t, s3t = BF8.load_glu_weights(gate, gate_scale, up, up_scale, down, down_scale)
+        for name, t in zip(self.FP8_BLOCK_BUFFERS, (qglu, sglu, q3t, s3t)):
+            buf = getattr(self, name)
+            if t.shape != buf.shape:
+                raise ValueError('load_fp8_block_weights: %s is %s for this module, the checkpoint gives %s'
+                                 % (name, tuple(buf.shape), tuple(t.shape)))
+            buf.copy_(t)
+
+    def export_fp8_block_weights(self):
+        """The inverse of ``load_fp8_block_weights`` for a bf16 layer (e.g. trained with ``fp8='block'``): the six
+        checkpoint tensors (gate, gate_scale, up, up_scale, down, down_scale) of its whole experts."""
+        if self.weight_format is not None or self.sharded_count != 1:
+            raise ValueError('export_fp8_block_weights needs a 16-bit layer with whole experts (sharded_count == 1)')
+        w1, w2, w3 = (getattr(self, n).view(self.full_shapes[n]) for n in ('W_fc1', 'W_fc2', 'W_fc3'))
+        return BF8.export_glu_weights(w1, w2, w3)
+
     def reset_parameters(self):
+        if self.weight_format is not None:
+            return
         with torch.no_grad():
             for name in ('W_fc1', 'W_fc2', 'W_fc3'):
                 getattr(self, name).normal_(0, 0.01)
@@ -55,7 +127,33 @@ class LlamaFFNNetwork(torch.nn.Module):
         # parameter (no copies in either direction)
         return C.zero_gather(param, full_shape=shape, group=group)
 
+    def _forward_fp8_block(self, x, ctx):
+        if torch.is_grad_enabled() and x.requires_grad:
+            raise RuntimeError("llama_ffn: weight_format='fp8_block' experts are inference-only (no master weights and no "
+                               "data-gradient copy); run the forward under torch.no_grad() or torch.inference_mode()")
+        if getattr(ctx, 'adaptive_degree', 1) == 0 and C.get_world_size(getattr(ctx, 'group', None)) > 1:
+            raise ValueError("llama_ffn: weight_format='fp8_block' experts stay local; adaptive_r=0 (which gathers the "
+                             "expert weights on every GPU) is not supported")
+        if x.dim() > 3:
+            x = x.reshape(x.size(0), x.size(1), -1)
+        kind = G.classify_activation(self.activation_fn)
+        if kind not in BF8.ACT_CODES:
+            raise ValueError("llama_ffn: weight_format='fp8_block' supports SiLU, GELU and ReLU activations")
+        if not BF8.can_use_stored_glu(x):
+            raise ValueError("llama_ffn: weight_format='fp8_block' runs on bf16 activations [E, rows, M] (got %s %s); "
+                             "convert the input or run under bf16 autocast" % (x.dtype, tuple(x.shape)))
+        qglu, sglu, q3t, s3t = (getattr(self, n) for n in self.FP8_BLOCK_BUFFERS)
+        row_counts = dropless_row_counts(x, ctx)
+        # the rule of the 16-bit experts: one launch that streams the active experts' bytes when the average expert fits
+        # in one pass of its rows, the block GEMMs (which read each weight once) otherwise
+        if (row_counts is not None and BF8.can_use_skinny_glu_ffn_block_fp8(x) and
+                x.size(1) * getattr(ctx, 'top_k', 1) <= G.SKINNY_PASS_ROWS * x.size(0)):
+            return BF8.skinny_glu_ffn_block_fp8(x, qglu, sglu, q3t, s3t, row_counts, kind)
+        return BF8.glu_ffn_block_fp8_stored(x, qglu, sglu, q3t, s3t, kind, row_counts)
+
     def forward(self, x, ctx):
+        if self.weight_format is not None:
+            return self._forward_fp8_block(x, ctx)
         w1, w2, w3 = (self._full(n, ctx.group) for n in ('W_fc1', 'W_fc2', 'W_fc3'))
         if x.dim() > 3:
             x = x.reshape(x.size(0), x.size(1), -1)
@@ -85,6 +183,8 @@ class LlamaFFNNetwork(torch.nn.Module):
 
     def supports_packed(self, x) -> bool:
         """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit experts without fp8 or block fp8."""
+        if self.weight_format is not None:
+            return False
         M, H = self.full_shapes['W_fc1'][1], self.full_shapes['W_fc1'][2]
         return (not self.fp8 and not self.block and x.dtype in (torch.float16, torch.bfloat16) and self.W_fc1.dtype == x.dtype and x.is_cuda and
                 self.sharded_count == 1 and G.classify_activation(self.activation_fn) in G.ACT_CODES and
@@ -96,6 +196,9 @@ class LlamaFFNNetwork(torch.nn.Module):
         return G.fused_glu_ffn(x, w1, w2, w3, G.classify_activation(self.activation_fn), False, None, layout=layout)
 
     def extra_repr(self):
+        if self.weight_format is not None:
+            return "weight_format='fp8_block', %d experts, model_dim=%d, hidden=%d" % (
+                self.W_down.size(0), self.model_dim, self.hidden_size)
         return 'full shapes: %s, sharded_count=%d' % ({k: tuple(v) for k, v in self.full_shapes.items()}, self.sharded_count)
 
 

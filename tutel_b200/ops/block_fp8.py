@@ -201,15 +201,27 @@ def quantize_glu_weight(w1: torch.Tensor, w2: torch.Tensor):
     return quantize_glu_weight_reference(w1, w2)
 
 
+def zero_rows_past(t: torch.Tensor, row_counts: torch.Tensor) -> torch.Tensor:
+    """t [G, R, ...] with rows r >= row_counts[g] of group g set to zero (whatever they held, NaN included)."""
+    live = torch.arange(t.size(1), device=t.device).view(1, -1) < row_counts.to(t.device).view(-1, 1).long()
+    return torch.where(live.view(*live.shape, *([1] * (t.dim() - 2))), t, torch.zeros((), dtype=t.dtype, device=t.device))
+
+
 def block_fp8_gemm(a, sa, b, sb, bias=None, aux=None, aux2=None, epilogue: int = EPI_NONE, act: str = 'silu',
-                   max_ctas: int = 0):
-    """``epilogue(a [G, M, K] @ b [G, N, K]^T)`` -> a list of bf16 results (see csrc/bindings.cpp: block_fp8_gemm)."""
+                   max_ctas: int = 0, row_counts: Optional[torch.Tensor] = None):
+    """``epilogue(a [G, M, K] @ b [G, N, K]^T)`` -> a list of bf16 results (see csrc/bindings.cpp: block_fp8_gemm).
+    ``row_counts`` (device int32 [G], optional): rows r >= row_counts[g] of every result are zero, and the kernel skips
+    the tiles that start at or past the count (dropless prefill)."""
     if _native(a, 'block_fp8_gemm'):
         backend.count_launch()
         if bias is not None:
             bias = bias.reshape(a.size(0), b.size(1)).to(torch.bfloat16).contiguous()
-        return backend.require_ext().block_fp8_gemm(a, sa, b, sb, bias, aux, aux2, int(epilogue), ACT_CODES[act], int(max_ctas))
-    return block_fp8_gemm_reference(a, sa, b, sb, bias, aux, aux2, epilogue, act)
+        args = (a, sa, b, sb, bias, aux, aux2, int(epilogue), ACT_CODES[act], int(max_ctas))
+        if row_counts is None:
+            return backend.require_ext().block_fp8_gemm(*args)
+        return backend.require_ext().block_fp8_gemm(*args, row_counts.to(torch.int32).contiguous())
+    out = block_fp8_gemm_reference(a, sa, b, sb, bias, aux, aux2, epilogue, act)
+    return out if row_counts is None else [zero_rows_past(t, row_counts) for t in out]
 
 
 _WEIGHT_CACHE = {}
@@ -333,3 +345,95 @@ class FusedGLUFFNBlockFp8(torch.autograd.Function):
 
 def fused_glu_ffn_block_fp8(x, w1, w2, w3, act='silu'):
     return FusedGLUFFNBlockFp8.apply(x, w1, w2, w3, act)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# stored block-fp8 experts (no 16-bit master weights): the checkpoint format of DeepSeek-V3, Kimi-K2, GLM-4.5, Moonlight
+# and Qwen3-FP8, and inference on it
+# ------------------------------------------------------------------------------------------------------------------
+# Checkpoint orientation, stacked over E local experts (HF ``{gate,up,down}_proj.weight`` / ``.weight_scale_inv``,
+# ``w ~= q * s`` per 128 x 128 block): gate, up e4m3 [E, H, M] + [E, H / 128, M / 128]; down e4m3 [E, M, H] +
+# [E, M / 128, H / 128].  Stored layout (what the block GEMM's forward reads): qglu [E, 2H, M] + sglu [E, 2H / 64, M / 128]
+# (gate / up interleaved every 64 rows, as ``quantize_glu_weight`` writes them) and q3t = down, s3t = down's scales.
+def export_glu_weights(w1: torch.Tensor, w2: torch.Tensor, w3: torch.Tensor):
+    """bf16 SwiGLU weights in the ``llama_ffn`` layout (w1, w2 [E, M, H], w3 [E, H, M]) -> the six checkpoint tensors
+    (gate, gate_scale, up, up_scale, down, down_scale), quantised per 128 x 128 block by ``quantize_weight``.  A block is
+    the same block in W and W^T, so ``load_glu_weights`` of the result is bit for bit the forward copy ``glu_weight(w1,
+    w2)[2:]`` and ``weight(w3)[2:]`` that a ``fp8='block'`` layer of these weights reads."""
+    for name, w in (('w1', w1), ('w2', w2), ('w3', w3)):
+        _check(w.dtype == torch.bfloat16 and w.dim() == 3, 'export_glu_weights: %s must be a bf16 [E, *, *] tensor (got %s %s)'
+               % (name, w.dtype, tuple(w.shape)))
+    _check(w1.shape == w2.shape and w3.shape == (w1.size(0), w1.size(2), w1.size(1)),
+           'export_glu_weights: w1, w2 [E, M, H] and w3 [E, H, M] expected (got %s, %s, %s)'
+           % (tuple(w1.shape), tuple(w2.shape), tuple(w3.shape)))
+    _, _, gate, gate_s = quantize_weight(w1.detach())
+    _, _, up, up_s = quantize_weight(w2.detach())
+    _, _, down, down_s = quantize_weight(w3.detach())
+    return gate, gate_s, up, up_s, down, down_s
+
+
+def load_glu_weights(gate, gate_scale, up, up_scale, down, down_scale):
+    """The six checkpoint tensors (see ``export_glu_weights``) -> the stored layout (qglu, sglu, q3t, s3t) on gate's device.
+    Shapes and dtypes are checked; the interleave is one-time torch indexing."""
+    def expect(t, dtype, shape, name):
+        _check(isinstance(t, torch.Tensor) and t.dtype == dtype and tuple(t.shape) == tuple(shape),
+               'load_fp8_block_weights: %s must be %s %s (got %s %s)' % (
+                   name, dtype, tuple(shape), getattr(t, 'dtype', type(t)), tuple(getattr(t, 'shape', ()))))
+    _check(isinstance(gate, torch.Tensor) and gate.dim() == 3, 'load_fp8_block_weights: gate must be e4m3 [E, H, M]')
+    E, H, M = gate.shape
+    _check(H % TILE == 0 and M % TILE == 0, 'load_fp8_block_weights: H and M must be multiples of 128 (got %d, %d)' % (H, M))
+    e4m3 = torch.float8_e4m3fn
+    expect(gate, e4m3, (E, H, M), 'gate')
+    expect(up, e4m3, (E, H, M), 'up')
+    expect(down, e4m3, (E, M, H), 'down')
+    expect(gate_scale, torch.float32, (E, H // TILE, M // TILE), 'gate_scale')
+    expect(up_scale, torch.float32, (E, H // TILE, M // TILE), 'up_scale')
+    expect(down_scale, torch.float32, (E, M // TILE, H // TILE), 'down_scale')
+    dev = gate.device
+    qglu = interleave_glu_reference(gate.view(torch.uint8), up.to(dev).view(torch.uint8)).view(e4m3)
+    sglu = interleave_glu_reference(gate_scale.to(dev).repeat_interleave(2, dim=1),
+                                    up_scale.to(dev).repeat_interleave(2, dim=1), rows_per=1)
+    return qglu.contiguous(), sglu.contiguous(), down.to(dev).contiguous(), down_scale.to(dev).contiguous()
+
+
+def can_use_stored_glu(x: torch.Tensor) -> bool:
+    """Inputs the stored block-fp8 SwiGLU expert runs on: bf16 [E, rows, M] (on a GPU or, through the references, on
+    CPU).  Nothing is cast: other dtypes are refused by the caller."""
+    return x.dtype == torch.bfloat16 and x.dim() == 3
+
+
+SKINNY_SMEM_LIMIT = 100 * 1024       # staged bf16 x rows (8 M bytes) + the 2 KB hidden slice: two blocks per SM
+
+
+def can_use_skinny_glu_ffn_block_fp8(x: torch.Tensor) -> bool:
+    """``skinny_glu_ffn_block_fp8`` covers up to 64 rows per expert and M up to 12544 (csrc/skinny_gemm.cu)."""
+    return can_use_stored_glu(x) and x.size(1) <= 64 and 8 * x.size(2) + 2048 <= SKINNY_SMEM_LIMIT
+
+
+def skinny_glu_ffn_block_fp8_reference(x, qglu, sglu, q3t, s3t, row_counts, act='silu'):
+    """fp32 composition on the dequantised stored weights; rows past the counts are zero.  The CPU path of the kernel."""
+    G, R, _ = x.shape
+    H = qglu.size(1) // 2
+    t = (x.float() @ dequantize_weight(qglu, sglu).transpose(1, 2)).view(G, R, H // 64, 2, 64)
+    g, u = t[:, :, :, 0].reshape(G, R, H), t[:, :, :, 1].reshape(G, R, H)
+    y = (_act(g, act)[0] * u) @ dequantize_weight(q3t, s3t).transpose(1, 2)
+    if row_counts is not None:
+        y = zero_rows_past(y, row_counts)
+    return y.to(x.dtype)
+
+
+def skinny_glu_ffn_block_fp8(x, qglu, sglu, q3t, s3t, row_counts, act='silu'):
+    """y[g, r] = (act(x @ W1) * (x @ W2)) @ W3 for r < row_counts[g] (other rows zero) on the stored block-scaled e4m3
+    weights, in one weight-streaming launch of ``skinny_glu_ffn_block_fp8_kernel`` on a GPU (x stays bf16)."""
+    if _native(x, 'block_fp8.skinny_glu_ffn_block_fp8'):
+        backend.count_launch(2)          # zero-fill of the fp32 accumulator + the kernel
+        y = backend.require_ext().skinny_glu_ffn_block_fp8(x.contiguous(), qglu, sglu, q3t, s3t, row_counts, ACT_CODES[act])
+        return y.to(x.dtype)
+    return skinny_glu_ffn_block_fp8_reference(x, qglu, sglu, q3t, s3t, row_counts, act)
+
+
+def glu_ffn_block_fp8_stored(x, qglu, sglu, q3t, s3t, act='silu', row_counts=None):
+    """Inference forward of the stored experts: the launches of ``FusedGLUFFNBlockFp8.forward`` on the stored bytes (GLU
+    GEMM, then the down projection), with the device row counts of dropless prefill when given."""
+    h = block_fp8_gemm(*quantize_act(x.contiguous()), qglu, sglu, epilogue=EPI_GLU, act=act, row_counts=row_counts)[0]
+    return block_fp8_gemm(*quantize_act(h), q3t, s3t, row_counts=row_counts)[0]

@@ -451,10 +451,10 @@ def engine_for(layer, x: torch.Tensor, crit, d: int):
             return None
         M, H, Mo = layer.model_dim, ex.hidden_size * (Sh // r if Sh > 1 else 1), ex.output_dim
     elif isinstance(ex, LlamaFFNNetwork):
+        if getattr(ex, 'block', False):
+            return None     # block-fp8 experts (stored ones have no W_fc1) run on the unfused path (ops/block_fp8.py)
         if G.classify_activation(ex.activation_fn) not in G.ACT_CODES or ex.W_fc1.dtype != x.dtype:
             return None
-        if getattr(ex, 'block', False):
-            return None     # block-fp8 experts run on the unfused path (ops/block_fp8.py)
         align = 16 if ex.fp8 else 8
         if any(int(v) % align for v in ex.full_shapes['W_fc1'][1:]) or int(ex.full_shapes['W_fc3'][2]) % align:
             return None
