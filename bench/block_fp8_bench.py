@@ -8,12 +8,17 @@ Three parts, each printing JSON lines with the card name and power limit:
 
 * ``gemm``: kernel time and TFLOP/s at the flagship expert shapes (8 experts, 2048 rows each; fc1 4096 -> 14336 and
   fc2 14336 -> 4096) for the bf16 grouped GEMM, row-scaled e4m3, MX and block-scaled e4m3, CUDA events over ``--iters``
-  launches after a warm-up.  Operand quantisation is not timed.
+  launches after a warm-up.  Operand quantisation is not timed.  The weight-gradient shapes (``wgrad``: 14336 x 4096,
+  the ``ffn`` dW1 and dW2; ``wgrad_glu``: 4096 x 28672, the ``llama_ffn`` [dW1 | dW2] in one split launch) over K = 2048
+  tokens per expert time the bf16 GEMM on the 16-bit activations against ``block_wgrad``, the block-scaled GEMM on
+  column-wise e4m3 copies; ``dual_quant`` is the dual quantiser on one [8, 2048, 14336] activation.
 * ``accuracy``: max |err| / max |ref| against an fp64 product of the same bf16 operands, row-scaled and block-scaled,
-  at K = 4096 and 14336 (1024 x 1024 outputs), quantisation included.
+  at K = 4096 and 14336 (1024 x 1024 outputs), quantisation included; and of the weight-gradient GEMM ``a^T b`` over
+  K = 2048 and 16384 tokens, bf16 and block-scaled.
 * ``train``: whole training steps (forward, backward, SGD) of the flagship ``ffn`` (ReLU) and ``llama_ffn`` layers
-  (top-2 of 8, 4096 / 14336, 8192 tokens, capacity factor 1) in bf16, row, MX (ffn only) and block, alternated in
-  ``--rounds`` rounds of ``--steps`` steps; median step time per mode.
+  (top-2 of 8, 4096 / 14336, 8192 tokens, capacity factor 1) in bf16, row, MX (ffn only), block and block with
+  ``fp8_wgrad``, alternated in ``--rounds`` rounds of ``--steps`` steps; median step time and peak memory
+  (``torch.cuda.max_memory_allocated`` over the mode's steps) per mode.
 """
 import argparse
 import json
@@ -91,6 +96,29 @@ def gemm_part():
             ms = timed(fn, args.iters)
             emit(part='gemm', shape=name, experts=E, rows=T, K=K, N=N, mode=mode, ms=round(ms, 4),
                  tflops=round(flops / ms / 1e9, 1))
+        del x, w, xq, wq, xm, wm, xb, wb
+    # weight gradients: D [E, Ma, N] = a^T b over the T tokens of each expert
+    for name, Ma, N in (('wgrad', 14336, 4096), ('wgrad_glu', 4096, 2 * 14336)):
+        torch.manual_seed(0)
+        a = torch.randn(E, T, Ma, device='cuda').bfloat16()
+        b = (torch.randn(E, T, N, device='cuda') * 1e-3).bfloat16()
+        _, _, aT, saT = BF.quantize_act_dual(a, rowwise=False)
+        _, _, bT, sbT = BF.quantize_act_dual(b, rowwise=False)
+        split = N // 2 if name == 'wgrad_glu' else None
+        flops = 2.0 * E * Ma * N * T
+        runs = {
+            'bf16': lambda: G.raw_gemm(a, b, a_mn=True, b_mn=True),
+            'block_wgrad': lambda: BF.wgrad_gemm(aT, saT, bT, sbT, split=split),
+        }
+        for mode, fn in runs.items():
+            ms = timed(fn, args.iters)
+            emit(part='gemm', shape=name, experts=E, rows=Ma, K=T, N=N, mode=mode, ms=round(ms, 4),
+                 tflops=round(flops / ms / 1e9, 1))
+        if name == 'wgrad':
+            ms = timed(lambda: BF.quantize_act_dual(a), args.iters)
+            emit(part='gemm', shape='dual_quant', experts=E, rows=T, K=Ma, mode='block', ms=round(ms, 4),
+                 gbps=round(E * T * Ma * (2 + 2 + 8 / 128) / ms / 1e6, 1))
+        del a, b, aT, bT
 
 
 def accuracy_part():
@@ -112,6 +140,17 @@ def accuracy_part():
         for mode, out in (('row', row), ('block', blk)):
             emit(part='accuracy', K=K, M=M, N=N, mode=mode, output=str(out.dtype).replace('torch.', ''),
                  max_err_over_max_ref=float((out.double() - ref).abs().max()) / scale)
+    for T in (2048, 16384):
+        gen = torch.Generator(device='cuda').manual_seed(T)
+        a = torch.randn(1, T, M, device='cuda', generator=gen).bfloat16()
+        b = (torch.randn(1, T, N, device='cuda', generator=gen) * 1e-3).bfloat16()
+        ref = a.double().transpose(1, 2) @ b.double()
+        scale = float(ref.abs().max())
+        bf = G.raw_gemm(a, b, a_mn=True, b_mn=True)
+        blk = BF.wgrad_gemm(*BF.quantize_act_dual(a, rowwise=False)[2:], *BF.quantize_act_dual(b, rowwise=False)[2:])[0]
+        for mode, out in (('bf16', bf), ('block_wgrad', blk)):
+            emit(part='accuracy', shape='wgrad', K=T, M=M, N=N, mode=mode, output=str(out.dtype).replace('torch.', ''),
+                 max_err_over_max_ref=float((out.double() - ref).abs().max()) / scale)
 
 
 def train_part():
@@ -119,14 +158,16 @@ def train_part():
     from tutel_b200.ops import gemm as G
     M, H, E = 4096, 14336, 8
     for kind in ('ffn', 'llama_ffn'):
-        modes = ['bf16', 'row', 'mx', 'block'] if kind == 'ffn' else ['bf16', 'row', 'block']
+        modes = ['bf16', 'row', 'mx', 'block', 'block+wgrad'] if kind == 'ffn' else ['bf16', 'row', 'block', 'block+wgrad']
         layers = {}
         for mode in modes:
             torch.manual_seed(0)
             experts = {'type': kind, 'num_experts_per_device': E, 'hidden_size_per_expert': H}
             if kind == 'ffn':
                 experts['activation_fn'] = lambda t: F.relu(t)
-            if mode != 'bf16':
+            if mode == 'block+wgrad':
+                experts.update(fp8='block', fp8_wgrad=True)
+            elif mode != 'bf16':
                 experts['fp8'] = mode
             layer = moe.moe_layer(gate_type={'type': 'top', 'k': 2, 'capacity_factor': 1.0}, model_dim=M,
                                   experts=experts, seeds=(1, 2, 3)).cuda().bfloat16()
@@ -142,18 +183,22 @@ def train_part():
             opt.step()
 
         times = {m: [] for m in modes}
+        peak = {m: 0 for m in modes}
         for m in modes:
             for _ in range(args.warmup):
                 step(m)
         for _ in range(args.rounds):
             for m in modes:
                 torch.cuda.synchronize()
+                torch.cuda.reset_peak_memory_stats()
                 ms = timed(lambda: step(m), args.steps)
                 times[m].append(ms)
+                peak[m] = max(peak[m], torch.cuda.max_memory_allocated())
                 G.invalidate_fp8_cache()
         for m in modes:
             emit(part='train', expert=kind, mode=m, model_dim=M, hidden=H, experts=E, tokens=args.tokens,
-                 median_step_ms=round(statistics.median(times[m]), 3), rounds=[round(t, 3) for t in times[m]])
+                 median_step_ms=round(statistics.median(times[m]), 3), rounds=[round(t, 3) for t in times[m]],
+                 peak_mem_gib=round(peak[m] / 2 ** 30, 3))
         del layers
 
 

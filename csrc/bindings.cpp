@@ -863,6 +863,73 @@ std::vector<at::Tensor> block_fp8_gemm_counts(const at::Tensor& a, const at::Ten
   return block_fp8_gemm_impl(a, sa, b, sb, bias, aux, aux2, epilogue, act, max_ctas, row_counts.data_ptr<int>());
 }
 
+// x [G, R, K] bf16 (K % 128 == 0), both orientations from one read (csrc/gemm_block_fp8.h) ->
+// rowwise: [q [G, R, K], s [G, K / 128, Rp], qT [G, K, Rp], sT [G, Rp / 128, K]];  otherwise [qT, sT].  Rp = roundup(R, 128).
+std::vector<at::Tensor> block_fp8_quantize_act_dual(const at::Tensor& x, bool rowwise) {
+  TORCH_CHECK(x.is_cuda() && x.is_contiguous() && x.dim() == 3 && x.scalar_type() == at::kBFloat16 && x.size(2) % 128 == 0 &&
+                  x.size(0) <= 65535,
+              "block_fp8_quantize_act_dual: contiguous bf16 CUDA tensor [G, R, K] with K % 128 == 0 and G <= 65535 expected");
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int G = static_cast<int>(x.size(0)), R = static_cast<int>(x.size(1)), K = static_cast<int>(x.size(2));
+  const int Rp = (R + 127) / 128 * 128;
+  const auto f8 = x.options().dtype(at::kFloat8_e4m3fn), f32 = x.options().dtype(at::kFloat);
+  at::Tensor qT = at::empty({G, K, Rp}, f8);
+  at::Tensor sT = at::empty({G, Rp / 128, K}, f32);
+  at::Tensor q, s;
+  if (rowwise) {
+    q = at::empty({G, R, K}, f8);
+    s = at::empty({G, K / 128, Rp}, f32);
+  }
+  TB_CHECK_CUDA(tb::block_fp8_quantize_act_dual(x.data_ptr(), rowwise ? q.data_ptr() : nullptr, rowwise ? s.data_ptr<float>() : nullptr,
+                                                qT.data_ptr(), sT.data_ptr<float>(), G, R, K, cur_stream()));
+  if (rowwise) return {q, s, qT, sT};
+  return {qT, sT};
+}
+
+// Weight-gradient GEMM d[g] = a[g] * b[g]^T over the padded token dimension K: a e4m3 [G, M, K] + sa fp32 [G, K / 128, M],
+// b e4m3 [G, N, K] + sb fp32 [G, K / 128, N] (one scale per row and K step) -> [d bf16 [G, M, N]]; split = H > 0
+// (N == 2H) -> [d1 [G, M, H] (columns < H), d2 [G, M, H] (columns >= H)].
+std::vector<at::Tensor> block_fp8_wgrad_gemm(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                             int64_t split, int64_t max_ctas) {
+  TORCH_CHECK(a.is_cuda() && b.is_cuda() && sa.is_cuda() && sb.is_cuda() && a.dim() == 3 && b.dim() == 3 && sa.dim() == 3 &&
+              sb.dim() == 3, "block_fp8_wgrad_gemm: 3-D CUDA tensors expected");
+  TORCH_CHECK(b.device() == a.device() && sa.device() == a.device() && sb.device() == a.device(),
+              "block_fp8_wgrad_gemm: operands on one device expected");
+  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && sa.is_contiguous() && sb.is_contiguous(),
+              "block_fp8_wgrad_gemm: contiguous operands expected");
+  TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn &&
+              sa.scalar_type() == at::kFloat && sb.scalar_type() == at::kFloat,
+              "block_fp8_wgrad_gemm: e4m3 operands and fp32 scales expected");
+  TORCH_CHECK(a.size(0) == b.size(0) && a.size(2) == b.size(2), "block_fp8_wgrad_gemm: a [G, M, K] and b [G, N, K] expected");
+  const c10::cuda::CUDAGuard guard(a.device());
+  tb::BlockFp8WgradProblem p;
+  p.G = static_cast<int>(a.size(0)); p.M = static_cast<int>(a.size(1)); p.K = static_cast<int>(a.size(2));
+  p.N = static_cast<int>(b.size(1));
+  TORCH_CHECK(p.M % 128 == 0 && p.N % 128 == 0 && p.K % 128 == 0, "block_fp8_wgrad_gemm: M, N and K must be multiples of 128");
+  const int64_t kb = p.K / 128;
+  TORCH_CHECK(sa.size(0) == p.G && sa.size(1) == kb && sa.size(2) == p.M && sb.size(0) == p.G && sb.size(1) == kb && sb.size(2) == p.N,
+              "block_fp8_wgrad_gemm: scale arrays do not match the operand shapes (sa [G, K / 128, M], sb [G, K / 128, N] expected)");
+  TORCH_CHECK(split == 0 || (split % 128 == 0 && 2 * split == p.N),
+              "block_fp8_wgrad_gemm: split must be 0 or N / 2, a multiple of 128");
+  const auto bf = a.options().dtype(at::kBFloat16);
+  std::vector<at::Tensor> out;
+  if (split == 0) {
+    out.push_back(at::empty({p.G, p.M, p.N}, bf));
+  } else {
+    out.push_back(at::empty({p.G, p.M, split}, bf));
+    out.push_back(at::empty({p.G, p.M, split}, bf));
+    p.d2 = out[1].data_ptr();
+  }
+  p.d = out[0].data_ptr();
+  p.split = static_cast<int>(split);
+  p.a = a.data_ptr(); p.sa = sa.data_ptr<float>(); p.b = b.data_ptr(); p.sb = sb.data_ptr<float>();
+  p.max_ctas = static_cast<int>(max_ctas);
+  const char* why = nullptr;
+  cudaError_t e = tb::block_fp8_wgrad_gemm_launch(p, cur_stream(), &why);
+  TORCH_CHECK(e == cudaSuccess, "block_fp8_wgrad_gemm: ", why ? why : cudaGetErrorString(e));
+  return out;
+}
+
 // Gated-linear-unit GEMMs (SwiGLU / GeGLU / ReGLU experts; reference: tutel/experts/llama_ffn.py:38-41 runs three
 // cuBLAS GEMMs plus separate activation and multiply kernels).
 //   forward  (b2 given):  h = act(a*b) .* (a*b2)   [+ g = a*b -> d2, u = a*b2 -> d3 when given]   ONE launch
@@ -1180,6 +1247,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("block_fp8_quantize_glu_weight", &block_fp8_quantize_glu_weight);
   m.def("block_fp8_gemm", &block_fp8_gemm);
   m.def("block_fp8_gemm", &block_fp8_gemm_counts);   // + row_counts
+  m.def("block_fp8_quantize_act_dual", &block_fp8_quantize_act_dual);
+  m.def("block_fp8_wgrad_gemm", &block_fp8_wgrad_gemm);
   m.def("skinny_glu_ffn_block_fp8", &skinny_glu_ffn_block_fp8);
   register_symm_bindings(m);
   register_cpu_bindings(m);

@@ -14,8 +14,13 @@
 //                 the CTA and stay in L1.  Epilogue straight from the accumulator fragment.
 // Persistent: CTA b works on tiles b, b + grid, ...; the producer runs ahead into the next tile during the epilogue.
 //
-// Quantisers: block_fp8_quantize_act_kernel (activations, 1 x 128 tiles) and block_fp8_quantize_weight_kernel (weights,
-// 128 x 128 blocks; both orientations from one read, optionally in the SwiGLU gate / up layout).
+// Weight gradients (WGRAD instantiation): K is the token dimension and B, like A, has one scale per row and K step
+// ([G, K / 128, N], MN-major).  The producer bulk-copies the B tile's 512 bytes of scales next to A's; each consumer
+// thread reads the 32 of its fragment's columns from shared memory and promotes with acc = fmaf(part, sa[m] * sb[n], acc).
+//
+// Quantisers: block_fp8_quantize_act_kernel (activations, 1 x 128 tiles), block_fp8_quantize_dual_kernel (activations,
+// 1 x 128 and, transposed, 128 x 1 tiles from one read, for the weight-gradient GEMM) and block_fp8_quantize_weight_kernel
+// (weights, 128 x 128 blocks; both orientations from one read, optionally in the SwiGLU gate / up layout).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp8.h>
@@ -65,7 +70,18 @@ struct Args {
   long long num_tiles;
   int epi, act;
   const int* row_counts;               // COUNTS: live rows of each group (device); null otherwise
+  int split;                           // WGRAD: columns >= split go to d2 (at column n - split); 0: all to d
 };
+
+// WGRAD: B's per-column scales of each stage, 512 bytes after the barriers
+constexpr uint32_t kWgradSmemBytes = Cfg::SMEM_BYTES + Cfg::STAGES * kSaBytes;
+static_assert(kWgradSmemBytes <= 232448, "227 KB of shared memory per block");
+
+__device__ __forceinline__ float2 lds_f2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
 
 __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
   uint32_t v;
@@ -110,9 +126,10 @@ __device__ __forceinline__ int live_rows(const Args& args, int g) {
   return COUNTS ? max(0, min(args.row_counts[g], args.M)) : args.M;
 }
 
-template <bool COUNTS>
+template <bool COUNTS, bool WGRAD>
 __global__ void __launch_bounds__(kThreads, 1)
 block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Args args) {
+  static_assert(!(COUNTS && WGRAD), "row counts are for the forward GEMMs");
   using C = Cfg;
   extern __shared__ uint8_t smem_raw[];
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
@@ -126,6 +143,7 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   auto smem_sa = [&](int s) { return sa_base + s * kSaBytes; };
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
+  auto smem_sb = [&](int s) { return bar_base + C::BAR_BYTES + s * kSaBytes; };   // WGRAD only
 
   if (warp == 0 && ptx::elect_one()) {
     ptx::prefetch_tensormap(&tmA);
@@ -158,10 +176,12 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
           ptx::mbar_wait_quiet(empty_bar(s), ph ^ 1u);
           if (ptx::elect_one()) {
             const uint32_t fb = full_bar(s);
-            ptx::mbar_expect_tx(fb, C::OP_BYTES + kSaBytes);
+            ptx::mbar_expect_tx(fb, C::OP_BYTES + (WGRAD ? 2 : 1) * kSaBytes);
             ptx::tma_load_3d(smem_a(s), &tmA, fb, kb * kBK, m0, g);
             ptx::tma_load_3d(smem_b(s), &tmB, fb, kb * kBK, n0, g);
             ptx::bulk_load(smem_sa(s), sa_g + static_cast<long long>(kb) * args.sa_rows, kSaBytes, fb);
+            if constexpr (WGRAD)
+              ptx::bulk_load(smem_sb(s), args.sb + (static_cast<long long>(g) * num_kb + kb) * args.N + n0, kSaBytes, fb);
           }
           __syncwarp();
           if (++s == C::STAGES) { s = 0; ph ^= 1u; }
@@ -186,7 +206,8 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       // B scales of this tile: columns 0..63 and 64..127 (the same row unless the tile holds 64 gate + 64 up columns)
       const float* sb_lo = args.sb + (static_cast<long long>(g) * args.sb_rows + (glu ? 2 * n_blk : n_blk)) * num_kb;
       const float* sb_hi = glu ? sb_lo + num_kb : sb_lo;
-      float sbl = __ldg(sb_lo), sbh = __ldg(sb_hi);
+      float sbl = 0.f, sbh = 0.f;
+      if constexpr (!WGRAD) { sbl = __ldg(sb_lo); sbh = __ldg(sb_hi); }
       float acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -206,6 +227,24 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         ptx::wgmma_commit();
         const float sa0 = __uint_as_float(lds_u32(smem_sa(s) + 4u * r0));
         const float sa1 = __uint_as_float(lds_u32(smem_sa(s) + 4u * (r0 + 8)));
+        if constexpr (WGRAD) {
+          // this thread's columns 8 j + c0 + {0, 1}: read before the stage is released
+          float2 sbv[16];
+#pragma unroll
+          for (int j = 0; j < 16; ++j) sbv[j] = lds_f2(smem_sb(s) + 4u * (8 * j + c0));
+          ptx::wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(empty_bar(s));
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            acc[4 * j] = fmaf(part[4 * j], sa0 * sbv[j].x, acc[4 * j]);
+            acc[4 * j + 1] = fmaf(part[4 * j + 1], sa0 * sbv[j].y, acc[4 * j + 1]);
+            acc[4 * j + 2] = fmaf(part[4 * j + 2], sa1 * sbv[j].x, acc[4 * j + 2]);
+            acc[4 * j + 3] = fmaf(part[4 * j + 3], sa1 * sbv[j].y, acc[4 * j + 3]);
+          }
+          if (++s == C::STAGES) { s = 0; ph ^= 1u; }
+          continue;
+        }
         const float s00 = sa0 * sbl, s01 = sa0 * sbh, s10 = sa1 * sbl, s11 = sa1 * sbh;
         if (kb + 1 < steps) { sbl = __ldg(sb_lo + kb + 1); sbh = __ldg(sb_hi + kb + 1); }
         ptx::wgmma_wait<0>();
@@ -223,6 +262,23 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       }
 
       // ------------------------------- epilogue -------------------------------
+      if constexpr (WGRAD) {
+        // bf16 D; with a split, tiles at or past column `split` store into the second output
+        __nv_bfloat16* dst = args.d;
+        int ncol = n_blk * kBN;
+        if (args.split > 0 && ncol >= args.split) { dst = args.d2; ncol -= args.split; }
+        dst += static_cast<long long>(g) * args.d_group_stride + ncol + c0;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = m_blk * kBM + r0 + 8 * h;
+          if (row >= args.M) continue;
+          __nv_bfloat16* o = dst + static_cast<long long>(row) * args.ldd;
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+            *reinterpret_cast<__nv_bfloat162*>(o + 8 * j) = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+        continue;
+      }
       const int epi = args.epi;
       const long long goff = static_cast<long long>(g) * args.d_group_stride;
       const long long aoff = static_cast<long long>(g) * args.aux_group_stride;
@@ -353,10 +409,109 @@ block_fp8_quantize_act_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __re
   }
 }
 
+constexpr int kTilePitch = 132;          // bytes: a column read by 8 threads 16 rows apart spreads over 8 banks
+
+// Transposed write of a 128 x 128 byte tile: thread (c, part) writes 16 bytes of row c of the output (tile column c),
+// 8 threads cover one 128-byte row segment.  `row_ptr(c)` is where output row c's 128 bytes go.
+template <typename RowPtr>
+__device__ __forceinline__ void store_tile_transposed(const uint8_t* tile, int t, RowPtr row_ptr) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int task = t + 256 * i;
+    const int c = task >> 3, part = task & 7;
+    uint32_t w4[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      uint32_t v = 0;
+#pragma unroll
+      for (int b = 0; b < 4; ++b) v |= static_cast<uint32_t>(tile[(part * 16 + 4 * k + b) * kTilePitch + c]) << (8 * b);
+      w4[k] = v;
+    }
+    *reinterpret_cast<uint4*>(row_ptr(c) + part * 16) = make_uint4(w4[0], w4[1], w4[2], w4[3]);
+  }
+}
+
+// Both orientations of an activation x [G, R, K] from one read, for the weight-gradient GEMM.  One block of 256 threads
+// per 128 x 128 tile (rows rb, K columns kt); thread t holds columns 8 (t % 16) + 0..7 of rows t / 16 + 16 i, i < 8.
+//   row-wise   (q != null): q [G, R, K] and s [G, K / 128, Rp], the 1 x 128 tiles of block_fp8_quantize_act_kernel with
+//              the same arithmetic (one half warp per row), so the bytes and scales are that kernel's
+//   column-wise: qT [G, K, Rp] and sT [G, Rp / 128, K], one scale per column and 128-row block; rows past R are not read,
+//              they are zero bytes and take no part in the scale
+__global__ void __launch_bounds__(256)
+block_fp8_quantize_dual_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q, float* __restrict__ s,
+                               uint8_t* __restrict__ qT, float* __restrict__ sT, int R, int Rp, int K) {
+  __shared__ __align__(16) uint8_t tile[kBM * kTilePitch];
+  __shared__ float red[8][kBK];
+  __shared__ float csc[kBK];
+  const int kt = blockIdx.x, rb = blockIdx.y, g = blockIdx.z;
+  const int t = threadIdx.x, c8 = (t & 15) * 8;
+  const int KT = K / kBK;
+  float f[8][8];
+  float cmax[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) cmax[j] = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int r = rb * kBM + (t >> 4) + 16 * i;
+    if (r < R) {
+      unpack8(ptx::ld_nc_v4(x + (static_cast<long long>(g) * R + r) * K + kt * kBK + c8), f[i]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[i][j] = 0.0f;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) cmax[j] = fmaxf(cmax[j], fabsf(f[i][j]));
+  }
+  if (q != nullptr) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int r = rb * kBM + (t >> 4) + 16 * i;
+      float amax = 0.0f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(f[i][j]));
+#pragma unroll
+      for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+      const float sc = block_scale(amax);
+      if (r < R) *reinterpret_cast<uint2*>(q + (static_cast<long long>(g) * R + r) * K + kt * kBK + c8) = quantize8(f[i], 1.0f / sc);
+      if ((t & 15) == 0) s[(static_cast<long long>(g) * KT + kt) * Rp + r] = r < R ? sc : 0.0f;
+    }
+  }
+  // column maxima: the two half warps, then the 8 warps through shared memory
+#pragma unroll
+  for (int j = 0; j < 8; ++j) cmax[j] = fmaxf(cmax[j], __shfl_xor_sync(0xffffffffu, cmax[j], 16));
+  if ((t & 31) < 16) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) red[t >> 5][c8 + j] = cmax[j];
+  }
+  __syncthreads();
+  if (t < kBK) {
+    float m = red[0][t];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) m = fmaxf(m, red[w][t]);
+    const float sc = block_scale(m);
+    csc[t] = sc;
+    sT[(static_cast<long long>(g) * (Rp / kBM) + rb) * K + kt * kBK + t] = sc;
+  }
+  __syncthreads();
+  float inv[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) inv[j] = 1.0f / csc[c8 + j];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const __nv_fp8x4_e4m3 lo(make_float4(f[i][0] * inv[0], f[i][1] * inv[1], f[i][2] * inv[2], f[i][3] * inv[3]));
+    const __nv_fp8x4_e4m3 hi(make_float4(f[i][4] * inv[4], f[i][5] * inv[5], f[i][6] * inv[6], f[i][7] * inv[7]));
+    uint32_t* dst = reinterpret_cast<uint32_t*>(tile + ((t >> 4) + 16 * i) * kTilePitch + c8);
+    dst[0] = *reinterpret_cast<const uint32_t*>(&lo);
+    dst[1] = *reinterpret_cast<const uint32_t*>(&hi);
+  }
+  __syncthreads();
+  uint8_t* qTg = qT + (static_cast<long long>(g) * K + kt * kBK) * Rp + rb * kBM;
+  store_tile_transposed(tile, t, [&](int c) { return qTg + static_cast<long long>(c) * Rp; });
+}
+
 // One block of 256 threads per 128 x 128 weight block: a reduction for the scale, the row-major e4m3 copy written
 // straight from registers, the transposed copy through a shared byte tile.  GLU: blockIdx.z = 2 g + (0 gate | 1 up),
 // rows are M, columns H, and the outputs go to the concatenated [G, M, 2H] and the interleaved [G, 2H, M] layouts.
-constexpr int kTilePitch = 132;          // bytes: a column read by 8 threads 16 rows apart spreads over 8 banks
 
 template <bool GLU>
 __global__ void __launch_bounds__(256)
@@ -415,25 +570,13 @@ block_fp8_quantize_weight_kernel(const __nv_bfloat16* __restrict__ w, const __nv
     }
   }
   __syncthreads();
-  // transposed copy: thread (c, part) writes 16 bytes of row c, 8 threads cover one 128-byte row segment
+  // transposed copy
   const long long NT = GLU ? 2LL * Cn : Cn;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int task = t + 256 * i;
-    const int c = task >> 3, part = task & 7;
-    uint32_t w4[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      uint32_t v = 0;
-#pragma unroll
-      for (int b = 0; b < 4; ++b) v |= static_cast<uint32_t>(tile[(part * 16 + 4 * k + b) * kTilePitch + c]) << (8 * b);
-      w4[k] = v;
-    }
+  store_tile_transposed(tile, t, [&](int c) {
     const int col = cb * kBK + c;
     const long long n = GLU ? (static_cast<long long>(col / 64) * 128 + which * 64 + col % 64) : col;
-    *reinterpret_cast<uint4*>(qT + (static_cast<long long>(g) * NT + n) * R + rb * kBM + part * 16) =
-        make_uint4(w4[0], w4[1], w4[2], w4[3]);
-  }
+    return qT + (static_cast<long long>(g) * NT + n) * R + rb * kBM;
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -470,6 +613,19 @@ bool operand_map(CUtensorMap* map, const void* base, long long rows, long long k
 }
 
 bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+// persistent grid: one resident CTA per SM (at most max_ctas if > 0), never more than there are tiles
+unsigned grid_size(long long num_tiles, int max_ctas) {
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+  }
+  long long ctas = sms;
+  if (max_ctas > 0) ctas = std::max<long long>(1, std::min<long long>(ctas, max_ctas));
+  return static_cast<unsigned>(std::min<long long>(num_tiles, ctas));
+}
 
 }  // namespace
 
@@ -520,28 +676,70 @@ cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t str
   a.epi = p.epilogue;
   a.act = p.act;
   a.row_counts = p.row_counts;
+  a.split = 0;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (attr_err == cudaSuccess)
-      attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+      attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
   });
   if (attr_err != cudaSuccess) return attr_err;
   a.num_tiles = static_cast<long long>(a.tiles_m) * a.tiles_n * p.G;
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-  }
-  long long ctas = sms;                                                    // one resident CTA per SM
-  if (p.max_ctas > 0) ctas = std::max<long long>(1, std::min<long long>(ctas, p.max_ctas));
-  const unsigned grid = static_cast<unsigned>(std::min<long long>(a.num_tiles, ctas));
+  const unsigned grid = grid_size(a.num_tiles, p.max_ctas);
   if (p.row_counts != nullptr)
-    block_fp8_gemm_kernel<true><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
+    block_fp8_gemm_kernel<true, false><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
   else
-    block_fp8_gemm_kernel<false><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
+    block_fp8_gemm_kernel<false, false><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
+  return cudaGetLastError();
+}
+
+cudaError_t block_fp8_wgrad_gemm_launch(const BlockFp8WgradProblem& p, cudaStream_t stream, const char** why) {
+  auto fail = [&](const char* msg) { if (why) *why = msg; return cudaErrorInvalidValue; };
+  if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.G <= 0) return fail("empty block fp8 weight-gradient GEMM");
+  if (p.M % kBM != 0 || p.N % kBN != 0 || p.K % kBK != 0)
+    return fail("block fp8 weight-gradient GEMM: M, N and K must be multiples of 128");
+  if (p.split != 0 && (p.split % kBN != 0 || p.N != 2 * p.split || p.d2 == nullptr))
+    return fail("block fp8 weight-gradient GEMM: a split output needs N == 2 * split, split % 128 == 0 and a second output");
+  if (misaligned(p.a) || misaligned(p.b) || misaligned(p.sa) || misaligned(p.sb) || misaligned(p.d) ||
+      (p.split != 0 && misaligned(p.d2)))
+    return fail("block fp8 weight-gradient GEMM: operands, scales and outputs must be 16-byte aligned");
+  CUtensorMap ta, tb_;
+  if (!operand_map(&ta, p.a, p.M, p.K, p.G) || !operand_map(&tb_, p.b, p.N, p.K, p.G))
+    return fail("cuTensorMapEncodeTiled failed for a block fp8 operand");
+  Args a{};
+  a.sa = p.sa;
+  a.sb = p.sb;
+  a.d = static_cast<__nv_bfloat16*>(p.d);
+  a.d2 = static_cast<__nv_bfloat16*>(p.d2);
+  a.split = p.split;
+  a.ldd = p.split != 0 ? p.split : p.N;
+  a.d_group_stride = static_cast<long long>(p.M) * a.ldd;
+  a.M = p.M; a.N = p.N; a.K = p.K; a.G = p.G;
+  a.tiles_m = p.M / kBM;
+  a.tiles_n = p.N / kBN;
+  a.sa_rows = p.M;
+  a.sb_rows = p.N;
+  a.epi = BF8_EPI_NONE;
+  a.num_tiles = static_cast<long long>(a.tiles_m) * a.tiles_n * p.G;
+  static std::once_flag once;
+  static cudaError_t attr_err = cudaSuccess;
+  std::call_once(once, [] {
+    attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgradSmemBytes);
+  });
+  if (attr_err != cudaSuccess) return attr_err;
+  block_fp8_gemm_kernel<false, true><<<grid_size(a.num_tiles, p.max_ctas), kThreads, kWgradSmemBytes, stream>>>(ta, tb_, a);
+  return cudaGetLastError();
+}
+
+cudaError_t block_fp8_quantize_act_dual(const void* x, void* q, float* s, void* qT, float* sT, int groups, int rows, int k,
+                                        cudaStream_t stream) {
+  if (k % kBK != 0 || groups < 0 || rows < 0 || groups > 65535 || (q == nullptr) != (s == nullptr)) return cudaErrorInvalidValue;
+  const int Rp = (rows + kBM - 1) / kBM * kBM;
+  if (groups == 0 || Rp == 0 || k == 0) return cudaSuccess;
+  const dim3 grid(k / kBK, Rp / kBM, groups);
+  block_fp8_quantize_dual_kernel<<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), static_cast<uint8_t*>(q), s,
+                                                          static_cast<uint8_t*>(qT), sT, rows, Rp, k);
   return cudaGetLastError();
 }
 

@@ -61,4 +61,31 @@ struct BlockFp8GemmProblem {
 
 cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t stream, const char** why = nullptr);
 
+// Activations x [G, R, K] bf16 (K % 128 == 0) quantised in both orientations from one read, for the weight gradients:
+//   row-wise    q [G, R, K] + s [G, K / 128, Rp]: bit for bit what block_fp8_quantize_act writes (skipped when q and s
+//               are null);
+//   column-wise qT [G, K, Rp] e4m3 (x^T; rows R..Rp-1 of x are zero bytes) + sT [G, Rp / 128, K] fp32, one scale per
+//               column of x and 128-row block, by the same rule over the block's real rows.
+cudaError_t block_fp8_quantize_act_dual(const void* x, void* q, float* s, void* qT, float* sT, int groups, int rows, int k,
+                                        cudaStream_t stream);
+
+// Weight-gradient GEMM  D[g] = A[g] B[g]^T  with K the (padded) token dimension: A e4m3 [G, M, K], B e4m3 [G, N, K]
+// (the column-wise outputs of block_fp8_quantize_act_dual), one fp32 scale per row and 128-deep K step for both, sa
+// [G, K / 128, M] and sb [G, K / 128, N].  Every K step is promoted as acc = fmaf(part, sa[m] * sb[n], acc).  D is bf16
+// [G, M, N]; with split = H > 0 (N == 2H), columns < H go to d [G, M, H] and columns >= H to d2 [G, M, H].
+// M, N, K multiples of 128.
+struct BlockFp8WgradProblem {
+  int M = 0, N = 0, K = 0, G = 1;
+  const void* a = nullptr;
+  const float* sa = nullptr;
+  const void* b = nullptr;
+  const float* sb = nullptr;
+  void* d = nullptr;
+  void* d2 = nullptr;
+  int split = 0;
+  int max_ctas = 0;              // 0: one CTA per SM
+};
+
+cudaError_t block_fp8_wgrad_gemm_launch(const BlockFp8WgradProblem& p, cudaStream_t stream, const char** why = nullptr);
+
 }  // namespace tb

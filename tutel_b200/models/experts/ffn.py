@@ -28,7 +28,7 @@ class FusedExpertsNetwork(torch.nn.Module):
 
     def __init__(self, model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count, activation_fn=None,
                  activation_fn_with_self=None, output_dim=None, has_fc1_bias=True, has_fc2_bias=True, fp8=None,
-                 weight_format=None):
+                 weight_format=None, fp8_wgrad=False):
         super().__init__()
         if weight_format is not None:
             raise ValueError("ffn experts have no stored weight format (got weight_format=%r): the block-fp8 checkpoints "
@@ -54,6 +54,12 @@ class FusedExpertsNetwork(torch.nn.Module):
         self.fp8 = mode in ('1', 'true', 'row')
         self.mx = mode == 'mx'
         self.block = mode == 'block'
+        # fp8_wgrad=True (with 'block' only): the weight-gradient GEMMs in block-scaled e4m3 too, on 128 x 1 token tiles
+        # of the transposed activations; the backward keeps e4m3 x^T instead of bf16 x.  Outputs, dx and bias gradients
+        # are those of fp8='block' bit for bit.
+        if fp8_wgrad and not self.block:
+            raise ValueError("fp8_wgrad=True needs fp8='block' (or TUTEL_B200_FP8=block); the resolved fp8 mode is %r" % (mode,))
+        self.fp8_wgrad = bool(fp8_wgrad)
 
         if activation_fn_with_self is not None:
             assert activation_fn is None, 'Option `activation_fn_with_self` has been specified, please keep exactly one of them.'
@@ -92,7 +98,7 @@ class FusedExpertsNetwork(torch.nn.Module):
     def extra_repr(self):
         return 'model_dim=%d, hidden_size=%d, output_dim=%d, num_experts_per_device=%d. has_fc1_bias=%s, has_fc2_bias=%s.' % (
             self.batched_fc1_w.size(2), self.batched_fc1_w.size(1), self.batched_fc2_w.size(2), self.batched_fc1_w.size(0),
-            self.batched_fc1_bias is not None, self.batched_fc2_bias is not None)
+            self.batched_fc1_bias is not None, self.batched_fc2_bias is not None) + (' fp8_wgrad=True' if self.fp8_wgrad else '')
 
     # ------------------------------------------------------------------------------------------------------------
     def materialize(self, ctx):
@@ -173,7 +179,7 @@ class FusedExpertsNetwork(torch.nn.Module):
         if self.mx and self._act_kind == 'relu' and row_counts is None and MX.can_use_mx(x, w1, w2):
             y = MX.fused_relu_ffn_mx(x, w1, b1, w2, b2)
         elif self.block and self._act_kind == 'relu' and row_counts is None and BF8.can_use_block_fp8(x, w1, w2):
-            y = BF8.fused_relu_ffn_block_fp8(x, w1, b1, w2, b2)
+            y = BF8.fused_relu_ffn_block_fp8(x, w1, b1, w2, b2, self.fp8_wgrad)
         elif self._act_kind in G.FWD_EPILOGUE and G.can_use_wgmma(x, w1) and G.can_use_wgmma(x, w2):
             if self.fp8 and self._act_kind == 'relu' and x.size(-1) % 16 == 0 and w1.size(1) % 16 == 0:
                 y = G.fused_relu_ffn_fp8(x, w1, b1, w2, b2, row_counts)

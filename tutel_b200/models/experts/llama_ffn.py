@@ -24,11 +24,15 @@ class LlamaFFNNetwork(torch.nn.Module):
     FP8_BLOCK_BUFFERS = ('W_gate_up', 'W_gate_up_scale', 'W_down', 'W_down_scale')
 
     def __init__(self, model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count,
-                 activation_fn=torch.nn.functional.silu, fp8=None, weight_format=None):
+                 activation_fn=torch.nn.functional.silu, fp8=None, weight_format=None, fp8_wgrad=False):
         super().__init__()
         import os
         self.weight_format = weight_format
+        self.fp8_wgrad = bool(fp8_wgrad)
         if weight_format is not None:
+            if fp8_wgrad:
+                raise ValueError("llama_ffn: fp8_wgrad=True is a training option; weight_format='fp8_block' experts have no "
+                                 "weight gradients")
             self._init_fp8_block(model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count,
                                  activation_fn, fp8, weight_format)
             return
@@ -40,6 +44,10 @@ class LlamaFFNNetwork(torch.nn.Module):
             'llama_ffn: fp8 must be a bool, "row" or "block" (got %r); "mx" has no SwiGLU path' % (mode,)
         self.fp8 = mode in ('1', 'true', 'row')
         self.block = mode == 'block'
+        # fp8_wgrad=True (with 'block' only): the weight-gradient GEMMs in block-scaled e4m3 too; see ffn.py
+        if fp8_wgrad and not self.block:
+            raise ValueError("llama_ffn: fp8_wgrad=True needs fp8='block' (or TUTEL_B200_FP8=block); the resolved fp8 mode "
+                             "is %r" % (mode,))
         self.sharded_count = sharded_count
         self.full_shapes = {
             'W_fc1': torch.Size([num_experts_per_device, model_dim, hidden_size_per_expert]),
@@ -171,7 +179,7 @@ class LlamaFFNNetwork(torch.nn.Module):
                 return G.skinny_glu_ffn_fp8(x, w1, w2, w3, row_counts, kind)
             return G.skinny_glu_ffn(x, w1, w2, w3, row_counts, kind)
         if self.block and row_counts is None and kind in BF8.ACT_CODES and BF8.can_use_block_fp8(x, w1, w2, w3):
-            return BF8.fused_glu_ffn_block_fp8(x, w1, w2, w3, kind)
+            return BF8.fused_glu_ffn_block_fp8(x, w1, w2, w3, kind, self.fp8_wgrad)
         if kind in G.ACT_CODES and G.can_use_wgmma(x, w1) and w3.size(-1) % 8 == 0:
             # gate/up GEMMs + activation + multiply in one dual-B wgmma launch; backward without elementwise passes
             return G.fused_glu_ffn(x, w1, w2, w3, kind, self.fp8 and x.size(-1) % 16 == 0 and w3.size(1) % 16 == 0,
@@ -199,7 +207,8 @@ class LlamaFFNNetwork(torch.nn.Module):
         if self.weight_format is not None:
             return "weight_format='fp8_block', %d experts, model_dim=%d, hidden=%d" % (
                 self.W_down.size(0), self.model_dim, self.hidden_size)
-        return 'full shapes: %s, sharded_count=%d' % ({k: tuple(v) for k, v in self.full_shapes.items()}, self.sharded_count)
+        return 'full shapes: %s, sharded_count=%d' % ({k: tuple(v) for k, v in self.full_shapes.items()}, self.sharded_count) + (
+            ', fp8_wgrad=True' if self.fp8_wgrad else '')
 
 
 ExpertModule = LlamaFFNNetwork

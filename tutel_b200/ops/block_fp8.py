@@ -24,6 +24,13 @@ against it, and it documents the format:
                    ``[G, 2H, M]`` (rows ``128 t + j`` = gate column ``64 t + j``, rows ``128 t + 64 + j`` = up column
                    ``64 t + j``) with one scale per 64 rows, ``[G, 2H / 64, M / 128]``, so that one 128-wide N tile holds
                    a gate column and its up partner in the same thread and the GLU epilogue stays in registers.
+* column-wise activations (weight gradients, ``fp8_wgrad``): ``x [G, R, K]`` transposed to ``qT [G, K, Rp]`` e4m3,
+                   ``Rp = roundup(R, 128)``, with one scale per column of ``x`` and 128-row block (128 x 1 tiles), stored
+                   ``sT [G, Rp / 128, K]``; rows ``R..Rp-1`` are zero bytes and take no part in the scale.  One launch
+                   (``quantize_act_dual``) writes it together with the row-wise operand above.
+* weight-gradient GEMM ``D[g] = A[g] B[g]^T`` over the padded token dimension: A ``[G, Ma, Rp]`` and B ``[G, N, Rp]``
+                   are both column-wise operands, so both have one scale per row and 128-deep K step, and each step is
+                   promoted as ``acc = fma(part, sa[m] * sb[n], acc)``.
 
 Every GEMM dimension but the token count must be a multiple of 128; the operands are bf16.
 """
@@ -75,6 +82,21 @@ def quantize_act_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]
     st = torch.zeros(G, KT, Rp, dtype=torch.float32, device=x.device)
     st[:, :, :R] = s.transpose(1, 2)
     return q, st
+
+
+def quantize_act_dual_reference(x: torch.Tensor, rowwise: bool = True):
+    """x [G, R, K] -> (q, s, qT [G, K, Rp], sT [G, Rp / 128, K]); q, s as ``quantize_act_reference`` (None unless
+    ``rowwise``)."""
+    G, R, K = x.shape
+    _check(K % TILE == 0, 'block fp8 activations need K %% 128 == 0 (got %d)' % K)
+    Rp = -(-R // TILE) * TILE
+    xp = torch.zeros(G, Rp, K, dtype=torch.float32, device=x.device)
+    xp[:, :R] = x.float()
+    blocks = xp.view(G, Rp // TILE, TILE, K)
+    sT = block_scale_reference(_nan_abs(blocks).amax(2))                              # [G, Rp / 128, K]
+    qT = _e4m3(blocks * (1.0 / sT).unsqueeze(2)).view(G, Rp, K).transpose(1, 2).contiguous()
+    q, s = quantize_act_reference(x) if rowwise else (None, None)
+    return q, s, qT, sT
 
 
 def quantize_weight_reference(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -161,6 +183,22 @@ def block_fp8_gemm_reference(a, sa, b, sb, bias=None, aux=None, aux2=None, epilo
     return [acc.bfloat16()]
 
 
+def wgrad_gemm_reference(aT, saT, bT, sbT, split: Optional[int] = None):
+    """fp32 emulation of one ``wgrad_gemm`` launch in the kernel's order: a fresh fp32 sum per 128-deep K step, promoted
+    with ``acc = fma(part, sa[m] * sb[n], acc)`` (the scale product rounded to fp32), then one bf16 rounding."""
+    G, M, K = aT.shape
+    N = bT.size(1)
+    acc = torch.zeros(G, M, N, dtype=torch.float32, device=aT.device)
+    af, bf = aT.float(), bT.float()
+    for kb in range(K // TILE):
+        k = slice(kb * TILE, (kb + 1) * TILE)
+        part = af[:, :, k] @ bf[:, :, k].transpose(1, 2)
+        sab = saT[:, kb, :, None] * sbT[:, kb, None, :]                                # fp32 product
+        acc = (part.double() * sab.double() + acc.double()).float()
+    d = acc.bfloat16()
+    return [d] if not split else [d[..., :split].contiguous(), d[..., split:].contiguous()]
+
+
 def _check(ok: bool, msg: str):
     if not ok:
         raise ValueError(msg)
@@ -183,6 +221,27 @@ def quantize_act(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         backend.count_launch()
         return backend.require_ext().block_fp8_quantize_act(x.contiguous())
     return quantize_act_reference(x)
+
+
+def quantize_act_dual(x: torch.Tensor, rowwise: bool = True):
+    """x [G, R, K] bf16 -> (q, s, qT, sT): the row-wise operand of ``quantize_act`` (bit for bit; None, None unless
+    ``rowwise``) and the column-wise operand of the weight-gradient GEMM, from one launch of
+    ``block_fp8_quantize_dual_kernel`` on a GPU."""
+    if _native(x, 'block_fp8.quantize_act_dual'):
+        backend.count_launch()
+        out = backend.require_ext().block_fp8_quantize_act_dual(x.contiguous(), bool(rowwise))
+        return tuple(out) if rowwise else (None, None, out[0], out[1])
+    return quantize_act_dual_reference(x, rowwise)
+
+
+def wgrad_gemm(aT, saT, bT, sbT, split: Optional[int] = None, max_ctas: int = 0):
+    """``aT [G, M, Kp] @ bT [G, N, Kp]^T`` over the padded token dimension, both operands column-wise (scales
+    ``[G, Kp / 128, rows]``) -> ``[d bf16 [G, M, N]]``, or with ``split = H`` (N = 2H) ``[d[..., :H], d[..., H:]]`` as two
+    contiguous tensors written by the one launch."""
+    if _native(aT, 'block_fp8.wgrad_gemm'):
+        backend.count_launch()
+        return backend.require_ext().block_fp8_wgrad_gemm(aT, saT, bT, sbT, int(split or 0), int(max_ctas))
+    return wgrad_gemm_reference(aT, saT, bT, sbT, split)
 
 
 def quantize_weight(w: torch.Tensor):
@@ -268,41 +327,65 @@ def can_use_block_fp8(x: torch.Tensor, *weights: torch.Tensor) -> bool:
 
 class FusedReluFFNBlockFp8(torch.autograd.Function):
     """ReLU expert FFN ``relu(x @ w1^T + b1) @ w2 + b2`` (x [E, C, M], w1 [E, H, M], w2 [E, H, Mo]: the layout of
-    models/experts/ffn.py) with block-scaled e4m3 forward and data-gradient GEMMs and 16-bit weight-gradient GEMMs on the
-    master weights.  Same structure as ``ops.mx.FusedReluFFNMx``."""
+    models/experts/ffn.py) with block-scaled e4m3 forward and data-gradient GEMMs.  The weight-gradient GEMMs are 16-bit on
+    the master weights, or with ``wgrad`` block-scaled e4m3 on column-wise operands: the forward then saves ``x^T`` in
+    e4m3 instead of bf16 ``x``, the backward quantises ``dy`` and ``dh`` in both orientations from one read each and
+    ``act^T`` column-wise only (``act`` stays bf16 for the ReLU-backward epilogue).  Same structure as
+    ``ops.mx.FusedReluFFNMx``."""
 
     @staticmethod
-    def forward(ctx: Any, x, w1, b1, w2, b2):
+    def forward(ctx: Any, x, w1, b1, w2, b2, wgrad: bool = False):
         q1, s1, _, _ = weight(w1)
         _, _, q2t, s2t = weight(w2)                                     # y = act @ W2: W2^T [Mo, H] K-major
-        act = block_fp8_gemm(*quantize_act(x), q1, s1, bias=b1, epilogue=EPI_RELU)[0]
+        if wgrad:
+            xq, xs, xqT, xsT = quantize_act_dual(x)
+        else:
+            xq, xs = quantize_act(x)
+        act = block_fp8_gemm(xq, xs, q1, s1, bias=b1, epilogue=EPI_RELU)[0]
         y = block_fp8_gemm(*quantize_act(act), q2t, s2t, bias=b2)[0]
-        ctx.save_for_backward(x, w1, w2, act)
-        ctx.has_b1, ctx.has_b2 = b1 is not None, b2 is not None
+        ctx.save_for_backward(*((xqT, xsT) if wgrad else (x,)), w1, w2, act)
+        ctx.has_b1, ctx.has_b2, ctx.wgrad = b1 is not None, b2 is not None, wgrad
         return y
 
     @staticmethod
     def backward(ctx: Any, dy: torch.Tensor):
         from . import gemm as _gemm
-        x, w1, w2, act = ctx.saved_tensors
+        if ctx.wgrad:
+            xqT, xsT, w1, w2, act = ctx.saved_tensors
+        else:
+            x, w1, w2, act = ctx.saved_tensors
         dy = dy.contiguous()
         q2, s2, _, _ = weight(w2)                                       # dh = dy @ W2^T: W2 [H, Mo] is K-major for it
-        dh = block_fp8_gemm(*quantize_act(dy), q2, s2, aux=act, epilogue=EPI_RELU_BWD)[0]
-        dw2 = _gemm.raw_gemm(act, dy, a_mn=True, b_mn=True) if ctx.needs_input_grad[3] else None
+        if ctx.wgrad:
+            dq, ds, dqT, dsT = quantize_act_dual(dy)
+        else:
+            dq, ds = quantize_act(dy)
+        dh = block_fp8_gemm(dq, ds, q2, s2, aux=act, epilogue=EPI_RELU_BWD)[0]
+        dw2 = None
+        if ctx.needs_input_grad[3]:                                     # dW2 = act^T dy: [H, C] [C, Mo]
+            dw2 = (wgrad_gemm(*quantize_act_dual(act, rowwise=False)[2:], dqT, dsT)[0] if ctx.wgrad else
+                   _gemm.raw_gemm(act, dy, a_mn=True, b_mn=True))
+        if ctx.wgrad:
+            del dqT, dsT                                                # lower the backward's peak memory
         db2 = _gemm.column_sums(dy) if ctx.has_b2 and ctx.needs_input_grad[4] else None
-        dx = None
+        dx = dw1 = None
+        if ctx.wgrad and (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]):
+            hq, hs, hqT, hsT = quantize_act_dual(dh, rowwise=ctx.needs_input_grad[0])
+        elif ctx.needs_input_grad[0]:
+            hq, hs = quantize_act(dh)
         if ctx.needs_input_grad[0]:
             _, _, q1t, s1t = weight(w1)                                 # dx = dh @ W1: W1^T [M, H] K-major
-            dx = block_fp8_gemm(*quantize_act(dh), q1t, s1t)[0]
-        dw1 = _gemm.raw_gemm(dh, x, a_mn=True, b_mn=True) if ctx.needs_input_grad[1] else None
+            dx = block_fp8_gemm(hq, hs, q1t, s1t)[0]
+        if ctx.needs_input_grad[1]:                                     # dW1 = dh^T x: [H, C] [C, M]
+            dw1 = wgrad_gemm(hqT, hsT, xqT, xsT)[0] if ctx.wgrad else _gemm.raw_gemm(dh, x, a_mn=True, b_mn=True)
         db1 = _gemm.column_sums(dh) if ctx.has_b1 and ctx.needs_input_grad[2] else None
-        return dx, dw1, db1, dw2, db2
+        return dx, dw1, db1, dw2, db2, None
 
 
-def fused_relu_ffn_block_fp8(x, w1, b1, w2, b2):
+def fused_relu_ffn_block_fp8(x, w1, b1, w2, b2, wgrad: bool = False):
     b1 = None if b1 is None else b1.reshape(w1.size(0), -1)
     b2 = None if b2 is None else b2.reshape(w2.size(0), -1)
-    return FusedReluFFNBlockFp8.apply(x, w1, b1, w2, b2)
+    return FusedReluFFNBlockFp8.apply(x, w1, b1, w2, b2, wgrad)
 
 
 class FusedGLUFFNBlockFp8(torch.autograd.Function):
@@ -312,39 +395,68 @@ class FusedGLUFFNBlockFp8(torch.autograd.Function):
     * forward: one GLU launch on the interleaved gate / up copy writes h and the 16-bit g and u; then the down projection;
     * backward: ``dy @ W3^T`` with the GLU-backward epilogue writes ``[dg du]`` side by side into one ``[E, C, 2H]``
       buffer, and ``dx = [dg du] @ [W1 W2]^T`` is one GEMM with K = 2H on the same quantised blocks as the forward;
-      ``dW1``, ``dW2`` and ``dW3`` are 16-bit GEMMs on the master weights."""
+      ``dW1``, ``dW2`` and ``dW3`` are 16-bit GEMMs on the master weights;
+    * with ``wgrad`` the weight gradients are block-scaled e4m3 GEMMs on column-wise operands: the forward quantises x and
+      h in both orientations and saves ``x^T`` and ``h^T`` in e4m3 instead of bf16 ``x`` and ``h``; the backward does
+      the same for dy and ``[dg du]``, and ``[dW1 | dW2] = x^T [dg du]`` is one launch writing both gradients."""
 
     @staticmethod
-    def forward(ctx: Any, x, w1, w2, w3, act: str):
+    def forward(ctx: Any, x, w1, w2, w3, act: str, wgrad: bool = False):
         _, _, qglu, sglu = glu_weight(w1, w2)
         _, _, q3t, s3t = weight(w3)
-        h, g, u = block_fp8_gemm(*quantize_act(x), qglu, sglu, epilogue=EPI_GLU, act=act)
-        y = block_fp8_gemm(*quantize_act(h), q3t, s3t)[0]
-        ctx.act = act
-        ctx.save_for_backward(x, w1, w2, w3, g, u, h)
+        quant = quantize_act_dual if wgrad else quantize_act
+        xs = quant(x)
+        h, g, u = block_fp8_gemm(xs[0], xs[1], qglu, sglu, epilogue=EPI_GLU, act=act)
+        hs = quant(h)
+        y = block_fp8_gemm(hs[0], hs[1], q3t, s3t)[0]
+        ctx.act, ctx.wgrad = act, wgrad
+        if wgrad:
+            ctx.save_for_backward(xs[2], xs[3], w1, w2, w3, g, u, hs[2], hs[3])
+        else:
+            ctx.save_for_backward(x, w1, w2, w3, g, u, h)
         return y
 
     @staticmethod
     def backward(ctx: Any, dy: torch.Tensor):
         from . import gemm as _gemm
-        x, w1, w2, w3, g, u, h = ctx.saved_tensors
+        if ctx.wgrad:
+            xqT, xsT, w1, w2, w3, g, u, hqT, hsT = ctx.saved_tensors
+        else:
+            x, w1, w2, w3, g, u, h = ctx.saved_tensors
         dy = dy.contiguous()
         H = g.size(-1)
         q3, s3, _, _ = weight(w3)                                       # dh = dy @ W3^T: W3 [H, Mo] is K-major for it
-        dgu = block_fp8_gemm(*quantize_act(dy), q3, s3, aux=g, aux2=u, epilogue=EPI_GLU_BWD, act=ctx.act)[0]
+        ds = quantize_act_dual(dy) if ctx.wgrad else quantize_act(dy)
+        dgu = block_fp8_gemm(ds[0], ds[1], q3, s3, aux=g, aux2=u, epilogue=EPI_GLU_BWD, act=ctx.act)[0]
+        dx = dw1 = dw2 = dw3 = None
+        if ctx.wgrad:
+            if ctx.needs_input_grad[3]:                                 # dW3 = h^T dy: [H, C] [C, Mo]
+                dw3 = wgrad_gemm(hqT, hsT, ds[2], ds[3])[0]
+            del ds, hqT, hsT                                            # lower the backward's peak memory
+            need_w12 = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
+            gs = None
+            if ctx.needs_input_grad[0] or need_w12:
+                gs = quantize_act_dual(dgu, rowwise=ctx.needs_input_grad[0])
+            if need_w12:                                                # [dW1 | dW2] = x^T [dg du]: [M, C] [C, 2H]
+                dw1, dw2 = wgrad_gemm(xqT, xsT, gs[2], gs[3], split=H)
+                dw1 = dw1 if ctx.needs_input_grad[1] else None
+                dw2 = dw2 if ctx.needs_input_grad[2] else None
+            if ctx.needs_input_grad[0]:
+                qcat, scat, _, _ = glu_weight(w1, w2)
+                dx = block_fp8_gemm(gs[0], gs[1], qcat, scat)[0]
+            return dx, dw1, dw2, dw3, None, None
         dg, du = dgu[..., :H], dgu[..., H:]
         dw3 = _gemm.raw_gemm(h, dy, a_mn=True, b_mn=True) if ctx.needs_input_grad[3] else None
         dw1 = _gemm.raw_gemm(x, dg, a_mn=True, b_mn=True) if ctx.needs_input_grad[1] else None
         dw2 = _gemm.raw_gemm(x, du, a_mn=True, b_mn=True) if ctx.needs_input_grad[2] else None
-        dx = None
         if ctx.needs_input_grad[0]:
             qcat, scat, _, _ = glu_weight(w1, w2)
             dx = block_fp8_gemm(*quantize_act(dgu), qcat, scat)[0]
-        return dx, dw1, dw2, dw3, None
+        return dx, dw1, dw2, dw3, None, None
 
 
-def fused_glu_ffn_block_fp8(x, w1, w2, w3, act='silu'):
-    return FusedGLUFFNBlockFp8.apply(x, w1, w2, w3, act)
+def fused_glu_ffn_block_fp8(x, w1, w2, w3, act='silu', wgrad: bool = False):
+    return FusedGLUFFNBlockFp8.apply(x, w1, w2, w3, act, wgrad)
 
 
 # ------------------------------------------------------------------------------------------------------------------
