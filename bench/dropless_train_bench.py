@@ -5,6 +5,7 @@ cap capacity_factor=-E, which pads every expert to the fullest one and reads tha
 
     python bench/dropless_train_bench.py                                   # flagship ffn + llama_ffn, fine-grained ffn
     python bench/dropless_train_bench.py --shapes flagship --experts_types llama_ffn --repeats 5
+    python bench/dropless_train_bench.py --fp8 block [--fp8_wgrad]       # block-fp8 experts (fp8_packed=True)
 
 For each shape, expert type and routing (``skewed``: the gate weight favours a few experts; ``balanced``: a random
 gate), the two layouts are timed alternately, ``--repeats`` rounds of ``--steps`` steps each after ``--warmup`` steps,
@@ -36,6 +37,11 @@ ap.add_argument('--routings', default='skewed,balanced')
 ap.add_argument('--steps', type=int, default=5)
 ap.add_argument('--warmup', type=int, default=2)
 ap.add_argument('--repeats', type=int, default=3)
+ap.add_argument('--fp8', default=None, choices=['block'],
+                help="block: experts with fp8='block' and fp8_packed=True (block-scaled e4m3 GEMMs on both layouts)")
+ap.add_argument('--fp8_wgrad', action='store_true', help='with --fp8 block: block-scaled e4m3 weight gradients too')
+ap.add_argument('--profile', default=None, metavar='DIR',
+                help='also write a torch.profiler table of --steps steps of each layout per configuration into DIR')
 args = ap.parse_args()
 
 
@@ -53,6 +59,8 @@ def build(kind, E, k, M, H, routing):
     from tutel_b200 import moe
     torch.manual_seed(0)
     experts = {'type': kind, 'num_experts_per_device': E, 'hidden_size_per_expert': H}
+    if args.fp8 == 'block':
+        experts.update(fp8='block', fp8_packed=True, fp8_wgrad=args.fp8_wgrad)
     if kind == 'ffn':
         experts['activation_fn'] = F.relu
     layer = moe.moe_layer(gate_type={'type': 'top', 'k': k, 'capacity_factor': 0}, model_dim=M, experts=experts,
@@ -78,8 +86,21 @@ def time_steps(layer, opt, x, cf, n):
     return start.elapsed_time(end) / n
 
 
+def profile_steps(layer, opt, x, cf, name):
+    """Device time per kernel over --steps steps (a separate run from the timed rounds: tracing slows the host)."""
+    from torch.profiler import ProfilerActivity, profile
+    os.makedirs(args.profile, exist_ok=True)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time_steps(layer, opt, x, cf, args.steps)
+    with open(os.path.join(args.profile, name + '.txt'), 'w') as f:
+        f.write(prof.key_averages().table(sort_by='cuda_time_total', row_limit=40, max_name_column_width=90))
+
+
 def main():
+    if args.fp8_wgrad and args.fp8 != 'block':
+        raise SystemExit('--fp8_wgrad needs --fp8 block')
     name, power = card()
+    precision = 'bf16' if args.fp8 is None else 'block_fp8' + ('+fp8_wgrad' if args.fp8_wgrad else '')
     for shape in args.shapes.split(','):
         E, k, M, H, S = SHAPES[shape]
         kinds = args.experts_types.split(',') if shape == 'flagship' else ['ffn']
@@ -100,9 +121,12 @@ def main():
                     for m, cf in modes.items():
                         times[m].append(time_steps(layer, opt, x, cf, args.steps))
                 med = {m: sorted(v)[len(v) // 2] for m, v in times.items()}
+                if args.profile:
+                    for m, cf in modes.items():
+                        profile_steps(layer, opt, x, cf, '%s_%s_%s_%s_%s' % (precision, shape, kind, routing, m))
                 print(json.dumps({
                     'shape': shape, 'experts': kind, 'routing': routing, 'E': E, 'top_k': k, 'model_dim': M, 'hidden': H,
-                    'tokens': S, 'dtype': 'bfloat16', 'counts': counts,
+                    'tokens': S, 'dtype': 'bfloat16', 'experts_precision': precision, 'counts': counts,
                     'work_ratio': round(E * max(counts) / max(packed_rows, 1), 3),
                     'packed_step_ms': [round(t, 3) for t in times['packed']],
                     'padded_step_ms': [round(t, 3) for t in times['padded']],

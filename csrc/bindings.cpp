@@ -745,6 +745,23 @@ std::vector<at::Tensor> block_fp8_quantize_act(const at::Tensor& x) {
   return {q, s};
 }
 
+// The same for one group x [1, R, K] bounded by live_rows (device int32 [1], the packed layout's seg_off[E]): rows at or
+// past it are neither read nor written (q and s are left uninitialised there).
+std::vector<at::Tensor> block_fp8_quantize_act_bounded(const at::Tensor& x, const at::Tensor& live_rows) {
+  TORCH_CHECK(x.is_cuda() && x.is_contiguous() && x.dim() == 3 && x.size(0) == 1 && x.scalar_type() == at::kBFloat16 &&
+                  x.size(2) % 128 == 0,
+              "block_fp8_quantize_act: a bounded launch takes a contiguous bf16 CUDA tensor [1, R, K] with K % 128 == 0");
+  TORCH_CHECK(live_rows.is_cuda() && live_rows.scalar_type() == at::kInt && live_rows.numel() == 1 && live_rows.device() == x.device(),
+              "block_fp8_quantize_act: live_rows must be a one-element int32 tensor on x's device");
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int R = static_cast<int>(x.size(1)), K = static_cast<int>(x.size(2));
+  at::Tensor q = at::empty({1, R, K}, x.options().dtype(at::kFloat8_e4m3fn));
+  at::Tensor s = at::empty({1, K / 128, (R + 127) / 128 * 128}, x.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::block_fp8_quantize_act(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), 1, R, K, cur_stream(),
+                                           live_rows.data_ptr<int>()));
+  return {q, s};
+}
+
 // w [G, R, C] bf16 (R, C % 128 == 0) -> [q [G, R, C], s [G, R / 128, C / 128], qT [G, C, R], sT [G, C / 128, R / 128]]
 std::vector<at::Tensor> block_fp8_quantize_weight(const at::Tensor& w) {
   TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.dim() == 3 && w.scalar_type() == at::kBFloat16 && w.size(1) % 128 == 0 &&
@@ -783,32 +800,39 @@ std::vector<at::Tensor> block_fp8_quantize_glu_weight(const at::Tensor& w1, cons
 // epilogue 0 none / 1 ReLU (+ bias [G, N]) -> [d [G, M, N]];  2 ReLU backward (aux = forward activation) -> [d];
 // 3 GLU (b = the interleaved gate / up copy, sb [G, N / 64, K / 128]) -> [h, g, u], each [G, M, N / 2];
 // 4 GLU backward (acc = dh, aux = g, aux2 = u) -> [dgu [G, M, 2N]] with dg in columns [0, N) and du in [N, 2N).
+// Block-mapped (b_group_map, csrc/gemm_block_fp8.h): a is [R, K] with sa [1, K / 128, R], aux / aux2 and the results are
+// [R, *], and G is b's group count.
 std::vector<at::Tensor> block_fp8_gemm_impl(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
                                             const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
                                             const c10::optional<at::Tensor>& aux2, int64_t epilogue, int64_t act, int64_t max_ctas,
-                                            const int* row_counts) {
-  TORCH_CHECK(a.is_cuda() && b.is_cuda() && sa.is_cuda() && sb.is_cuda() && a.dim() == 3 && b.dim() == 3 && sa.dim() == 3 &&
-              sb.dim() == 3, "block_fp8_gemm: 3-D CUDA tensors expected");
+                                            const int* row_counts, const int* b_group_map = nullptr) {
+  const bool mapped = b_group_map != nullptr;
+  TORCH_CHECK(a.is_cuda() && b.is_cuda() && sa.is_cuda() && sb.is_cuda() && a.dim() == (mapped ? 2 : 3) && b.dim() == 3 &&
+              sa.dim() == 3 && sb.dim() == 3, mapped ? "block_fp8_gemm: a [R, K] and 3-D b, sa, sb CUDA tensors expected"
+                                                     : "block_fp8_gemm: 3-D CUDA tensors expected");
   TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && sa.is_contiguous() && sb.is_contiguous(),
               "block_fp8_gemm: contiguous operands expected");
   TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn &&
               sa.scalar_type() == at::kFloat && sb.scalar_type() == at::kFloat, "block_fp8_gemm: e4m3 operands and fp32 scales expected");
-  TORCH_CHECK(a.size(0) == b.size(0) && a.size(2) == b.size(2), "block_fp8_gemm: a [G, M, K] and b [G, N, K] expected");
+  TORCH_CHECK(mapped ? a.size(1) == b.size(2) : (a.size(0) == b.size(0) && a.size(2) == b.size(2)),
+              mapped ? "block_fp8_gemm: a [R, K] and b [G, N, K] expected" : "block_fp8_gemm: a [G, M, K] and b [G, N, K] expected");
   TORCH_CHECK(epilogue >= tb::BF8_EPI_NONE && epilogue <= tb::BF8_EPI_GLU_BWD, "block_fp8_gemm: unknown epilogue");
   const c10::cuda::CUDAGuard guard(a.device());
   tb::BlockFp8GemmProblem p;
-  p.G = static_cast<int>(a.size(0)); p.M = static_cast<int>(a.size(1)); p.K = static_cast<int>(a.size(2));
+  p.G = static_cast<int>(b.size(0)); p.M = static_cast<int>(a.size(-2)); p.K = static_cast<int>(a.size(-1));
   p.N = static_cast<int>(b.size(1));
+  const int64_t ga = mapped ? 1 : p.G;                 // groups of a, sa, aux and the results
   const bool glu = epilogue == tb::BF8_EPI_GLU, glu_bwd = epilogue == tb::BF8_EPI_GLU_BWD;
   const int64_t kb = (p.K + 127) / 128, mp = (p.M + 127) / 128 * 128, nb = glu ? (p.N + 63) / 64 : (p.N + 127) / 128;
-  TORCH_CHECK(sa.size(0) == p.G && sa.size(1) == kb && sa.size(2) == mp && sb.size(0) == p.G && sb.size(1) == nb && sb.size(2) == kb,
+  TORCH_CHECK(sa.size(0) == ga && sa.size(1) == kb && sa.size(2) == mp && sb.size(0) == p.G && sb.size(1) == nb && sb.size(2) == kb,
               glu ? "block_fp8_gemm: scale arrays do not match the operand shapes (sa [G, K / 128, roundup(M, 128)], sb [G, N / 64, K / 128] expected)"
                   : "block_fp8_gemm: scale arrays do not match the operand shapes (sa [G, K / 128, roundup(M, 128)], sb [G, N / 128, K / 128] expected)");
   const auto bf = a.options().dtype(at::kBFloat16);
+  auto shape = [&](int64_t cols) { return mapped ? std::vector<int64_t>{p.M, cols} : std::vector<int64_t>{p.G, p.M, cols}; };
   auto check_mn = [&](const c10::optional<at::Tensor>& t, const char* name) -> const void* {
     if (!t.has_value() || !t->defined()) return nullptr;
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->dim() == 3 && t->size(0) == p.G &&
-                t->size(1) == p.M && t->size(2) == p.N, "block_fp8_gemm: ", name, " must be a contiguous bf16 [G, M, N]");
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->sizes() == at::IntArrayRef(shape(p.N)),
+                "block_fp8_gemm: ", name, mapped ? " must be a contiguous bf16 [R, N]" : " must be a contiguous bf16 [G, M, N]");
     return t->data_ptr();
   };
   p.aux = check_mn(aux, "aux");
@@ -821,15 +845,15 @@ std::vector<at::Tensor> block_fp8_gemm_impl(const at::Tensor& a, const at::Tenso
   }
   std::vector<at::Tensor> out;
   if (glu) {
-    for (int i = 0; i < 3; ++i) out.push_back(at::empty({p.G, p.M, p.N / 2}, bf));
+    for (int i = 0; i < 3; ++i) out.push_back(at::empty(shape(p.N / 2), bf));
     p.d = out[0].data_ptr(); p.d2 = out[1].data_ptr(); p.d3 = out[2].data_ptr();
     p.ldd = p.N / 2;
   } else if (glu_bwd) {
-    out.push_back(at::empty({p.G, p.M, 2LL * p.N}, bf));
+    out.push_back(at::empty(shape(2LL * p.N), bf));
     p.d = out[0].data_ptr(); p.d2 = static_cast<__nv_bfloat16*>(p.d) + p.N;
     p.ldd = 2LL * p.N;
   } else {
-    out.push_back(at::empty({p.G, p.M, p.N}, bf));
+    out.push_back(at::empty(shape(p.N), bf));
     p.d = out[0].data_ptr();
     p.ldd = p.N;
   }
@@ -839,6 +863,7 @@ std::vector<at::Tensor> block_fp8_gemm_impl(const at::Tensor& a, const at::Tenso
   p.act = static_cast<int>(act);
   p.max_ctas = static_cast<int>(max_ctas);
   p.row_counts = row_counts;
+  p.b_group_map = b_group_map;
   const char* why = nullptr;
   cudaError_t e = tb::block_fp8_gemm_launch(p, cur_stream(), &why);
   TORCH_CHECK(e == cudaSuccess, "block_fp8_gemm: ", why ? why : cudaGetErrorString(e));
@@ -863,9 +888,28 @@ std::vector<at::Tensor> block_fp8_gemm_counts(const at::Tensor& a, const at::Ten
   return block_fp8_gemm_impl(a, sa, b, sb, bias, aux, aux2, epilogue, act, max_ctas, row_counts.data_ptr<int>());
 }
 
+// block_fp8_gemm, block-mapped over an expert-packed buffer: a e4m3 [R, K] (R % 128 == 0) + sa [1, K / 128, R], b the
+// [E, N, K] expert operand; row tile m (128 rows) is multiplied by b[b_group_map[m]] (and that expert's sb and bias), and
+// only its first row_counts[m] rows are live (both int32 [R / 128]).  Results and aux are [R, *]; rows past a tile's count
+// are zero, tiles with no live rows are neither loaded nor stored.
+std::vector<at::Tensor> block_fp8_gemm_packed(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                              const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& aux,
+                                              const c10::optional<at::Tensor>& aux2, int64_t epilogue, int64_t act, int64_t max_ctas,
+                                              const at::Tensor& row_counts, const at::Tensor& b_group_map) {
+  TORCH_CHECK(a.dim() == 2 && a.size(0) % 128 == 0, "block_fp8_gemm: a block-mapped a must be [R, K] with R % 128 == 0");
+  for (const at::Tensor* t : {&row_counts, &b_group_map})
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == a.size(0) / 128 &&
+                    t->device() == a.device(),
+                "block_fp8_gemm: row_counts and b_group_map must be contiguous int32 CUDA tensors [R / 128] on a's device");
+  return block_fp8_gemm_impl(a, sa, b, sb, bias, aux, aux2, epilogue, act, max_ctas, row_counts.data_ptr<int>(),
+                             b_group_map.data_ptr<int>());
+}
+
 // x [G, R, K] bf16 (K % 128 == 0), both orientations from one read (csrc/gemm_block_fp8.h) ->
 // rowwise: [q [G, R, K], s [G, K / 128, Rp], qT [G, K, Rp], sT [G, Rp / 128, K]];  otherwise [qT, sT].  Rp = roundup(R, 128).
-std::vector<at::Tensor> block_fp8_quantize_act_dual(const at::Tensor& x, bool rowwise) {
+// live_rows (optional device int32 [1], G == 1, a multiple of 128): the 128-row tiles at or past it are neither read nor
+// written.
+std::vector<at::Tensor> block_fp8_quantize_act_dual_impl(const at::Tensor& x, bool rowwise, const int* live_rows) {
   TORCH_CHECK(x.is_cuda() && x.is_contiguous() && x.dim() == 3 && x.scalar_type() == at::kBFloat16 && x.size(2) % 128 == 0 &&
                   x.size(0) <= 65535,
               "block_fp8_quantize_act_dual: contiguous bf16 CUDA tensor [G, R, K] with K % 128 == 0 and G <= 65535 expected");
@@ -881,16 +925,29 @@ std::vector<at::Tensor> block_fp8_quantize_act_dual(const at::Tensor& x, bool ro
     s = at::empty({G, K / 128, Rp}, f32);
   }
   TB_CHECK_CUDA(tb::block_fp8_quantize_act_dual(x.data_ptr(), rowwise ? q.data_ptr() : nullptr, rowwise ? s.data_ptr<float>() : nullptr,
-                                                qT.data_ptr(), sT.data_ptr<float>(), G, R, K, cur_stream()));
+                                                qT.data_ptr(), sT.data_ptr<float>(), G, R, K, cur_stream(), live_rows));
   if (rowwise) return {q, s, qT, sT};
   return {qT, sT};
+}
+
+std::vector<at::Tensor> block_fp8_quantize_act_dual(const at::Tensor& x, bool rowwise) {
+  return block_fp8_quantize_act_dual_impl(x, rowwise, nullptr);
+}
+
+std::vector<at::Tensor> block_fp8_quantize_act_dual_bounded(const at::Tensor& x, bool rowwise, const at::Tensor& live_rows) {
+  TORCH_CHECK(x.dim() == 3 && x.size(0) == 1, "block_fp8_quantize_act_dual: a bounded launch takes one group [1, R, K]");
+  TORCH_CHECK(live_rows.is_cuda() && live_rows.scalar_type() == at::kInt && live_rows.numel() == 1 && live_rows.device() == x.device(),
+              "block_fp8_quantize_act_dual: live_rows must be a one-element int32 tensor on x's device");
+  return block_fp8_quantize_act_dual_impl(x, rowwise, live_rows.data_ptr<int>());
 }
 
 // Weight-gradient GEMM d[g] = a[g] * b[g]^T over the padded token dimension K: a e4m3 [G, M, K] + sa fp32 [G, K / 128, M],
 // b e4m3 [G, N, K] + sb fp32 [G, K / 128, N] (one scale per row and K step) -> [d bf16 [G, M, N]]; split = H > 0
 // (N == 2H) -> [d1 [G, M, H] (columns < H), d2 [G, M, H] (columns >= H)].
-std::vector<at::Tensor> block_fp8_wgrad_gemm(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
-                                             int64_t split, int64_t max_ctas) {
+// Ragged K (k_offsets int32 [E + 1], multiples of 128): a [1, M, R] and b [1, N, R] are single operands with scales
+// [1, R / 128, M] and [1, R / 128, N], and d[e] reduces over K in [k_offsets[e], k_offsets[e + 1]) -> d [E, M, N] (or split).
+std::vector<at::Tensor> block_fp8_wgrad_gemm_impl(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                                  int64_t split, int64_t max_ctas, const at::Tensor* k_offsets) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && sa.is_cuda() && sb.is_cuda() && a.dim() == 3 && b.dim() == 3 && sa.dim() == 3 &&
               sb.dim() == 3, "block_fp8_wgrad_gemm: 3-D CUDA tensors expected");
   TORCH_CHECK(b.device() == a.device() && sa.device() == a.device() && sb.device() == a.device(),
@@ -901,13 +958,18 @@ std::vector<at::Tensor> block_fp8_wgrad_gemm(const at::Tensor& a, const at::Tens
               sa.scalar_type() == at::kFloat && sb.scalar_type() == at::kFloat,
               "block_fp8_wgrad_gemm: e4m3 operands and fp32 scales expected");
   TORCH_CHECK(a.size(0) == b.size(0) && a.size(2) == b.size(2), "block_fp8_wgrad_gemm: a [G, M, K] and b [G, N, K] expected");
+  if (k_offsets != nullptr)
+    TORCH_CHECK(a.size(0) == 1 && k_offsets->is_cuda() && k_offsets->scalar_type() == at::kInt && k_offsets->is_contiguous() &&
+                    k_offsets->numel() >= 2 && k_offsets->device() == a.device(),
+                "block_fp8_wgrad_gemm: ragged K takes single operands [1, M, R], [1, N, R] and contiguous int32 CUDA k_offsets [E + 1]");
   const c10::cuda::CUDAGuard guard(a.device());
   tb::BlockFp8WgradProblem p;
-  p.G = static_cast<int>(a.size(0)); p.M = static_cast<int>(a.size(1)); p.K = static_cast<int>(a.size(2));
+  p.G = k_offsets != nullptr ? static_cast<int>(k_offsets->numel() - 1) : static_cast<int>(a.size(0));
+  p.M = static_cast<int>(a.size(1)); p.K = static_cast<int>(a.size(2));
   p.N = static_cast<int>(b.size(1));
   TORCH_CHECK(p.M % 128 == 0 && p.N % 128 == 0 && p.K % 128 == 0, "block_fp8_wgrad_gemm: M, N and K must be multiples of 128");
   const int64_t kb = p.K / 128;
-  TORCH_CHECK(sa.size(0) == p.G && sa.size(1) == kb && sa.size(2) == p.M && sb.size(0) == p.G && sb.size(1) == kb && sb.size(2) == p.N,
+  TORCH_CHECK(sa.size(0) == a.size(0) && sa.size(1) == kb && sa.size(2) == p.M && sb.size(0) == a.size(0) && sb.size(1) == kb && sb.size(2) == p.N,
               "block_fp8_wgrad_gemm: scale arrays do not match the operand shapes (sa [G, K / 128, M], sb [G, K / 128, N] expected)");
   TORCH_CHECK(split == 0 || (split % 128 == 0 && 2 * split == p.N),
               "block_fp8_wgrad_gemm: split must be 0 or N / 2, a multiple of 128");
@@ -924,10 +986,22 @@ std::vector<at::Tensor> block_fp8_wgrad_gemm(const at::Tensor& a, const at::Tens
   p.split = static_cast<int>(split);
   p.a = a.data_ptr(); p.sa = sa.data_ptr<float>(); p.b = b.data_ptr(); p.sb = sb.data_ptr<float>();
   p.max_ctas = static_cast<int>(max_ctas);
+  p.k_offsets = k_offsets != nullptr ? k_offsets->data_ptr<int>() : nullptr;
   const char* why = nullptr;
   cudaError_t e = tb::block_fp8_wgrad_gemm_launch(p, cur_stream(), &why);
   TORCH_CHECK(e == cudaSuccess, "block_fp8_wgrad_gemm: ", why ? why : cudaGetErrorString(e));
   return out;
+}
+
+std::vector<at::Tensor> block_fp8_wgrad_gemm(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b, const at::Tensor& sb,
+                                             int64_t split, int64_t max_ctas) {
+  return block_fp8_wgrad_gemm_impl(a, sa, b, sb, split, max_ctas, nullptr);
+}
+
+std::vector<at::Tensor> block_fp8_wgrad_gemm_ragged(const at::Tensor& a, const at::Tensor& sa, const at::Tensor& b,
+                                                    const at::Tensor& sb, int64_t split, int64_t max_ctas,
+                                                    const at::Tensor& k_offsets) {
+  return block_fp8_wgrad_gemm_impl(a, sa, b, sb, split, max_ctas, &k_offsets);
 }
 
 // Gated-linear-unit GEMMs (SwiGLU / GeGLU / ReGLU experts; reference: tutel/experts/llama_ffn.py:38-41 runs three
@@ -1243,12 +1317,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mx_quantize_transpose", &mx_quantize_transpose);
   m.def("mx_gemm", &mx_gemm);
   m.def("block_fp8_quantize_act", &block_fp8_quantize_act);
+  m.def("block_fp8_quantize_act", &block_fp8_quantize_act_bounded);   // + live_rows
   m.def("block_fp8_quantize_weight", &block_fp8_quantize_weight);
   m.def("block_fp8_quantize_glu_weight", &block_fp8_quantize_glu_weight);
   m.def("block_fp8_gemm", &block_fp8_gemm);
   m.def("block_fp8_gemm", &block_fp8_gemm_counts);   // + row_counts
+  m.def("block_fp8_gemm", &block_fp8_gemm_packed);   // + row_counts, b_group_map
   m.def("block_fp8_quantize_act_dual", &block_fp8_quantize_act_dual);
+  m.def("block_fp8_quantize_act_dual", &block_fp8_quantize_act_dual_bounded);   // + live_rows
   m.def("block_fp8_wgrad_gemm", &block_fp8_wgrad_gemm);
+  m.def("block_fp8_wgrad_gemm", &block_fp8_wgrad_gemm_ragged);   // + k_offsets
   m.def("skinny_glu_ffn_block_fp8", &skinny_glu_ffn_block_fp8);
   register_symm_bindings(m);
   register_cpu_bindings(m);

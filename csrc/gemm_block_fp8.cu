@@ -69,8 +69,10 @@ struct Args {
   long long ld_aux, aux_group_stride;
   long long num_tiles;
   int epi, act;
-  const int* row_counts;               // COUNTS: live rows of each group (device); null otherwise
+  const int* row_counts;               // COUNTS: live rows of each group (device); PACKED: of each row tile
   int split;                           // WGRAD: columns >= split go to d2 (at column n - split); 0: all to d
+  const int* b_group_map;              // PACKED forward: B group of each row tile of the packed A (device)
+  const int* k_offsets;                // PACKED WGRAD: K range [k_offsets[g], k_offsets[g + 1]) of group g (device)
 };
 
 // WGRAD: B's per-column scales of each stage, 512 bytes after the barriers
@@ -126,10 +128,25 @@ __device__ __forceinline__ int live_rows(const Args& args, int g) {
   return COUNTS ? max(0, min(args.row_counts[g], args.M)) : args.M;
 }
 
-template <bool COUNTS, bool WGRAD>
+// Ragged K (weight gradients on the expert-packed layout): group g reduces over the 128-deep K steps [kb0, kb0 + steps)
+// of the one packed operand pair.  The producer and the consumers both derive the step count from here.
+__device__ __forceinline__ void k_range(const Args& args, int g, int num_kb, int& kb0, int& steps) {
+  const int lo = min(max(args.k_offsets[g], 0) / kBK, num_kb);
+  const int hi = min(max(args.k_offsets[g + 1], 0) / kBK, num_kb);
+  kb0 = lo;
+  steps = max(hi - lo, 0);
+}
+
+// PACKED selects the expert-packed launch modes (csrc/gemm_block_fp8.h): with COUNTS, the block-mapped forward (A is one
+// [R, K] buffer; row tile m takes B, its scales and bias from group b_group_map[m], row_counts[m] of its rows are live;
+// a tile with none is skipped entirely); with WGRAD, ragged K (A and B are single operands, group g reduces over its
+// K range).
+template <bool COUNTS, bool WGRAD, bool PACKED = false>
 __global__ void __launch_bounds__(kThreads, 1)
 block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Args args) {
   static_assert(!(COUNTS && WGRAD), "row counts are for the forward GEMMs");
+  static_assert(!PACKED || COUNTS || WGRAD, "the block-mapped forward takes per-tile row counts");
+  constexpr bool MAPPED = PACKED && !WGRAD, RAGGED = PACKED && WGRAD;
   using C = Cfg;
   extern __shared__ uint8_t smem_raw[];
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
@@ -170,18 +187,26 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         int g, m_blk, n_blk;
         decode_tile(t, args.tiles_m, args.tiles_n, g, m_blk, n_blk);
         const int m0 = m_blk * kBM, n0 = n_blk * kBN;
-        if (COUNTS && m0 >= live_rows<COUNTS>(args, g)) continue;      // no stage is filled for a tile past the count
-        const float* sa_g = args.sa + static_cast<long long>(g) * num_kb * args.sa_rows + m0;
-        for (int kb = 0; kb < num_kb; ++kb) {
+        if constexpr (MAPPED) {
+          if (args.row_counts[m_blk] <= 0) continue;                    // a tile with no live rows: no stage
+        } else {
+          if (COUNTS && m0 >= live_rows<COUNTS>(args, g)) continue;    // no stage is filled for a tile past the count
+        }
+        const int gb = MAPPED ? args.b_group_map[m_blk] : g;           // B group
+        const int ga = RAGGED ? 0 : g;                                 // operand group of A (and of B, ragged)
+        int kb0 = 0, steps = num_kb;
+        if constexpr (RAGGED) k_range(args, g, num_kb, kb0, steps);
+        const float* sa_g = args.sa + static_cast<long long>(ga) * num_kb * args.sa_rows + m0;
+        for (int kb = kb0; kb < kb0 + steps; ++kb) {
           ptx::mbar_wait_quiet(empty_bar(s), ph ^ 1u);
           if (ptx::elect_one()) {
             const uint32_t fb = full_bar(s);
             ptx::mbar_expect_tx(fb, C::OP_BYTES + (WGRAD ? 2 : 1) * kSaBytes);
-            ptx::tma_load_3d(smem_a(s), &tmA, fb, kb * kBK, m0, g);
-            ptx::tma_load_3d(smem_b(s), &tmB, fb, kb * kBK, n0, g);
+            ptx::tma_load_3d(smem_a(s), &tmA, fb, kb * kBK, m0, ga);
+            ptx::tma_load_3d(smem_b(s), &tmB, fb, kb * kBK, n0, RAGGED ? 0 : gb);
             ptx::bulk_load(smem_sa(s), sa_g + static_cast<long long>(kb) * args.sa_rows, kSaBytes, fb);
             if constexpr (WGRAD)
-              ptx::bulk_load(smem_sb(s), args.sb + (static_cast<long long>(g) * num_kb + kb) * args.N + n0, kSaBytes, fb);
+              ptx::bulk_load(smem_sb(s), args.sb + (static_cast<long long>(ga) * num_kb + kb) * args.N + n0, kSaBytes, fb);
           }
           __syncwarp();
           if (++s == C::STAGES) { s = 0; ph ^= 1u; }
@@ -203,17 +228,27 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     for (long long t = tile_first; t < args.num_tiles; t += tile_step) {
       int g, m_blk, n_blk;
       decode_tile(t, args.tiles_m, args.tiles_n, g, m_blk, n_blk);
+      int gb = g;                                  // B group (B scales, bias)
+      if constexpr (MAPPED) {
+        if (args.row_counts[m_blk] <= 0) continue;  // as in the producer: no stage, and nothing is stored
+        gb = args.b_group_map[m_blk];
+      }
       // B scales of this tile: columns 0..63 and 64..127 (the same row unless the tile holds 64 gate + 64 up columns)
-      const float* sb_lo = args.sb + (static_cast<long long>(g) * args.sb_rows + (glu ? 2 * n_blk : n_blk)) * num_kb;
+      const float* sb_lo = args.sb + (static_cast<long long>(gb) * args.sb_rows + (glu ? 2 * n_blk : n_blk)) * num_kb;
       const float* sb_hi = glu ? sb_lo + num_kb : sb_lo;
       float sbl = 0.f, sbh = 0.f;
       if constexpr (!WGRAD) { sbl = __ldg(sb_lo); sbh = __ldg(sb_hi); }
       float acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      const int live = live_rows<COUNTS>(args, g);
+      // MAPPED: row_counts[m_blk] of this tile's rows are live (absolute bound m_blk * 128 + count)
+      const int live = MAPPED ? m_blk * kBM + min(args.row_counts[m_blk], kBM) : live_rows<COUNTS>(args, g);
       // a tile past the count takes no stage (as in the producer) and stores zeros
-      const int steps = COUNTS && m_blk * kBM >= live ? 0 : num_kb;
+      int steps = COUNTS && m_blk * kBM >= live ? 0 : num_kb;
+      if constexpr (RAGGED) {
+        int kb0;
+        k_range(args, g, num_kb, kb0, steps);     // an empty group runs no step and stores zeros
+      }
       for (int kb = 0; kb < steps; ++kb) {
         ptx::mbar_wait_quiet(full_bar(s), ph);
         const uint32_t a_lo = (((smem_a(s) + static_cast<uint32_t>(wg) * 8192u) >> 4) & 0x3FFFu) | (1u << 16);
@@ -322,7 +357,7 @@ block_fp8_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         const int n0 = n_blk * kBN + c0;
         const long long o = drow + n0;
         const long long ao = aoff + static_cast<long long>(row) * args.ld_aux + n0;
-        const __nv_bfloat16* bias = args.bias == nullptr ? nullptr : args.bias + static_cast<long long>(g) * args.bias_group_stride + n0;
+        const __nv_bfloat16* bias = args.bias == nullptr ? nullptr : args.bias + static_cast<long long>(gb) * args.bias_group_stride + n0;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           float lo = acc[4 * j + 2 * h], hi = acc[4 * j + 2 * h + 1];
@@ -379,11 +414,15 @@ __device__ __forceinline__ void unpack8(const uint4& raw, float* f) {
 // 16 consecutive threads own one 1 x 128 tile (8 elements = one 16-byte load each); tiles are walked K-fastest so a
 // warp reads 512 contiguous bytes.  Pad rows (R <= r < Rp) only write their scale, 0.  The loop runs per warp (two
 // tiles), so that every lane reaches the shuffles.
+// BOUND (G == 1): only rows below *bound are walked; the units past it read and write nothing, and the ones below are
+// exactly those of the unbounded launch.
+template <bool BOUND>
 __global__ void __launch_bounds__(256)
 block_fp8_quantize_act_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q, float* __restrict__ s, int G,
-                              int R, int Rp, int K) {
+                              int R, int Rp, int K, const int* __restrict__ bound) {
   const int KT = K / kBK;
-  const long long units = static_cast<long long>(G) * Rp * KT;
+  long long units = static_cast<long long>(G) * Rp * KT;
+  if constexpr (BOUND) units = min(units, static_cast<long long>(max(0, __ldg(bound))) * KT);
   const int sub = threadIdx.x & 15, half = (threadIdx.x >> 4) & 1;
   const long long warps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
   for (long long wi = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; wi * 2 < units; wi += warps) {
@@ -437,13 +476,18 @@ __device__ __forceinline__ void store_tile_transposed(const uint8_t* tile, int t
 //              the same arithmetic (one half warp per row), so the bytes and scales are that kernel's
 //   column-wise: qT [G, K, Rp] and sT [G, Rp / 128, K], one scale per column and 128-row block; rows past R are not read,
 //              they are zero bytes and take no part in the scale
+// BOUND (G == 1): the tiles of 128 rows that start at or past *bound (a multiple of 128) read and write nothing.
+template <bool BOUND>
 __global__ void __launch_bounds__(256)
 block_fp8_quantize_dual_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q, float* __restrict__ s,
-                               uint8_t* __restrict__ qT, float* __restrict__ sT, int R, int Rp, int K) {
+                               uint8_t* __restrict__ qT, float* __restrict__ sT, int R, int Rp, int K, const int* __restrict__ bound) {
   __shared__ __align__(16) uint8_t tile[kBM * kTilePitch];
   __shared__ float red[8][kBK];
   __shared__ float csc[kBK];
   const int kt = blockIdx.x, rb = blockIdx.y, g = blockIdx.z;
+  if constexpr (BOUND) {
+    if (rb * kBM >= __ldg(bound)) return;              // the whole block: no thread reaches a barrier
+  }
   const int t = threadIdx.x, c8 = (t & 15) * 8;
   const int KT = K / kBK;
   float f[8][8];
@@ -651,10 +695,13 @@ cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t str
   if (p.bias != nullptr && (glu || reads_aux)) return fail("block fp8 GEMM: bias is for the NONE and RELU epilogues");
   if (p.bias != nullptr && (misaligned(p.bias) || p.bias_group_stride % 8)) return fail("block fp8 GEMM: bias must be 16-byte aligned");
 
+  const bool mapped = p.b_group_map != nullptr;
+  if (mapped && (p.row_counts == nullptr || p.M % kBM != 0))
+    return fail("block fp8 GEMM: a block-mapped launch needs per-tile row counts and M (packed rows) % 128 == 0");
   CUtensorMap ta, tb_;
-  if (!operand_map(&ta, p.a, p.M, p.K, p.G) || !operand_map(&tb_, p.b, p.N, p.K, p.G))
+  if (!operand_map(&ta, p.a, p.M, p.K, mapped ? 1 : p.G) || !operand_map(&tb_, p.b, p.N, p.K, p.G))
     return fail("cuTensorMapEncodeTiled failed for a block fp8 operand");
-  Args a;
+  Args a{};
   a.sa = p.sa;
   a.sb = p.sb;
   a.d = static_cast<__nv_bfloat16*>(p.d);
@@ -677,17 +724,23 @@ cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t str
   a.act = p.act;
   a.row_counts = p.row_counts;
   a.split = 0;
+  a.b_group_map = p.b_group_map;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] {
     attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (attr_err == cudaSuccess)
       attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    if (attr_err == cudaSuccess)
+      attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
   });
   if (attr_err != cudaSuccess) return attr_err;
-  a.num_tiles = static_cast<long long>(a.tiles_m) * a.tiles_n * p.G;
+  // block-mapped: one A group of R / 128 row tiles, walked in the same 8-tile bands (neighbouring tiles mostly share B)
+  a.num_tiles = static_cast<long long>(a.tiles_m) * a.tiles_n * (mapped ? 1 : p.G);
   const unsigned grid = grid_size(a.num_tiles, p.max_ctas);
-  if (p.row_counts != nullptr)
+  if (mapped)
+    block_fp8_gemm_kernel<true, false, true><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
+  else if (p.row_counts != nullptr)
     block_fp8_gemm_kernel<true, false><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
   else
     block_fp8_gemm_kernel<false, false><<<grid, kThreads, C::SMEM_BYTES, stream>>>(ta, tb_, a);
@@ -704,12 +757,14 @@ cudaError_t block_fp8_wgrad_gemm_launch(const BlockFp8WgradProblem& p, cudaStrea
   if (misaligned(p.a) || misaligned(p.b) || misaligned(p.sa) || misaligned(p.sb) || misaligned(p.d) ||
       (p.split != 0 && misaligned(p.d2)))
     return fail("block fp8 weight-gradient GEMM: operands, scales and outputs must be 16-byte aligned");
+  const bool ragged = p.k_offsets != nullptr;
   CUtensorMap ta, tb_;
-  if (!operand_map(&ta, p.a, p.M, p.K, p.G) || !operand_map(&tb_, p.b, p.N, p.K, p.G))
+  if (!operand_map(&ta, p.a, p.M, p.K, ragged ? 1 : p.G) || !operand_map(&tb_, p.b, p.N, p.K, ragged ? 1 : p.G))
     return fail("cuTensorMapEncodeTiled failed for a block fp8 operand");
   Args a{};
   a.sa = p.sa;
   a.sb = p.sb;
+  a.k_offsets = p.k_offsets;
   a.d = static_cast<__nv_bfloat16*>(p.d);
   a.d2 = static_cast<__nv_bfloat16*>(p.d2);
   a.split = p.split;
@@ -726,31 +781,48 @@ cudaError_t block_fp8_wgrad_gemm_launch(const BlockFp8WgradProblem& p, cudaStrea
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] {
     attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgradSmemBytes);
+    if (attr_err == cudaSuccess)
+      attr_err = cudaFuncSetAttribute(block_fp8_gemm_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgradSmemBytes);
   });
   if (attr_err != cudaSuccess) return attr_err;
-  block_fp8_gemm_kernel<false, true><<<grid_size(a.num_tiles, p.max_ctas), kThreads, kWgradSmemBytes, stream>>>(ta, tb_, a);
+  const unsigned grid = grid_size(a.num_tiles, p.max_ctas);
+  if (ragged)
+    block_fp8_gemm_kernel<false, true, true><<<grid, kThreads, kWgradSmemBytes, stream>>>(ta, tb_, a);
+  else
+    block_fp8_gemm_kernel<false, true><<<grid, kThreads, kWgradSmemBytes, stream>>>(ta, tb_, a);
   return cudaGetLastError();
 }
 
 cudaError_t block_fp8_quantize_act_dual(const void* x, void* q, float* s, void* qT, float* sT, int groups, int rows, int k,
-                                        cudaStream_t stream) {
+                                        cudaStream_t stream, const int* live_rows) {
   if (k % kBK != 0 || groups < 0 || rows < 0 || groups > 65535 || (q == nullptr) != (s == nullptr)) return cudaErrorInvalidValue;
+  if (live_rows != nullptr && groups > 1) return cudaErrorInvalidValue;
   const int Rp = (rows + kBM - 1) / kBM * kBM;
   if (groups == 0 || Rp == 0 || k == 0) return cudaSuccess;
   const dim3 grid(k / kBK, Rp / kBM, groups);
-  block_fp8_quantize_dual_kernel<<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), static_cast<uint8_t*>(q), s,
-                                                          static_cast<uint8_t*>(qT), sT, rows, Rp, k);
+  const auto* xb = static_cast<const __nv_bfloat16*>(x);
+  if (live_rows != nullptr)
+    block_fp8_quantize_dual_kernel<true><<<grid, 256, 0, stream>>>(xb, static_cast<uint8_t*>(q), s, static_cast<uint8_t*>(qT), sT,
+                                                                  rows, Rp, k, live_rows);
+  else
+    block_fp8_quantize_dual_kernel<false><<<grid, 256, 0, stream>>>(xb, static_cast<uint8_t*>(q), s, static_cast<uint8_t*>(qT), sT,
+                                                                   rows, Rp, k, nullptr);
   return cudaGetLastError();
 }
 
-cudaError_t block_fp8_quantize_act(const void* x, void* q, float* s, int groups, int rows, int k, cudaStream_t stream) {
+cudaError_t block_fp8_quantize_act(const void* x, void* q, float* s, int groups, int rows, int k, cudaStream_t stream,
+                                   const int* live_rows) {
   if (k % kBK != 0 || groups < 0 || rows < 0) return cudaErrorInvalidValue;
+  if (live_rows != nullptr && groups > 1) return cudaErrorInvalidValue;
   const int Rp = (rows + kBM - 1) / kBM * kBM;
   const long long units = static_cast<long long>(groups) * Rp * (k / kBK);
   if (units == 0) return cudaSuccess;
   const int blocks = static_cast<int>(std::min<long long>((units * 16 + 255) / 256, 132LL * 16));
-  block_fp8_quantize_act_kernel<<<blocks, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), static_cast<uint8_t*>(q), s,
-                                                           groups, rows, Rp, k);
+  const auto* xb = static_cast<const __nv_bfloat16*>(x);
+  if (live_rows != nullptr)
+    block_fp8_quantize_act_kernel<true><<<blocks, 256, 0, stream>>>(xb, static_cast<uint8_t*>(q), s, groups, rows, Rp, k, live_rows);
+  else
+    block_fp8_quantize_act_kernel<false><<<blocks, 256, 0, stream>>>(xb, static_cast<uint8_t*>(q), s, groups, rows, Rp, k, nullptr);
   return cudaGetLastError();
 }
 

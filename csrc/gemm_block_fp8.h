@@ -12,7 +12,10 @@ namespace tb {
 //
 // Activations x [G, R, K] bf16 -> q e4m3 [G, R, K] and scales fp32 [G, K / 128, Rp], Rp = roundup(R, 128): MN-major, so
 // that one K step of a 128-row tile is 512 contiguous bytes.  Pad rows get scale 0.  K % 128 == 0.
-cudaError_t block_fp8_quantize_act(const void* x, void* q, float* s, int groups, int rows, int k, cudaStream_t stream);
+// live_rows (optional device int32, groups == 1; the packed layout's seg_off[E]): rows at or past *live_rows are neither
+// read nor written, rows below it are quantised bit for bit as without the bound.
+cudaError_t block_fp8_quantize_act(const void* x, void* q, float* s, int groups, int rows, int k, cudaStream_t stream,
+                                   const int* live_rows = nullptr);
 
 // Weights w [G, R, C] bf16, 128 x 128 blocks (R % 128 == 0, C % 128 == 0), one launch for both orientations:
 //   q [G, R, C] + s [G, R / 128, C / 128]      and      qT [G, C, R] + sT [G, C / 128, R / 128]
@@ -57,6 +60,12 @@ struct BlockFp8GemmProblem {
   // is at or past the count are skipped (no operand is loaded for them); every output row past the count is stored as
   // zero.  Null: all M rows, the same kernel as without the field.
   const int* row_counts = nullptr;
+  // Optional device int32 [M / 128], the block-mapped launch of the expert-packed layout (tutel_b200/ops/packed.py): a is one
+  // e4m3 [M, K] buffer (M = R packed rows, a multiple of 128) with scales [1, K / 128, M], d, d2, d3, aux and aux2 are
+  // [M, *] (group strides unused), and row tile m is multiplied by B, sb and bias of group b_group_map[m] (G = the number
+  // of B groups).  row_counts is then required and holds the live rows of each row tile: rows past it are stored as
+  // zero in every output (whatever the epilogue), and a tile with no live rows loads and stores nothing.
+  const int* b_group_map = nullptr;
 };
 
 cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t stream, const char** why = nullptr);
@@ -66,14 +75,19 @@ cudaError_t block_fp8_gemm_launch(const BlockFp8GemmProblem& p, cudaStream_t str
 //               are null);
 //   column-wise qT [G, K, Rp] e4m3 (x^T; rows R..Rp-1 of x are zero bytes) + sT [G, Rp / 128, K] fp32, one scale per
 //               column of x and 128-row block, by the same rule over the block's real rows.
+// live_rows (optional device int32, groups == 1, a multiple of 128): the 128-row tiles at or past *live_rows are neither read
+// nor written; the others are bit for bit those of the unbounded launch.
 cudaError_t block_fp8_quantize_act_dual(const void* x, void* q, float* s, void* qT, float* sT, int groups, int rows, int k,
-                                        cudaStream_t stream);
+                                        cudaStream_t stream, const int* live_rows = nullptr);
 
 // Weight-gradient GEMM  D[g] = A[g] B[g]^T  with K the (padded) token dimension: A e4m3 [G, M, K], B e4m3 [G, N, K]
 // (the column-wise outputs of block_fp8_quantize_act_dual), one fp32 scale per row and 128-deep K step for both, sa
 // [G, K / 128, M] and sb [G, K / 128, N].  Every K step is promoted as acc = fmaf(part, sa[m] * sb[n], acc).  D is bf16
 // [G, M, N]; with split = H > 0 (N == 2H), columns < H go to d [G, M, H] and columns >= H to d2 [G, M, H].
 // M, N, K multiples of 128.
+// Ragged K (optional device int32 k_offsets [G + 1], multiples of 128; the packed layout's seg_off): a [M, K] and b
+// [N, K] are single operands with scales [1, K / 128, M] and [1, K / 128, N], and group g reduces over the K range
+// [k_offsets[g], k_offsets[g + 1]) only; a group with an empty range gets zeros.
 struct BlockFp8WgradProblem {
   int M = 0, N = 0, K = 0, G = 1;
   const void* a = nullptr;
@@ -84,6 +98,7 @@ struct BlockFp8WgradProblem {
   void* d2 = nullptr;
   int split = 0;
   int max_ctas = 0;              // 0: one CTA per SM
+  const int* k_offsets = nullptr;
 };
 
 cudaError_t block_fp8_wgrad_gemm_launch(const BlockFp8WgradProblem& p, cudaStream_t stream, const char** why = nullptr);

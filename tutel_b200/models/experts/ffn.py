@@ -28,7 +28,7 @@ class FusedExpertsNetwork(torch.nn.Module):
 
     def __init__(self, model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count, activation_fn=None,
                  activation_fn_with_self=None, output_dim=None, has_fc1_bias=True, has_fc2_bias=True, fp8=None,
-                 weight_format=None, fp8_wgrad=False):
+                 weight_format=None, fp8_wgrad=False, fp8_packed=False):
         super().__init__()
         if weight_format is not None:
             raise ValueError("ffn experts have no stored weight format (got weight_format=%r): the block-fp8 checkpoints "
@@ -68,6 +68,20 @@ class FusedExpertsNetwork(torch.nn.Module):
         else:
             self.activation_fn = activation_fn if activation_fn is not None else F.relu
             self._act_kind = G.classify_activation(self.activation_fn)
+        # fp8_packed=True (with 'block' only): dropless training on one GPU runs the block-fp8 experts on the expert-packed
+        # layout (ops/packed.py) instead of the padded one - no host read of the largest count, graph-capturable, and the
+        # e4m3 GEMMs cover sum(roundup128(count)) rows instead of E * max(count).  An option for now: a follow-up may make
+        # it the default for fp8='block' and delete it.
+        if fp8_packed:
+            if not self.block:
+                raise ValueError("fp8_packed=True needs fp8='block' (or TUTEL_B200_FP8=block); the resolved fp8 mode is %r" % (mode,))
+            if self._act_kind != 'relu':
+                raise ValueError("fp8_packed=True: block-fp8 ffn experts run ReLU only; the activation here is %s"
+                                 % (self._act_kind or 'custom',))
+            if any(d % 128 for d in (model_dim, self.hidden_size, self.output_dim)):
+                raise ValueError("fp8_packed=True needs model_dim, hidden_size_per_expert / sharded_count and output_dim "
+                                 "to be multiples of 128 (got %d, %d, %d)" % (model_dim, self.hidden_size, self.output_dim))
+        self.fp8_packed = bool(fp8_packed)
 
         El, Hs = num_experts_per_device, self.hidden_size
         self.batched_fc1_w = torch.nn.Parameter(torch.empty(El, Hs, model_dim))
@@ -98,7 +112,8 @@ class FusedExpertsNetwork(torch.nn.Module):
     def extra_repr(self):
         return 'model_dim=%d, hidden_size=%d, output_dim=%d, num_experts_per_device=%d. has_fc1_bias=%s, has_fc2_bias=%s.' % (
             self.batched_fc1_w.size(2), self.batched_fc1_w.size(1), self.batched_fc2_w.size(2), self.batched_fc1_w.size(0),
-            self.batched_fc1_bias is not None, self.batched_fc2_bias is not None) + (' fp8_wgrad=True' if self.fp8_wgrad else '')
+            self.batched_fc1_bias is not None, self.batched_fc2_bias is not None) + (' fp8_wgrad=True' if self.fp8_wgrad else '') + (
+            ' fp8_packed=True' if self.fp8_packed else '')
 
     # ------------------------------------------------------------------------------------------------------------
     def materialize(self, ctx):
@@ -146,8 +161,12 @@ class FusedExpertsNetwork(torch.nn.Module):
 
     def supports_packed(self, x) -> bool:
         """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit ReLU / GELU / SiLU experts
-        without fp8 / MX / block fp8, on weights of x's dtype."""
+        without fp8 / MX / block fp8, on weights of x's dtype, and with ``fp8_packed`` block-fp8 ReLU experts on bf16."""
         w1 = self.batched_fc1_w
+        if self.block:
+            return (self.fp8_packed and self._act_kind == 'relu' and x.is_cuda and x.dtype == torch.bfloat16 and
+                    w1.dtype == x.dtype and self.sharded_count == 1 and
+                    all(d % 128 == 0 for d in (self.model_dim, self.hidden_size, self.output_dim)))
         return (not self.fp8 and not self.mx and not self.block and self._act_kind in G.FWD_EPILOGUE and x.dtype in (torch.float16, torch.bfloat16)
                 and w1.dtype == x.dtype and x.is_cuda and self.sharded_count == 1 and
                 all(d % 8 == 0 for d in (self.model_dim, self.hidden_size, self.output_dim)))
@@ -157,6 +176,8 @@ class FusedExpertsNetwork(torch.nn.Module):
         if self.skip_expert:
             return x
         w1, b1, w2, b2 = self.materialize(ctx)
+        if self.block:
+            return BF8.fused_relu_ffn_block_fp8(x, w1, b1, w2, b2, self.fp8_wgrad, layout=layout)
         return G.fused_act_ffn(x, w1, b1, w2, b2, None, self._act_kind, layout=layout)
 
     def compute(self, x, w1, b1, w2, b2, row_counts=None):

@@ -24,15 +24,19 @@ class LlamaFFNNetwork(torch.nn.Module):
     FP8_BLOCK_BUFFERS = ('W_gate_up', 'W_gate_up_scale', 'W_down', 'W_down_scale')
 
     def __init__(self, model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count,
-                 activation_fn=torch.nn.functional.silu, fp8=None, weight_format=None, fp8_wgrad=False):
+                 activation_fn=torch.nn.functional.silu, fp8=None, weight_format=None, fp8_wgrad=False, fp8_packed=False):
         super().__init__()
         import os
         self.weight_format = weight_format
         self.fp8_wgrad = bool(fp8_wgrad)
+        self.fp8_packed = bool(fp8_packed)
         if weight_format is not None:
             if fp8_wgrad:
                 raise ValueError("llama_ffn: fp8_wgrad=True is a training option; weight_format='fp8_block' experts have no "
                                  "weight gradients")
+            if fp8_packed:
+                raise ValueError("llama_ffn: fp8_packed=True is a training option (the packed layout runs dropless training "
+                                 "steps); weight_format='fp8_block' experts are inference-only")
             self._init_fp8_block(model_dim, hidden_size_per_expert, num_experts_per_device, sharded_count,
                                  activation_fn, fp8, weight_format)
             return
@@ -48,6 +52,14 @@ class LlamaFFNNetwork(torch.nn.Module):
         if fp8_wgrad and not self.block:
             raise ValueError("llama_ffn: fp8_wgrad=True needs fp8='block' (or TUTEL_B200_FP8=block); the resolved fp8 mode "
                              "is %r" % (mode,))
+        # fp8_packed=True (with 'block' only): dropless training on one GPU on the expert-packed layout; see ffn.py.  A
+        # follow-up may make it the default for fp8='block' and delete the option.
+        if fp8_packed and not self.block:
+            raise ValueError("llama_ffn: fp8_packed=True needs fp8='block' (or TUTEL_B200_FP8=block); the resolved fp8 mode "
+                             "is %r" % (mode,))
+        if fp8_packed and (model_dim % 128 or hidden_size_per_expert % 128):
+            raise ValueError("llama_ffn: fp8_packed=True needs model_dim and hidden_size_per_expert to be multiples of 128 "
+                             "(got %d, %d)" % (model_dim, hidden_size_per_expert))
         self.sharded_count = sharded_count
         self.full_shapes = {
             'W_fc1': torch.Size([num_experts_per_device, model_dim, hidden_size_per_expert]),
@@ -190,10 +202,15 @@ class LlamaFFNNetwork(torch.nn.Module):
         return G.grouped_linear(self.activation_fn(y1) * y2, w3, None, 'kn', fp8=self.fp8)
 
     def supports_packed(self, x) -> bool:
-        """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit experts without fp8 or block fp8."""
+        """The expert-packed layout (MOELayer's dropless path on one GPU) covers 16-bit experts without fp8 or block fp8,
+        and with ``fp8_packed`` block-fp8 experts on bf16."""
         if self.weight_format is not None:
             return False
         M, H = self.full_shapes['W_fc1'][1], self.full_shapes['W_fc1'][2]
+        if self.block:
+            return (self.fp8_packed and x.is_cuda and x.dtype == torch.bfloat16 and self.W_fc1.dtype == x.dtype and
+                    self.sharded_count == 1 and G.classify_activation(self.activation_fn) in BF8.ACT_CODES and
+                    M % 128 == 0 and H % 128 == 0)
         return (not self.fp8 and not self.block and x.dtype in (torch.float16, torch.bfloat16) and self.W_fc1.dtype == x.dtype and x.is_cuda and
                 self.sharded_count == 1 and G.classify_activation(self.activation_fn) in G.ACT_CODES and
                 M % 8 == 0 and H % 8 == 0)
@@ -201,14 +218,17 @@ class LlamaFFNNetwork(torch.nn.Module):
     def forward_packed(self, x, layout, ctx):
         """x [R, M]: an expert-packed buffer (ops/packed.py) -> [R, M] in the same layout."""
         w1, w2, w3 = (self._full(n, ctx.group) for n in ('W_fc1', 'W_fc2', 'W_fc3'))
-        return G.fused_glu_ffn(x, w1, w2, w3, G.classify_activation(self.activation_fn), False, None, layout=layout)
+        kind = G.classify_activation(self.activation_fn)
+        if self.block:
+            return BF8.fused_glu_ffn_block_fp8(x, w1, w2, w3, kind, self.fp8_wgrad, layout=layout)
+        return G.fused_glu_ffn(x, w1, w2, w3, kind, False, None, layout=layout)
 
     def extra_repr(self):
         if self.weight_format is not None:
             return "weight_format='fp8_block', %d experts, model_dim=%d, hidden=%d" % (
                 self.W_down.size(0), self.model_dim, self.hidden_size)
         return 'full shapes: %s, sharded_count=%d' % ({k: tuple(v) for k, v in self.full_shapes.items()}, self.sharded_count) + (
-            ', fp8_wgrad=True' if self.fp8_wgrad else '')
+            ', fp8_wgrad=True' if self.fp8_wgrad else '') + (', fp8_packed=True' if self.fp8_packed else '')
 
 
 ExpertModule = LlamaFFNNetwork

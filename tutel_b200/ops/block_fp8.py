@@ -31,6 +31,12 @@ against it, and it documents the format:
 * weight-gradient GEMM ``D[g] = A[g] B[g]^T`` over the padded token dimension: A ``[G, Ma, Rp]`` and B ``[G, N, Rp]``
                    are both column-wise operands, so both have one scale per row and 128-deep K step, and each step is
                    promoted as ``acc = fma(part, sa[m] * sb[n], acc)``.
+* expert-packed layout (ops/packed.py; dropless training on one GPU): every packed buffer ``[R, K]`` is one group.  The
+                   GEMM runs block-mapped (``b_group_map``: row tile ``m`` takes expert ``block_expert[m]``'s weights,
+                   ``row_counts`` = ``block_rows``), the weight-gradient GEMM with ragged K (``k_offsets`` = ``seg_off``:
+                   expert ``e`` reduces over its own segment) and the quantisers stop at ``live_rows`` = ``seg_off[E]``.
+                   Segments start on 128-row boundaries and padding rows are zero, so every 1 x 128 and 128 x 1 tile an
+                   expert sees is the one it sees in the padded layout.
 
 Every GEMM dimension but the token count must be a multiple of 128; the operands are bf16.
 """
@@ -199,6 +205,77 @@ def wgrad_gemm_reference(aT, saT, bT, sbT, split: Optional[int] = None):
     return [d] if not split else [d[..., :split].contiguous(), d[..., split:].contiguous()]
 
 
+# ------------------------------------------------------------------------------------------------------------------
+# expert-packed launch modes (pure PyTorch): the references above, applied per segment.  What the kernels leave
+# unwritten (rows past ``live_rows``, tiles with no live rows) is zero here.
+# ------------------------------------------------------------------------------------------------------------------
+def _host_int(t: torch.Tensor) -> int:
+    return int(t.reshape(-1)[0])
+
+
+def quantize_act_bounded_reference(x: torch.Tensor, live_rows: torch.Tensor):
+    """x [1, R, K] -> (q, s) of ``quantize_act_reference`` for the rows below ``live_rows``; zero past it."""
+    _, R, K = x.shape
+    n = max(0, min(_host_int(live_rows), R))
+    q = torch.zeros(1, R, K, dtype=torch.float8_e4m3fn, device=x.device)
+    s = torch.zeros(1, K // TILE, -(-R // TILE) * TILE, dtype=torch.float32, device=x.device)
+    qn, sn = quantize_act_reference(x[:, :n])
+    q[:, :n], s[:, :, :sn.size(2)] = qn, sn
+    return q, s
+
+
+def quantize_act_dual_bounded_reference(x: torch.Tensor, live_rows: torch.Tensor, rowwise: bool = True):
+    """x [1, R, K] -> (q, s, qT, sT) of ``quantize_act_dual_reference`` for the 128-row tiles below ``live_rows``;
+    zero past it."""
+    _, R, K = x.shape
+    Rp = -(-R // TILE) * TILE
+    n = max(0, min(_host_int(live_rows), R))
+    _, _, qTn, sTn = quantize_act_dual_reference(x[:, :n], rowwise=False)
+    qT = torch.zeros(1, K, Rp, dtype=torch.float8_e4m3fn, device=x.device)
+    sT = torch.zeros(1, Rp // TILE, K, dtype=torch.float32, device=x.device)
+    qT[:, :, :qTn.size(2)], sT[:, :sTn.size(1)] = qTn, sTn
+    q, s = quantize_act_bounded_reference(x, live_rows) if rowwise else (None, None)
+    return q, s, qT, sT
+
+
+def block_fp8_gemm_packed_reference(a, sa, b, sb, bias=None, aux=None, aux2=None, epilogue=EPI_NONE, act='silu', *,
+                                    row_counts, b_group_map):
+    """One block-mapped ``block_fp8_gemm`` launch: a [R, K] (sa [1, K / 128, R]); the row tiles of expert e are the
+    reference GEMM on expert e's operand, rows at or past a tile's ``row_counts`` are zero.  Results (and aux) are
+    [R, *]."""
+    R = a.size(0)
+    rc, bm = row_counts.cpu().long(), b_group_map.cpu().long()
+    N = b.size(1)
+    widths = [N // 2] * 3 if epilogue == EPI_GLU else [2 * N] if epilogue == EPI_GLU_BWD else [N]
+    outs = [torch.zeros(R, w, dtype=torch.bfloat16, device=a.device) for w in widths]
+    zero = torch.zeros((), dtype=torch.bfloat16, device=a.device)
+    for e in sorted(set(bm[rc > 0].tolist())):
+        tiles = torch.nonzero((bm == e) & (rc > 0)).flatten()
+        rows = (tiles.view(-1, 1) * TILE + torch.arange(TILE)).flatten().to(a.device)
+        side = None if aux is None else aux.reshape(R, -1)[rows].unsqueeze(0)
+        side2 = None if aux2 is None else aux2.reshape(R, -1)[rows].unsqueeze(0)
+        res = block_fp8_gemm_reference(a[rows].unsqueeze(0), sa[:, :, rows], b[e:e + 1], sb[e:e + 1],
+                                       None if bias is None else bias.reshape(b.size(0), -1)[e:e + 1],
+                                       side, side2, epilogue, act)
+        live = (torch.arange(TILE).view(1, -1) < rc[tiles].view(-1, 1)).flatten().to(a.device)
+        for o, t in zip(outs, res):
+            o[rows] = torch.where(live.view(-1, 1), t[0], zero)
+    return outs
+
+
+def wgrad_gemm_ragged_reference(aT, saT, bT, sbT, k_offsets, split: Optional[int] = None):
+    """One ragged-K ``wgrad_gemm`` launch: aT [1, M, R], bT [1, N, R] (scales [1, R / 128, *]); expert e is the
+    reference weight-gradient GEMM over the tokens from k_offsets[e] to k_offsets[e + 1] (zeros if none), [E, M, N]."""
+    ko = [int(v) for v in k_offsets.cpu().tolist()]
+    M, N = aT.size(1), bT.size(1)
+    d = torch.zeros(len(ko) - 1, M, N, dtype=torch.bfloat16, device=aT.device)
+    for e, (k0, k1) in enumerate(zip(ko[:-1], ko[1:])):
+        if k1 > k0:
+            kb = slice(k0 // TILE, k1 // TILE)
+            d[e] = wgrad_gemm_reference(aT[:, :, k0:k1], saT[:, kb], bT[:, :, k0:k1], sbT[:, kb])[0][0]
+    return [d] if not split else [d[..., :split].contiguous(), d[..., split:].contiguous()]
+
+
 def _check(ok: bool, msg: str):
     if not ok:
         raise ValueError(msg)
@@ -215,32 +292,53 @@ def _native(x: torch.Tensor, what: str) -> bool:
     return False
 
 
-def quantize_act(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    """x [G, R, K] bf16 -> (q, s).  One launch of ``block_fp8_quantize_act_kernel`` on a GPU."""
+def quantize_act(x: torch.Tensor, live_rows: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """x [G, R, K] bf16 -> (q, s).  One launch of ``block_fp8_quantize_act_kernel`` on a GPU.
+    ``live_rows`` (one-element device int32, the packed layout's ``used_rows``): x is one packed buffer ([R, K] or
+    [1, R, K]); rows at or past the bound are neither read nor written, and the result is [1, R, K]."""
+    if live_rows is not None:
+        x = x.reshape(1, -1, x.size(-1))
     if _native(x, 'block_fp8.quantize_act'):
         backend.count_launch()
-        return backend.require_ext().block_fp8_quantize_act(x.contiguous())
-    return quantize_act_reference(x)
+        if live_rows is None:
+            return backend.require_ext().block_fp8_quantize_act(x.contiguous())
+        return backend.require_ext().block_fp8_quantize_act(x.contiguous(), live_rows.to(torch.int32))
+    return quantize_act_reference(x) if live_rows is None else quantize_act_bounded_reference(x, live_rows)
 
 
-def quantize_act_dual(x: torch.Tensor, rowwise: bool = True):
+def quantize_act_dual(x: torch.Tensor, rowwise: bool = True, live_rows: Optional[torch.Tensor] = None):
     """x [G, R, K] bf16 -> (q, s, qT, sT): the row-wise operand of ``quantize_act`` (bit for bit; None, None unless
     ``rowwise``) and the column-wise operand of the weight-gradient GEMM, from one launch of
-    ``block_fp8_quantize_dual_kernel`` on a GPU."""
+    ``block_fp8_quantize_dual_kernel`` on a GPU.  ``live_rows``: as for ``quantize_act``, a multiple of 128 (the
+    128-row tiles at or past it are skipped)."""
+    if live_rows is not None:
+        x = x.reshape(1, -1, x.size(-1))
     if _native(x, 'block_fp8.quantize_act_dual'):
         backend.count_launch()
-        out = backend.require_ext().block_fp8_quantize_act_dual(x.contiguous(), bool(rowwise))
+        ext = backend.require_ext()
+        out = (ext.block_fp8_quantize_act_dual(x.contiguous(), bool(rowwise)) if live_rows is None else
+               ext.block_fp8_quantize_act_dual(x.contiguous(), bool(rowwise), live_rows.to(torch.int32)))
         return tuple(out) if rowwise else (None, None, out[0], out[1])
+    if live_rows is not None:
+        return quantize_act_dual_bounded_reference(x, live_rows, rowwise)
     return quantize_act_dual_reference(x, rowwise)
 
 
-def wgrad_gemm(aT, saT, bT, sbT, split: Optional[int] = None, max_ctas: int = 0):
+def wgrad_gemm(aT, saT, bT, sbT, split: Optional[int] = None, max_ctas: int = 0,
+               k_offsets: Optional[torch.Tensor] = None):
     """``aT [G, M, Kp] @ bT [G, N, Kp]^T`` over the padded token dimension, both operands column-wise (scales
     ``[G, Kp / 128, rows]``) -> ``[d bf16 [G, M, N]]``, or with ``split = H`` (N = 2H) ``[d[..., :H], d[..., H:]]`` as two
-    contiguous tensors written by the one launch."""
+    contiguous tensors written by the one launch.
+    ``k_offsets`` (device int32 [E + 1], the packed layout's ``seg_off``): ragged K over single packed operands
+    ``[1, *, R]``; ``d[e]`` reduces over the tokens ``k_offsets[e]`` to ``k_offsets[e + 1]`` (zero if there are none)."""
     if _native(aT, 'block_fp8.wgrad_gemm'):
         backend.count_launch()
-        return backend.require_ext().block_fp8_wgrad_gemm(aT, saT, bT, sbT, int(split or 0), int(max_ctas))
+        if k_offsets is None:
+            return backend.require_ext().block_fp8_wgrad_gemm(aT, saT, bT, sbT, int(split or 0), int(max_ctas))
+        return backend.require_ext().block_fp8_wgrad_gemm(aT, saT, bT, sbT, int(split or 0), int(max_ctas),
+                                                          k_offsets.to(torch.int32).contiguous())
+    if k_offsets is not None:
+        return wgrad_gemm_ragged_reference(aT, saT, bT, sbT, k_offsets, split)
     return wgrad_gemm_reference(aT, saT, bT, sbT, split)
 
 
@@ -267,18 +365,34 @@ def zero_rows_past(t: torch.Tensor, row_counts: torch.Tensor) -> torch.Tensor:
 
 
 def block_fp8_gemm(a, sa, b, sb, bias=None, aux=None, aux2=None, epilogue: int = EPI_NONE, act: str = 'silu',
-                   max_ctas: int = 0, row_counts: Optional[torch.Tensor] = None):
+                   max_ctas: int = 0, row_counts: Optional[torch.Tensor] = None,
+                   b_group_map: Optional[torch.Tensor] = None):
     """``epilogue(a [G, M, K] @ b [G, N, K]^T)`` -> a list of bf16 results (see csrc/bindings.cpp: block_fp8_gemm).
     ``row_counts`` (device int32 [G], optional): rows r >= row_counts[g] of every result are zero, and the kernel skips
-    the tiles that start at or past the count (dropless prefill)."""
+    the tiles that start at or past the count (dropless prefill).
+    ``b_group_map`` (device int32 [R / 128], the packed layout's ``block_expert``, with ``row_counts`` = ``block_rows``):
+    ``a`` is one packed buffer ([R, K] or [1, R, K], scales [1, K / 128, R]) whose row tile m is multiplied by expert
+    ``b_group_map[m]``'s operand, scales and bias; ``aux``, ``aux2`` and the results are [R, *].  Rows of a tile at or
+    past its count are zero; tiles with no live rows are neither read nor written."""
+    if b_group_map is not None:
+        _check(row_counts is not None, "block_fp8_gemm: a block-mapped launch needs the row tiles' row_counts")
+        a = a.reshape(-1, a.size(-1))
+        aux = None if aux is None else aux.reshape(a.size(0), -1)
+        aux2 = None if aux2 is None else aux2.reshape(a.size(0), -1)
     if _native(a, 'block_fp8_gemm'):
         backend.count_launch()
         if bias is not None:
-            bias = bias.reshape(a.size(0), b.size(1)).to(torch.bfloat16).contiguous()
+            bias = bias.reshape(b.size(0), b.size(1)).to(torch.bfloat16).contiguous()
         args = (a, sa, b, sb, bias, aux, aux2, int(epilogue), ACT_CODES[act], int(max_ctas))
         if row_counts is None:
             return backend.require_ext().block_fp8_gemm(*args)
-        return backend.require_ext().block_fp8_gemm(*args, row_counts.to(torch.int32).contiguous())
+        if b_group_map is None:
+            return backend.require_ext().block_fp8_gemm(*args, row_counts.to(torch.int32).contiguous())
+        return backend.require_ext().block_fp8_gemm(*args, row_counts.to(torch.int32).contiguous(),
+                                                    b_group_map.to(torch.int32).contiguous())
+    if b_group_map is not None:
+        return block_fp8_gemm_packed_reference(a, sa, b, sb, bias, aux, aux2, epilogue, act, row_counts=row_counts,
+                                               b_group_map=b_group_map)
     out = block_fp8_gemm_reference(a, sa, b, sb, bias, aux, aux2, epilogue, act)
     return out if row_counts is None else [zero_rows_past(t, row_counts) for t in out]
 
@@ -331,20 +445,26 @@ class FusedReluFFNBlockFp8(torch.autograd.Function):
     the master weights, or with ``wgrad`` block-scaled e4m3 on column-wise operands: the forward then saves ``x^T`` in
     e4m3 instead of bf16 ``x``, the backward quantises ``dy`` and ``dh`` in both orientations from one read each and
     ``act^T`` column-wise only (``act`` stays bf16 for the ReLU-backward epilogue).  Same structure as
-    ``ops.mx.FusedReluFFNMx``."""
+    ``ops.mx.FusedReluFFNMx``.
+
+    ``layout`` (:class:`tutel_b200.ops.packed.PackedLayout`): ``x [R, M]`` is an expert-packed buffer and so is the
+    result.  Every GEMM then runs block-mapped, every quantiser stops at ``used_rows``, the weight gradients reduce over
+    each expert's segment (ragged K: the block GEMM with ``wgrad``, the 16-bit one otherwise) and the bias gradients are
+    segmented column sums.  ``dy``'s padding rows must be zero, as the packed decode's backward leaves them."""
 
     @staticmethod
-    def forward(ctx: Any, x, w1, b1, w2, b2, wgrad: bool = False):
+    def forward(ctx: Any, x, w1, b1, w2, b2, wgrad: bool = False, layout=None):
+        pk, qk = _packed_kwargs(layout)
         q1, s1, _, _ = weight(w1)
         _, _, q2t, s2t = weight(w2)                                     # y = act @ W2: W2^T [Mo, H] K-major
         if wgrad:
-            xq, xs, xqT, xsT = quantize_act_dual(x)
+            xq, xs, xqT, xsT = quantize_act_dual(x, **qk)
         else:
-            xq, xs = quantize_act(x)
-        act = block_fp8_gemm(xq, xs, q1, s1, bias=b1, epilogue=EPI_RELU)[0]
-        y = block_fp8_gemm(*quantize_act(act), q2t, s2t, bias=b2)[0]
+            xq, xs = quantize_act(x, **qk)
+        act = block_fp8_gemm(xq, xs, q1, s1, bias=b1, epilogue=EPI_RELU, **pk)[0]
+        y = block_fp8_gemm(*quantize_act(act, **qk), q2t, s2t, bias=b2, **pk)[0]
         ctx.save_for_backward(*((xqT, xsT) if wgrad else (x,)), w1, w2, act)
-        ctx.has_b1, ctx.has_b2, ctx.wgrad = b1 is not None, b2 is not None, wgrad
+        ctx.has_b1, ctx.has_b2, ctx.wgrad, ctx.layout = b1 is not None, b2 is not None, wgrad, layout
         return y
 
     @staticmethod
@@ -354,38 +474,58 @@ class FusedReluFFNBlockFp8(torch.autograd.Function):
             xqT, xsT, w1, w2, act = ctx.saved_tensors
         else:
             x, w1, w2, act = ctx.saved_tensors
+        layout = ctx.layout
+        pk, qk = _packed_kwargs(layout)
+        wk = {} if layout is None else dict(k_offsets=layout.seg_off)  # weight gradients: one K range per expert
         dy = dy.contiguous()
         q2, s2, _, _ = weight(w2)                                       # dh = dy @ W2^T: W2 [H, Mo] is K-major for it
         if ctx.wgrad:
-            dq, ds, dqT, dsT = quantize_act_dual(dy)
+            dq, ds, dqT, dsT = quantize_act_dual(dy, **qk)
         else:
-            dq, ds = quantize_act(dy)
-        dh = block_fp8_gemm(dq, ds, q2, s2, aux=act, epilogue=EPI_RELU_BWD)[0]
+            dq, ds = quantize_act(dy, **qk)
+        dh = block_fp8_gemm(dq, ds, q2, s2, aux=act, epilogue=EPI_RELU_BWD, **pk)[0]
         dw2 = None
         if ctx.needs_input_grad[3]:                                     # dW2 = act^T dy: [H, C] [C, Mo]
-            dw2 = (wgrad_gemm(*quantize_act_dual(act, rowwise=False)[2:], dqT, dsT)[0] if ctx.wgrad else
-                   _gemm.raw_gemm(act, dy, a_mn=True, b_mn=True))
+            dw2 = (wgrad_gemm(*quantize_act_dual(act, rowwise=False, **qk)[2:], dqT, dsT, **wk)[0] if ctx.wgrad else
+                   _gemm.raw_gemm(act, dy, a_mn=True, b_mn=True, **wk))
         if ctx.wgrad:
             del dqT, dsT                                                # lower the backward's peak memory
-        db2 = _gemm.column_sums(dy) if ctx.has_b2 and ctx.needs_input_grad[4] else None
+        db2 = _column_sums(dy, layout) if ctx.has_b2 and ctx.needs_input_grad[4] else None
         dx = dw1 = None
         if ctx.wgrad and (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]):
-            hq, hs, hqT, hsT = quantize_act_dual(dh, rowwise=ctx.needs_input_grad[0])
+            hq, hs, hqT, hsT = quantize_act_dual(dh, rowwise=ctx.needs_input_grad[0], **qk)
         elif ctx.needs_input_grad[0]:
-            hq, hs = quantize_act(dh)
+            hq, hs = quantize_act(dh, **qk)
         if ctx.needs_input_grad[0]:
             _, _, q1t, s1t = weight(w1)                                 # dx = dh @ W1: W1^T [M, H] K-major
-            dx = block_fp8_gemm(hq, hs, q1t, s1t)[0]
+            dx = block_fp8_gemm(hq, hs, q1t, s1t, **pk)[0]
         if ctx.needs_input_grad[1]:                                     # dW1 = dh^T x: [H, C] [C, M]
-            dw1 = wgrad_gemm(hqT, hsT, xqT, xsT)[0] if ctx.wgrad else _gemm.raw_gemm(dh, x, a_mn=True, b_mn=True)
-        db1 = _gemm.column_sums(dh) if ctx.has_b1 and ctx.needs_input_grad[2] else None
-        return dx, dw1, db1, dw2, db2, None
+            dw1 = (wgrad_gemm(hqT, hsT, xqT, xsT, **wk)[0] if ctx.wgrad else
+                   _gemm.raw_gemm(dh, x, a_mn=True, b_mn=True, **wk))
+        db1 = _column_sums(dh, layout) if ctx.has_b1 and ctx.needs_input_grad[2] else None
+        return dx, dw1, db1, dw2, db2, None, None
 
 
-def fused_relu_ffn_block_fp8(x, w1, b1, w2, b2, wgrad: bool = False):
+def _packed_kwargs(layout):
+    """Keyword arguments of the packed launch modes (block-mapped GEMMs, bounded quantisers), or two empty dicts."""
+    if layout is None:
+        return {}, {}
+    return dict(row_counts=layout.block_rows, b_group_map=layout.block_expert), dict(live_rows=layout.used_rows)
+
+
+def _column_sums(t: torch.Tensor, layout) -> torch.Tensor:
+    """Bias gradient: [G, T, N] -> [G, N] column sums, or per expert segment of a packed [R, N]."""
+    from . import gemm as _gemm
+    if layout is None:
+        return _gemm.column_sums(t)
+    from .packed import segment_colsum
+    return segment_colsum(t, layout)
+
+
+def fused_relu_ffn_block_fp8(x, w1, b1, w2, b2, wgrad: bool = False, layout=None):
     b1 = None if b1 is None else b1.reshape(w1.size(0), -1)
     b2 = None if b2 is None else b2.reshape(w2.size(0), -1)
-    return FusedReluFFNBlockFp8.apply(x, w1, b1, w2, b2, wgrad)
+    return FusedReluFFNBlockFp8.apply(x, w1, b1, w2, b2, wgrad, layout)
 
 
 class FusedGLUFFNBlockFp8(torch.autograd.Function):
@@ -398,18 +538,21 @@ class FusedGLUFFNBlockFp8(torch.autograd.Function):
       ``dW1``, ``dW2`` and ``dW3`` are 16-bit GEMMs on the master weights;
     * with ``wgrad`` the weight gradients are block-scaled e4m3 GEMMs on column-wise operands: the forward quantises x and
       h in both orientations and saves ``x^T`` and ``h^T`` in e4m3 instead of bf16 ``x`` and ``h``; the backward does
-      the same for dy and ``[dg du]``, and ``[dW1 | dW2] = x^T [dg du]`` is one launch writing both gradients."""
+      the same for dy and ``[dg du]``, and ``[dW1 | dW2] = x^T [dg du]`` is one launch writing both gradients;
+    * ``layout`` (a ``PackedLayout``): ``x [R, M]`` and the result are expert-packed buffers, and the launches run in the
+      packed modes, as in :class:`FusedReluFFNBlockFp8`."""
 
     @staticmethod
-    def forward(ctx: Any, x, w1, w2, w3, act: str, wgrad: bool = False):
+    def forward(ctx: Any, x, w1, w2, w3, act: str, wgrad: bool = False, layout=None):
+        pk, qk = _packed_kwargs(layout)
         _, _, qglu, sglu = glu_weight(w1, w2)
         _, _, q3t, s3t = weight(w3)
         quant = quantize_act_dual if wgrad else quantize_act
-        xs = quant(x)
-        h, g, u = block_fp8_gemm(xs[0], xs[1], qglu, sglu, epilogue=EPI_GLU, act=act)
-        hs = quant(h)
-        y = block_fp8_gemm(hs[0], hs[1], q3t, s3t)[0]
-        ctx.act, ctx.wgrad = act, wgrad
+        xs = quant(x, **qk)
+        h, g, u = block_fp8_gemm(xs[0], xs[1], qglu, sglu, epilogue=EPI_GLU, act=act, **pk)
+        hs = quant(h, **qk)
+        y = block_fp8_gemm(hs[0], hs[1], q3t, s3t, **pk)[0]
+        ctx.act, ctx.wgrad, ctx.layout = act, wgrad, layout
         if wgrad:
             ctx.save_for_backward(xs[2], xs[3], w1, w2, w3, g, u, hs[2], hs[3])
         else:
@@ -423,40 +566,43 @@ class FusedGLUFFNBlockFp8(torch.autograd.Function):
             xqT, xsT, w1, w2, w3, g, u, hqT, hsT = ctx.saved_tensors
         else:
             x, w1, w2, w3, g, u, h = ctx.saved_tensors
+        layout = ctx.layout
+        pk, qk = _packed_kwargs(layout)
+        wk = {} if layout is None else dict(k_offsets=layout.seg_off)  # weight gradients: one K range per expert
         dy = dy.contiguous()
         H = g.size(-1)
         q3, s3, _, _ = weight(w3)                                       # dh = dy @ W3^T: W3 [H, Mo] is K-major for it
-        ds = quantize_act_dual(dy) if ctx.wgrad else quantize_act(dy)
-        dgu = block_fp8_gemm(ds[0], ds[1], q3, s3, aux=g, aux2=u, epilogue=EPI_GLU_BWD, act=ctx.act)[0]
+        ds = quantize_act_dual(dy, **qk) if ctx.wgrad else quantize_act(dy, **qk)
+        dgu = block_fp8_gemm(ds[0], ds[1], q3, s3, aux=g, aux2=u, epilogue=EPI_GLU_BWD, act=ctx.act, **pk)[0]
         dx = dw1 = dw2 = dw3 = None
         if ctx.wgrad:
             if ctx.needs_input_grad[3]:                                 # dW3 = h^T dy: [H, C] [C, Mo]
-                dw3 = wgrad_gemm(hqT, hsT, ds[2], ds[3])[0]
+                dw3 = wgrad_gemm(hqT, hsT, ds[2], ds[3], **wk)[0]
             del ds, hqT, hsT                                            # lower the backward's peak memory
             need_w12 = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
             gs = None
             if ctx.needs_input_grad[0] or need_w12:
-                gs = quantize_act_dual(dgu, rowwise=ctx.needs_input_grad[0])
+                gs = quantize_act_dual(dgu, rowwise=ctx.needs_input_grad[0], **qk)
             if need_w12:                                                # [dW1 | dW2] = x^T [dg du]: [M, C] [C, 2H]
-                dw1, dw2 = wgrad_gemm(xqT, xsT, gs[2], gs[3], split=H)
+                dw1, dw2 = wgrad_gemm(xqT, xsT, gs[2], gs[3], split=H, **wk)
                 dw1 = dw1 if ctx.needs_input_grad[1] else None
                 dw2 = dw2 if ctx.needs_input_grad[2] else None
             if ctx.needs_input_grad[0]:
                 qcat, scat, _, _ = glu_weight(w1, w2)
-                dx = block_fp8_gemm(gs[0], gs[1], qcat, scat)[0]
-            return dx, dw1, dw2, dw3, None, None
+                dx = block_fp8_gemm(gs[0], gs[1], qcat, scat, **pk)[0]
+            return dx, dw1, dw2, dw3, None, None, None
         dg, du = dgu[..., :H], dgu[..., H:]
-        dw3 = _gemm.raw_gemm(h, dy, a_mn=True, b_mn=True) if ctx.needs_input_grad[3] else None
-        dw1 = _gemm.raw_gemm(x, dg, a_mn=True, b_mn=True) if ctx.needs_input_grad[1] else None
-        dw2 = _gemm.raw_gemm(x, du, a_mn=True, b_mn=True) if ctx.needs_input_grad[2] else None
+        dw3 = _gemm.raw_gemm(h, dy, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[3] else None
+        dw1 = _gemm.raw_gemm(x, dg, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[1] else None
+        dw2 = _gemm.raw_gemm(x, du, a_mn=True, b_mn=True, **wk) if ctx.needs_input_grad[2] else None
         if ctx.needs_input_grad[0]:
             qcat, scat, _, _ = glu_weight(w1, w2)
-            dx = block_fp8_gemm(*quantize_act(dgu), qcat, scat)[0]
-        return dx, dw1, dw2, dw3, None, None
+            dx = block_fp8_gemm(*quantize_act(dgu, **qk), qcat, scat, **pk)[0]
+        return dx, dw1, dw2, dw3, None, None, None
 
 
-def fused_glu_ffn_block_fp8(x, w1, w2, w3, act='silu', wgrad: bool = False):
-    return FusedGLUFFNBlockFp8.apply(x, w1, w2, w3, act, wgrad)
+def fused_glu_ffn_block_fp8(x, w1, w2, w3, act='silu', wgrad: bool = False, layout=None):
+    return FusedGLUFFNBlockFp8.apply(x, w1, w2, w3, act, wgrad, layout)
 
 
 # ------------------------------------------------------------------------------------------------------------------
