@@ -28,6 +28,11 @@ biases - not the bytes of the 16-bit master parameters.  `rel_err_vs_padded` the
 GEMMs with device row counts.  `active_weight_bytes` counts the e4m3 bytes and their scales.  `expert_memory_bytes` is
 what the expert module holds; with `--fp8_weights`, `bf16_block_expert_memory_bytes` is what the source bf16
 `fp8='block'` layer held after one forward (its parameters and the cached e4m3 copies).
+`--int4_weights` (`llama_ffn`, bfloat16) builds the experts with `weight_format='int4'` (group-32 int4, one bf16 scale
+per 32 input elements, doc/INT4.md), loaded from `export_int4_weights()` of a bf16 layer.  Dropless decoding streams them
+with `skinny_glu_ffn_int4_kernel`; larger steps run the mixed-input GEMM `w4a16_gemm_kernel` with device row counts.
+`active_weight_bytes` counts the nibbles and their scales.  `--shared_int4 0` keeps the shared experts 16-bit
+(`shared_experts={'weight_format': None}`, as Kimi-K2-Thinking ships them); the JSON records `shared_format`.
 `--shared_experts N` adds N shared experts (DeepSeek-V3: 1).
 """
 import argparse
@@ -50,6 +55,9 @@ ap.add_argument('--iters', type=int, default=50)
 ap.add_argument('--fp8', action='store_true', help='fp8 experts (e4m3 weights with per-row scales); 16-bit --dtype only')
 ap.add_argument('--fp8_weights', action='store_true',
                 help="llama_ffn, bfloat16: stored block-fp8 experts (weight_format='fp8_block') with no 16-bit copy")
+ap.add_argument('--int4_weights', action='store_true',
+                help="llama_ffn, bfloat16: group-32 int4 experts (weight_format='int4') exported from a bf16 layer")
+ap.add_argument('--shared_int4', type=int, default=1, help='with --int4_weights: 1 int4 shared experts, 0 16-bit ones')
 ap.add_argument('--shared_experts', type=int, default=0, help='shared experts of the routed type (0: none)')
 ap.add_argument('--graph', action='store_true', help='ours only: replay the forward as one CUDA graph (tutel_b200.utils.graph)')
 args = ap.parse_args()
@@ -57,6 +65,8 @@ hidden = args.hidden or args.dim
 assert not args.fp8 or (args.impl == 'ours' and args.dtype in ('bfloat16', 'float16')), '--fp8: ours, with a 16-bit --dtype'
 assert not args.fp8_weights or (args.impl == 'ours' and args.dtype == 'bfloat16' and args.expert_type == 'llama_ffn' and
                                 not args.fp8), '--fp8_weights: ours, llama_ffn, bfloat16, without --fp8'
+assert not args.int4_weights or (args.impl == 'ours' and args.dtype == 'bfloat16' and args.expert_type == 'llama_ffn' and
+                                 not args.fp8 and not args.fp8_weights), '--int4_weights: ours, llama_ffn, bfloat16, alone'
 if args.impl == 'reference':
     sys.path.insert(0, os.path.join(ROOT, 'baseline', '_ref'))
     from tutel import moe, system
@@ -105,6 +115,20 @@ if args.fp8_weights:
     del src
     BF8._WEIGHT_CACHE.clear()
     torch.cuda.empty_cache()
+elif args.int4_weights:
+    src = build(experts)
+    if args.shared_experts and not args.shared_int4:
+        shared['shared_experts'] = dict(shared['shared_experts'], weight_format=None)
+    layer = build(dict(experts, weight_format='int4'))
+    layer.load_state_dict({k: v for k, v in src.state_dict().items() if not k.startswith(('experts.', 'shared_experts.'))},
+                          strict=False)
+    layer.experts.load_int4_weights(*src.experts.export_int4_weights())
+    if args.shared_experts and args.shared_int4:
+        layer.shared_experts.load_int4_weights(*src.shared_experts.export_int4_weights())
+    elif args.shared_experts:
+        layer.shared_experts.load_state_dict(src.shared_experts.state_dict())
+    del src
+    torch.cuda.empty_cache()
 else:
     layer = build(experts)
 x = torch.randn(1, args.tokens, args.dim, device=dev)
@@ -147,7 +171,7 @@ def expert_bytes():
     """Weight bytes one expert's forward reads: the parameters, or with --fp8 the e4m3 copies (1 byte per weight), one
     fp32 scale per quantised row (ops/gemm.py: fp8_weight) and the 16-bit biases."""
     e = layer.experts
-    if args.fp8_weights:                   # e4m3 W_gate_up [2H, M] + W_down [M, H] and their fp32 block scales
+    if args.fp8_weights or args.int4_weights:   # stored W_gate_up [2H, M] + W_down [M, H] bytes and their scales
         return module_bytes(e) // args.experts
     if not args.fp8:
         return sum(p.numel() * p.element_size() for p in e.parameters()) // args.experts
@@ -164,11 +188,15 @@ config = 'dropless cf=0 top-%d E=%d tokens=%d dim=%d hidden=%d %s %s megablocks_
     args.top_k, args.experts, args.tokens, args.dim, hidden, args.expert_type, args.dtype, args.megablocks_size,
     ' fp8' if args.fp8 else '', ' cuda-graph' if args.graph and args.impl == 'ours' else '')
 config += ' fp8_weights' if args.fp8_weights else ''
+config += ' int4_weights' if args.int4_weights else ''
 config += ' shared=%d' % args.shared_experts if args.shared_experts else ''
+shared_format = None
+if args.shared_experts:
+    shared_format = getattr(layer.shared_experts, 'weight_format', None) or args.dtype
 print(json.dumps({'impl': args.impl, 'config': config, 'median_ms': median, 'min_ms': times[0], 'max_ms': times[-1],
     'experts_median_ms': expert_median, 'active_experts': active, 'active_weight_bytes': active * bytes_per_expert,
     'active_weight_GBps': active * bytes_per_expert / (median * 1e-3) / 1e9,
     'experts_active_weight_GBps': active * bytes_per_expert / (expert_median * 1e-3) / 1e9,
     'rel_err_vs_padded': float((y.float() - padded.float()).norm() / padded.float().norm()),
     'checksum': float(y.float().abs().sum()), 'expert_memory_bytes': module_bytes(layer.experts),
-    'bf16_block_expert_memory_bytes': bf16_block_bytes}))
+    'bf16_block_expert_memory_bytes': bf16_block_bytes, 'shared_format': shared_format}))

@@ -10,6 +10,7 @@
 #include "gemm_block_fp8.h"
 #include "gemm_mx.h"
 #include "gemm_sm90.h"
+#include "gemm_w4a16.h"
 #include "jit_nvrtc.h"
 #include "moe_kernels.h"
 #include "p2p_kernels.h"
@@ -1272,6 +1273,78 @@ at::Tensor skinny_glu_ffn_block_fp8(const at::Tensor& x, const at::Tensor& qglu,
   return y;
 }
 
+bool int4_operand_ok(const at::Tensor& t, const at::Tensor& like, at::ScalarType dt, int64_t d0, int64_t d1, int64_t d2) {
+  return t.is_cuda() && t.device() == like.device() && t.is_contiguous() && t.scalar_type() == dt && t.dim() == 3 &&
+         t.size(0) == d0 && t.size(1) == d1 && t.size(2) == d2;
+}
+
+// x [G, R, M] bf16, qglu [G, 2H, M / 2] uint8 (packed int4, gate / up rows interleaved every 64) + sglu bf16 [G, 2H, M / 32],
+// q3t [G, N, H / 2] uint8 + s3t bf16 [G, N, H / 32], counts int [G] or None -> fp32 [G, R, N], rows past the counts zero
+at::Tensor skinny_glu_ffn_int4(const at::Tensor& x, const at::Tensor& qglu, const at::Tensor& sglu, const at::Tensor& q3t,
+                               const at::Tensor& s3t, const c10::optional<at::Tensor>& counts, int64_t act) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 3 && x.is_contiguous() && x.scalar_type() == at::kBFloat16,
+              "skinny_glu_ffn_int4: x must be a contiguous bf16 CUDA tensor [G, R, M]");
+  const int64_t G = x.size(0), R = x.size(1), M = x.size(2);
+  TORCH_CHECK(qglu.dim() == 3 && q3t.dim() == 3, "skinny_glu_ffn_int4: 3-D weights expected");
+  const int64_t H = qglu.size(1) / 2, N = q3t.size(1);
+  TORCH_CHECK(M % 128 == 0 && H % 128 == 0 && N % 128 == 0, "skinny_glu_ffn_int4: M, H and N must be multiples of 128");
+  TORCH_CHECK(int4_operand_ok(qglu, x, at::kByte, G, 2 * H, M / 2),
+              "skinny_glu_ffn_int4: qglu must be a contiguous uint8 CUDA tensor [G, 2H, M / 2]");
+  TORCH_CHECK(int4_operand_ok(sglu, x, at::kBFloat16, G, 2 * H, M / 32),
+              "skinny_glu_ffn_int4: sglu must be a contiguous bf16 CUDA tensor [G, 2H, M / 32]");
+  TORCH_CHECK(int4_operand_ok(q3t, x, at::kByte, G, N, H / 2),
+              "skinny_glu_ffn_int4: q3t must be a contiguous uint8 CUDA tensor [G, N, H / 2]");
+  TORCH_CHECK(int4_operand_ok(s3t, x, at::kBFloat16, G, N, H / 32),
+              "skinny_glu_ffn_int4: s3t must be a contiguous bf16 CUDA tensor [G, N, H / 32]");
+  TORCH_CHECK(act >= 1 && act <= 3, "skinny_glu_ffn_int4: act must be 1 (relu), 2 (gelu) or 3 (silu)");
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor y = at::zeros({G, R, N}, x.options().dtype(at::kFloat));
+  TB_CHECK_CUDA(tb::skinny_grouped_glu_ffn_int4(x.data_ptr(), qglu.data_ptr(), sglu.data_ptr(), q3t.data_ptr(), s3t.data_ptr(),
+                                                y.data_ptr<float>(), opt_counts(counts, G), static_cast<int>(G),
+                                                static_cast<int>(R), static_cast<int>(M), static_cast<int>(H),
+                                                static_cast<int>(N), static_cast<int>(act), cur_stream()));
+  return y;
+}
+
+// a bf16 [G, M, K], b uint8 [G, N, K / 2] packed int4 + sb bf16 [G, N, K / 32], row_counts int32 [G] or None ->
+// epilogue 0 (none): bf16 [G, M, N];  1 (GLU, b's rows interleaved every 64 gate / up): h = act(gate) * up, bf16 [G, M, N / 2].
+// Rows at or past a group's count are zero.
+at::Tensor w4a16_gemm(const at::Tensor& a, const at::Tensor& b, const at::Tensor& sb, const c10::optional<at::Tensor>& row_counts,
+                      int64_t epilogue, int64_t act) {
+  TORCH_CHECK(a.is_cuda() && a.dim() == 3 && a.is_contiguous() && a.scalar_type() == at::kBFloat16,
+              "w4a16_gemm: a must be a contiguous bf16 CUDA tensor [G, M, K]");
+  const int64_t G = a.size(0), M = a.size(1), K = a.size(2);
+  TORCH_CHECK(b.dim() == 3 && b.size(0) == G && b.size(2) * 2 == K, "w4a16_gemm: b must be uint8 [G, N, K / 2]");
+  const int64_t N = b.size(1);
+  TORCH_CHECK(K % 64 == 0 && N % 128 == 0, "w4a16_gemm: K must be a multiple of 64 and N of 128");
+  TORCH_CHECK(int4_operand_ok(b, a, at::kByte, G, N, K / 2), "w4a16_gemm: b must be a contiguous uint8 CUDA tensor [G, N, K / 2]");
+  TORCH_CHECK(int4_operand_ok(sb, a, at::kBFloat16, G, N, K / 32),
+              "w4a16_gemm: sb must be a contiguous bf16 CUDA tensor [G, N, K / 32]");
+  TORCH_CHECK(epilogue == tb::W4A16_EPI_NONE || epilogue == tb::W4A16_EPI_GLU, "w4a16_gemm: epilogue must be 0 (none) or 1 (glu)");
+  TORCH_CHECK(epilogue != tb::W4A16_EPI_GLU || (act >= 1 && act <= 3), "w4a16_gemm: act must be 1 (relu), 2 (gelu) or 3 (silu)");
+  if (row_counts.has_value() && row_counts->defined())
+    TORCH_CHECK(row_counts->is_cuda() && row_counts->scalar_type() == at::kInt && row_counts->is_contiguous() &&
+                    row_counts->numel() == G && row_counts->device() == a.device(),
+                "w4a16_gemm: row_counts must be a contiguous int32 CUDA tensor [G] on a's device");
+  const c10::cuda::CUDAGuard guard(a.device());
+  const bool glu = epilogue == tb::W4A16_EPI_GLU;
+  at::Tensor d = at::empty({G, M, glu ? N / 2 : N}, a.options());
+  if (G == 0 || M == 0) return d;
+  tb::W4A16GemmProblem p;
+  p.a = a.data_ptr();
+  p.b = b.data_ptr();
+  p.sb = sb.data_ptr();
+  p.d = d.data_ptr();
+  p.G = static_cast<int>(G); p.M = static_cast<int>(M); p.N = static_cast<int>(N); p.K = static_cast<int>(K);
+  p.epilogue = static_cast<int>(epilogue);
+  p.act = static_cast<int>(act);
+  p.row_counts = opt_counts(row_counts, G);
+  const char* why = nullptr;
+  const cudaError_t e = tb::w4a16_gemm_launch(p, cur_stream(), &why);
+  TORCH_CHECK(e == cudaSuccess, "w4a16_gemm: ", why != nullptr ? why : cudaGetErrorString(e));
+  return d;
+}
+
 }  // namespace
 
 void register_symm_bindings(pybind11::module& m);  // symm_heap.cpp / p2p bindings
@@ -1328,6 +1401,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("block_fp8_wgrad_gemm", &block_fp8_wgrad_gemm);
   m.def("block_fp8_wgrad_gemm", &block_fp8_wgrad_gemm_ragged);   // + k_offsets
   m.def("skinny_glu_ffn_block_fp8", &skinny_glu_ffn_block_fp8);
+  m.def("skinny_glu_ffn_int4", &skinny_glu_ffn_int4);
+  m.def("w4a16_gemm", &w4a16_gemm);
   register_symm_bindings(m);
   register_cpu_bindings(m);
   register_jit_bindings(m);

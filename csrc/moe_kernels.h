@@ -174,5 +174,12 @@ cudaError_t skinny_grouped_glu_ffn_fp8(const void* x, const void* q1t, const flo
 cudaError_t skinny_grouped_glu_ffn_block_fp8(const void* x, const void* qglu, const float* sglu, const void* q3t,
                                              const float* s3t, float* y, const int* counts, int G, int rows_cap, int M, int H,
                                              int N, int act, cudaStream_t stream);
+//   skinny_grouped_glu_ffn_int4: the same SwiGLU expert on group-32 int4 weights (W4A16), x bf16:
+//       Qglu [G, 2H, M / 2] packed nibbles (W1^T and W2^T rows interleaved every 64), Sglu bf16 [G, 2H, M / 32];
+//       Q3t [G, N, H / 2], S3t bf16 [G, N, H / 32]; nibble = q + 8, element 2j in bits 0-3 of byte j, 2j + 1 in bits 4-7.
+// cudaErrorInvalidValue for unaligned pointers, M, H or N not a multiple of 128, or act outside 1..3.
+cudaError_t skinny_grouped_glu_ffn_int4(const void* x, const void* qglu, const void* sglu, const void* q3t, const void* s3t,
+                                        float* y, const int* counts, int G, int rows_cap, int M, int H, int N, int act,
+                                        cudaStream_t stream);
 
 }  // namespace tb

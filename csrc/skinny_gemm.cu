@@ -894,6 +894,230 @@ skinny_glu_ffn_block_fp8_kernel(const __nv_bfloat16* __restrict__ x, const uint8
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Group-32 int4 SwiGLU expert (W4A16, the compressed-tensors pack-quantized format), one launch
+// ------------------------------------------------------------------------------------------------
+// Operands are the stored weights of LlamaFFNNetwork(weight_format='int4') (ops/int4.py):
+//   qglu [G, 2H, M / 2] bytes: W1^T and W2^T rows interleaved every 64 (as for fp8_block), byte j of a row holds element
+//        2j in bits 0-3 and 2j + 1 in bits 4-7, each as u = q + 8; sglu [G, 2H, M / 32] bf16, one scale per 32 elements;
+//   q3t  [G, N, H / 2] bytes (the down projection, K = H), s3t [G, N, H / 32] bf16.
+// A 16-byte load of a row is exactly one 32-element group: its word i holds elements 8i .. 8i + 7, element 8i + e in bits
+// 4e .. 4e + 3.  Block (g, s) owns hidden units [128 s, 128 s + 128), two whole interleave groups:
+//   layer 1: one hidden unit per warp and pass; lane c takes groups c, c + 32, ... of the gate row and its up partner.  A
+//            group's 32 products q * x are exact in fp32 (4 + 8 significant bits); their fp32 sum is multiplied by the
+//            group's scale inside one fma into the lane's sum (acc = fma(part, s, acc)), then a 5-step shuffle tree;
+//   layer 2: the block's 128-unit slice of q3t row n is 64 bytes, four groups: lane (sub, c) takes group c of output
+//            sub + 8 i, sums its 32 products h * q, multiplies by the group's scale, and the four lanes of an output are
+//            reduced with two shuffles before one fp32 atomic add.
+// x stays bf16 in shared memory with the four 8-element quarters of group c at uint4 p * M/32 + c (lanes read consecutive
+// 16 bytes): 8 M + 2 KB per block, as for fp8_block.  Every active expert's bytes are read once per kFfnRows rows.
+__device__ __forceinline__ float int4_value(uint32_t w, int e) {
+  return __uint_as_float(0x4B000000u | ((w >> (4 * e)) & 0xFu)) - 8388616.0f;   // (2^23 + u) - (2^23 + 8) = u - 8, exact
+}
+
+__device__ __forceinline__ float bf16_value(uint16_t b) { return __uint_as_float(static_cast<uint32_t>(b) << 16); }
+
+// Rows [0, nr) of x (bf16 [nr, K], K % 32 == 0) into xs [kFfnRows][K]: quarter p of group c of a row at uint4 p * K/32 + c.
+__device__ __forceinline__ void stage_rows_int4(uint4* __restrict__ xs, const __nv_bfloat16* __restrict__ xrow0, int nr, int K) {
+  const int K8 = K >> 3, K32 = K >> 5;
+  __syncthreads();
+  for (int i = threadIdx.x; i < nr * K8; i += 256) {
+    const int r = i / K8, h = i - r * K8;
+    xs[r * K8 + (h & 3) * K32 + (h >> 2)] = __ldg(reinterpret_cast<const uint4*>(xrow0) + i);
+  }
+  if (nr > 2)
+    for (int i = threadIdx.x + nr * K8; i < kFfnRows * K8; i += 256) xs[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+}
+
+// Warp-wide gate and up dot products of ROWS staged rows with one gate row and one up row of K int4 weights whose group
+// scales are sg[K / 32] and su[K / 32]; every lane gets the full sums.
+template <int ROWS>
+__device__ __forceinline__ void int4_glu_dots(const uint4* __restrict__ xs, const uint8_t* __restrict__ qg,
+                                              const uint8_t* __restrict__ qu, const __nv_bfloat16* __restrict__ sg,
+                                              const __nv_bfloat16* __restrict__ su, int K, float (&acc)[2][ROWS]) {
+  const int lane = threadIdx.x & 31;
+  const int K32 = K >> 5, K8 = K >> 3;
+  const uint16_t* sgb = reinterpret_cast<const uint16_t*>(sg);
+  const uint16_t* sub = reinterpret_cast<const uint16_t*>(su);
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) acc[m][r] = 0.0f;
+  for (int c = lane; c < K32; c += 32 * 2) {
+    uint4 raw[2][2];
+    float sc[2][2];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int cc = c + 32 * u;
+      const bool in = cc < K32;
+      raw[u][0] = in ? __ldcs(reinterpret_cast<const uint4*>(qg) + cc) : make_uint4(0, 0, 0, 0);
+      raw[u][1] = in ? __ldcs(reinterpret_cast<const uint4*>(qu) + cc) : make_uint4(0, 0, 0, 0);
+      sc[u][0] = in ? bf16_value(__ldg(sgb + cc)) : 0.0f;
+      sc[u][1] = in ? bf16_value(__ldg(sub + cc)) : 0.0f;
+    }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int cc = c + 32 * u;
+      if (cc < K32) {
+        const uint32_t w[2][4] = {{raw[u][0].x, raw[u][0].y, raw[u][0].z, raw[u][0].w},
+                                  {raw[u][1].x, raw[u][1].y, raw[u][1].z, raw[u][1].w}};
+        float part[2][ROWS];
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+          for (int r = 0; r < ROWS; ++r) part[m][r] = 0.0f;
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          float wv[2][8];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            wv[0][e] = int4_value(w[0][p], e);
+            wv[1][e] = int4_value(w[1][p], e);
+          }
+#pragma unroll
+          for (int r = 0; r < ROWS; ++r) {
+            float xf[8];
+            bf16x8(xs[r * K8 + p * K32 + cc], xf);
+#pragma unroll
+            for (int m = 0; m < 2; ++m)
+#pragma unroll
+              for (int e = 0; e < 8; ++e) part[m][r] = fmaf(xf[e], wv[m][e], part[m][r]);
+          }
+        }
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+          for (int r = 0; r < ROWS; ++r) acc[m][r] = fmaf(part[m][r], sc[u][m], acc[m][r]);
+      }
+    }
+  }
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r)
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc[m][r] += __shfl_xor_sync(0xffffffffu, acc[m][r], o);
+}
+
+// Layer 2: yrow0[r, n] += sum over the slice's four groups of s3[n, group] * sum_{32 units} h[r, j] * q3[n, j], r < nr.
+// hsm holds h [ROWS][kHS8] with unit 32 c + e at index (e >> 2) * 16 + 4 c + (e & 3), so the four lanes of an output
+// read four consecutive float4s.
+template <int ROWS>
+__device__ __forceinline__ void int4_layer2(const float* __restrict__ hsm, const uint8_t* __restrict__ q,
+                                            const __nv_bfloat16* __restrict__ s, float* __restrict__ yrow0, int nr, int H,
+                                            int N) {
+  constexpr int U = 4;                          // loads in flight per lane
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int c = lane & 3, sub = lane >> 2;
+  const uint16_t* sb = reinterpret_cast<const uint16_t*>(s);
+  const long long qld = H >> 1, sld = H >> 5;
+  for (int nb = warp * 8; nb < N; nb += 64 * U) {   // warp-uniform bound: all lanes reach the shuffles
+    uint4 raw[U];
+    float sc[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int n = nb + sub + 64 * u;
+      raw[u] = n < N ? __ldcs(reinterpret_cast<const uint4*>(q + n * qld) + c) : make_uint4(0, 0, 0, 0);
+      sc[u] = n < N ? bf16_value(__ldg(sb + n * sld + c)) : 0.0f;
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const uint32_t w[4] = {raw[u].x, raw[u].y, raw[u].z, raw[u].w};
+      float acc[ROWS];
+#pragma unroll
+      for (int r = 0; r < ROWS; ++r) acc[r] = 0.0f;
+#pragma unroll 1
+      for (int p = 0; p < 4; ++p) {
+        float wv[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) wv[e] = int4_value(w[p], e);
+#pragma unroll
+        for (int r = 0; r < ROWS; ++r) {
+          const float4* hr = reinterpret_cast<const float4*>(hsm + r * kHS8);
+          const float4 h0 = hr[(2 * p) * 4 + c], h1 = hr[(2 * p + 1) * 4 + c];
+          acc[r] = fmaf(h0.x, wv[0], acc[r]);
+          acc[r] = fmaf(h0.y, wv[1], acc[r]);
+          acc[r] = fmaf(h0.z, wv[2], acc[r]);
+          acc[r] = fmaf(h0.w, wv[3], acc[r]);
+          acc[r] = fmaf(h1.x, wv[4], acc[r]);
+          acc[r] = fmaf(h1.y, wv[5], acc[r]);
+          acc[r] = fmaf(h1.z, wv[6], acc[r]);
+          acc[r] = fmaf(h1.w, wv[7], acc[r]);
+        }
+      }
+#pragma unroll
+      for (int r = 0; r < ROWS; ++r) {
+        acc[r] *= sc[u];
+        acc[r] += __shfl_xor_sync(0xffffffffu, acc[r], 1);
+        acc[r] += __shfl_xor_sync(0xffffffffu, acc[r], 2);
+      }
+      const int n = nb + sub + 64 * u;
+      if (c < nr && n < N) {
+        float v = acc[0];
+#pragma unroll
+        for (int r = 1; r < ROWS; ++r) if (c == r) v = acc[r];
+        atomicAdd(yrow0 + static_cast<long long>(c) * N + n, v);
+      }
+    }
+  }
+}
+
+template <int ROWS>
+__device__ __forceinline__ void glu_int4_pass(const uint4* __restrict__ xs, float* __restrict__ hsm,
+                                              const uint8_t* __restrict__ qglu_s, const __nv_bfloat16* __restrict__ sglu_s,
+                                              const uint8_t* __restrict__ q3g, const __nv_bfloat16* __restrict__ s3g,
+                                              float* __restrict__ yrow0, int nr, int M, int H, int N, int act) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long qld = M >> 1, sld = M >> 5;
+  for (int j = warp; j < kHS8; j += 8) {
+    const int t = j >> 6, jj = j & 63;                 // interleave group of the slice, unit inside it
+    const long long row = 128 * t + jj;
+    float acc[2][ROWS];
+    int4_glu_dots<ROWS>(xs, qglu_s + row * qld, qglu_s + (row + 64) * qld, sglu_s + row * sld, sglu_s + (row + 64) * sld,
+                        M, acc);
+    if (lane < ROWS) {
+      float gv = acc[0][0], uv = acc[1][0];
+#pragma unroll
+      for (int r = 1; r < ROWS; ++r)
+        if (lane == r) { gv = acc[0][r]; uv = acc[1][r]; }
+      const int c = j >> 5, e = j & 31;
+      hsm[lane * kHS8 + (e >> 2) * 16 + 4 * c + (e & 3)] = ffn_act(gv, act) * uv;
+    }
+  }
+  __syncthreads();
+  int4_layer2<ROWS>(hsm, q3g, s3g, yrow0, nr, H, N);
+}
+
+__global__ void __launch_bounds__(256, 2)
+skinny_glu_ffn_int4_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict__ qglu,
+                           const __nv_bfloat16* __restrict__ sglu, const uint8_t* __restrict__ q3t,
+                           const __nv_bfloat16* __restrict__ s3t, float* __restrict__ y, const int* __restrict__ counts,
+                           int rows_cap, int M, int H, int N, int act) {
+  extern __shared__ __align__(16) uint4 smb[];   // x rows [kFfnRows][M] bf16, group-split | hidden slice [kFfnRows][kHS8] fp32
+  const int g = blockIdx.y;
+  const int count = counts != nullptr ? min(counts[g], rows_cap) : rows_cap;
+  if (count <= 0) return;
+  const int s = blockIdx.x, h0 = s * kHS8;
+  uint4* xs = smb;
+  float* hsm = reinterpret_cast<float*>(smb + kFfnRows * (M >> 3));
+  const __nv_bfloat16* xg = x + static_cast<long long>(g) * rows_cap * M;
+  const uint8_t* qglu_s = qglu + (static_cast<long long>(g) * 2 * H + 2 * h0) * (M >> 1);
+  const __nv_bfloat16* sglu_s = sglu + (static_cast<long long>(g) * 2 * H + 2 * h0) * (M >> 5);
+  const uint8_t* q3g = q3t + static_cast<long long>(g) * N * (H >> 1) + (h0 >> 1);
+  const __nv_bfloat16* s3g = s3t + static_cast<long long>(g) * N * (H >> 5) + (h0 >> 5);
+  float* yg = y + static_cast<long long>(g) * rows_cap * N;
+
+  for (int r0 = 0; r0 < count; r0 += kFfnRows) {
+    const int nr = min(kFfnRows, count - r0);
+    stage_rows_int4(xs, xg + static_cast<long long>(r0) * M, nr, M);
+    float* yrow0 = yg + static_cast<long long>(r0) * N;
+    if (nr == 1) glu_int4_pass<1>(xs, hsm, qglu_s, sglu_s, q3g, s3g, yrow0, nr, M, H, N, act);
+    else if (nr == 2) glu_int4_pass<2>(xs, hsm, qglu_s, sglu_s, q3g, s3g, yrow0, nr, M, H, N, act);
+    else glu_int4_pass<kFfnRows>(xs, hsm, qglu_s, sglu_s, q3g, s3g, yrow0, nr, M, H, N, act);
+  }
+}
+
 
 // Dynamic shared memory of both fp8 kernels: the staged x rows and the hidden slice (K % 16 == 0 keeps both 16-byte aligned).
 size_t fp8_smem_bytes(int K) { return sizeof(float) * (static_cast<size_t>(kFfnRows) * K + kFfnRows * kHS8); }
@@ -1018,6 +1242,25 @@ cudaError_t skinny_grouped_glu_ffn_block_fp8(const void* x, const void* qglu, co
   dim3 grid(H / kHS8, G);
   kern<<<grid, 256, smem, stream>>>(static_cast<const __nv_bfloat16*>(x), static_cast<const uint8_t*>(qglu), sglu,
                                     static_cast<const uint8_t*>(q3t), s3t, y, counts, rows_cap, M, H, N, act);
+  return cudaGetLastError();
+}
+
+cudaError_t skinny_grouped_glu_ffn_int4(const void* x, const void* qglu, const void* sglu, const void* q3t, const void* s3t,
+                                        float* y, const int* counts, int G, int rows_cap, int M, int H, int N, int act,
+                                        cudaStream_t stream) {
+  if (G <= 0 || rows_cap <= 0 || M <= 0 || H <= 0 || N <= 0) return cudaSuccess;
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(qglu) | reinterpret_cast<uintptr_t>(q3t)) & 15)
+    return cudaErrorInvalidValue;
+  if ((reinterpret_cast<uintptr_t>(sglu) | reinterpret_cast<uintptr_t>(s3t)) & 1) return cudaErrorInvalidValue;
+  if (M % 128 || H % 128 || N % 128 || act < 1 || act > 3) return cudaErrorInvalidValue;
+  const size_t smem = block_fp8_smem_bytes(M);     // the same bf16 x rows and fp32 hidden slice
+  auto* kern = skinny_glu_ffn_int4_kernel;
+  cudaError_t e = fp8_opt_in(kern, smem);
+  if (e != cudaSuccess) return e;
+  dim3 grid(H / kHS8, G);
+  kern<<<grid, 256, smem, stream>>>(static_cast<const __nv_bfloat16*>(x), static_cast<const uint8_t*>(qglu),
+                                    static_cast<const __nv_bfloat16*>(sglu), static_cast<const uint8_t*>(q3t),
+                                    static_cast<const __nv_bfloat16*>(s3t), y, counts, rows_cap, M, H, N, act);
   return cudaGetLastError();
 }
 

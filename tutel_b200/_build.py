@@ -23,7 +23,7 @@ BUILD = os.path.join(ROOT, 'build', 'obj')
 EXT_SUFFIX = sysconfig.get_config_var('EXT_SUFFIX') or '.so'
 TARGET = os.path.join(ROOT, 'tutel_b200', '_C' + EXT_SUFFIX)
 
-CUDA_SOURCES = ['gemm_sm90.cu', 'gemm_mx.cu', 'gemm_block_fp8.cu', 'moe_kernels.cu', 'gate_route.cu', 'p2p_kernels.cu', 'skinny_gemm.cu']
+CUDA_SOURCES = ['gemm_sm90.cu', 'gemm_mx.cu', 'gemm_block_fp8.cu', 'moe_kernels.cu', 'gate_route.cu', 'p2p_kernels.cu', 'skinny_gemm.cu', 'gemm_w4a16.cu']
 CPP_SOURCES = ['bindings.cpp', 'cpu_kernels.cpp', 'symm_heap.cpp', 'jit_nvrtc.cpp']
 
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',

@@ -124,7 +124,10 @@ class MOELayer(torch.nn.Module):
         ``hidden_size_per_expert`` H that are always selected with weight 1 are one dense expert of hidden size nH, of the
         routed experts' type (``ffn`` or ``llama_ffn``) and options, replicated on every rank: ``shared_experts.*``.
         ``'gate': True`` adds ``shared_expert_gate`` (``Linear(model_dim, 1, bias=False)``) and scales the shared output
-        by sigmoid(x . w) per token (Qwen1.5/2-MoE).  The shared term is added inside the combine kernel."""
+        by sigmoid(x . w) per token (Qwen1.5/2-MoE).  The shared term is added inside the combine kernel.
+        ``'weight_format': None | 'fp8_block' | 'int4'`` overrides the routed experts' stored weight format for the
+        shared expert alone (``llama_ffn``), e.g. bf16 shared experts beside int4 routed ones as Kimi-K2-Thinking ships
+        them; without the key the shared expert takes the routed experts' format."""
         super().__init__()
         assert model_dim % 2 == 0, 'Model_dim (%s) must be even value, while this Model_dim mod 2 > 0.' % model_dim
         if 'pad_samples' in kwargs:
@@ -207,6 +210,8 @@ class MOELayer(torch.nn.Module):
         self.shared_experts, self.shared_expert_gate = None, None
         if shared_spec is not None:
             spec = dict(experts, hidden_size_per_expert=experts['hidden_size_per_expert'] * shared_spec['num_experts'])
+            if 'weight_format' in shared_spec:
+                spec['weight_format'] = shared_spec['weight_format']
             self.shared_experts = self._build_experts(spec, num_experts_per_device=1, sharded_count=1)
             if shared_spec.get('gate', False):
                 self.shared_expert_gate = torch.nn.Linear(model_dim, 1, bias=False)
@@ -221,7 +226,7 @@ class MOELayer(torch.nn.Module):
             return None
         if not isinstance(shared_experts, dict):
             raise ValueError("shared_experts must be None or a dict like {'num_experts': 2, 'gate': False}")
-        unknown = set(shared_experts) - {'num_experts', 'gate'}
+        unknown = set(shared_experts) - {'num_experts', 'gate', 'weight_format'}
         if unknown:
             raise ValueError('Unrecognized shared_experts option(s): %s' % sorted(unknown))
         n = shared_experts.get('num_experts')
@@ -234,6 +239,9 @@ class MOELayer(torch.nn.Module):
             raise ValueError("shared_experts need 'ffn' or 'llama_ffn' experts (got %r)" % (kind,))
         if 'hidden_size_per_expert' not in experts:
             raise ValueError('shared_experts need the routed experts\' hidden_size_per_expert')
+        if 'weight_format' in shared_experts and shared_experts['weight_format'] not in (None, 'fp8_block', 'int4'):
+            raise ValueError("shared_experts: weight_format must be None, 'fp8_block' or 'int4' (got %r)"
+                             % (shared_experts['weight_format'],))
         return dict(shared_experts)
 
     def _build_experts(self, experts: dict, num_experts_per_device=None, sharded_count=None):

@@ -451,8 +451,8 @@ def engine_for(layer, x: torch.Tensor, crit, d: int):
             return None
         M, H, Mo = layer.model_dim, ex.hidden_size * (Sh // r if Sh > 1 else 1), ex.output_dim
     elif isinstance(ex, LlamaFFNNetwork):
-        if getattr(ex, 'block', False):
-            return None     # block-fp8 experts (stored ones have no W_fc1) run on the unfused path (ops/block_fp8.py)
+        if getattr(ex, 'block', False) or getattr(ex, 'weight_format', None) is not None:
+            return None     # block-fp8 and stored experts (no W_fc1) run on the unfused path (ops/block_fp8.py, ops/int4.py)
         if G.classify_activation(ex.activation_fn) not in G.ACT_CODES or ex.W_fc1.dtype != x.dtype:
             return None
         align = 16 if ex.fp8 else 8
